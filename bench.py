@@ -1,13 +1,15 @@
 #!/usr/bin/env python
 """Benchmark of the denoising-loop hot path (BASELINE.json): images/sec for SD-v1 512x512, 50-step PLMS, CFG 7.5.
 
-  python bench.py --gpus N --steps K --warmup W            # B200 engine (torchrun launches one rank per GPU)
+  python bench.py --gpus N --steps K --warmup W            # H100 engine (torchrun launches one rank per GPU)
   python bench.py --impl reference --steps K --warmup W    # CPU baseline arm (oracle port of the reference, host cores)
 
 A "step" is one pass of the hot path over one batch: CLIP text encode of [uncond; prompts] -> 51 guided UNet
 evaluations (PLMS-50) -> AutoencoderKL decode -> uint8 images. Weights are seeded random-init of the SD-v1
 architecture (no checkpoint offline), data is synthetic (seeded token ids and start noise).
-Prints ONE JSON line (rank 0).
+Prints ONE JSON line (rank 0). --dump-outputs DIR also writes the images of the last timed step (rank 0) as
+DIR/images.npy (float32, [B, 512, 512, 3], values 0..255): with the same arguments the inputs are identical from run
+to run, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -30,39 +32,14 @@ VAE_DEC_GF = 2514.5             # per image @ 512x512
 CLIP_GF_PER_PROMPT = 13.0
 
 
-def gemm_dram_traffic():
-    """DRAM bytes per gemm_tc launch from the committed ncu capture of one UNet evaluation (dram__bytes_read.sum +
-    dram__bytes_write.sum per launch, `ncu --metrics ... -k regex:gemm_tc python scripts/profile_unet.py`): newest round
-    first. Returns (bytes per launch or None, source file, launches in the capture)."""
-    import csv
-    for name in ("r02_gemm_dram.csv", "r01_gemm_dram.csv"):
-        path = os.path.join(ROOT, "profiles", name)
-        if not os.path.exists(path):
-            continue
-        try:
-            rows = [r for r in csv.reader(l for l in open(path) if l.startswith('"'))]
-            hdr = rows[0]
-            i_id, i_name, i_unit, i_val = hdr.index("ID"), hdr.index("Metric Name"), hdr.index("Metric Unit"), hdr.index("Metric Value")
-            scale = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-            tot, ids = 0.0, set()
-            for r in rows[1:]:
-                if r[i_name].startswith("dram__bytes_"):
-                    tot += float(r[i_val].replace(",", "")) * scale.get(r[i_unit], 1.0)
-                    ids.add(r[i_id])
-            if ids:
-                return tot / len(ids), "profiles/" + name, len(ids)
-        except Exception:
-            continue
-    return None, None, 0
-
-
 def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(tensor_burst=d["bf16_tflops"], tensor_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     hbm=d["hbm_gbs"], source="measured (MEASURED_PEAKS.json)")
-    return dict(tensor_burst=1590.0, tensor_sustained=1400.0, hbm=6650.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet: dense FP16 / BF16 tensor rate and HBM3 bandwidth, for a card allowed 700 W
+    return dict(tensor_burst=989.4, tensor_sustained=989.4, hbm=3350.0, source="H100 SXM data sheet (dense fp16, 700 W)")
 
 
 class ClockSampler:
@@ -127,8 +104,8 @@ def cpu_unet_eval_seconds(threads, reps=1):
 
 
 def run_reference(args):
-    """`--impl reference`: the reference's CPU implementation of the path (oracle port; /root/reference cannot travel
-    to the GPU box) on all host threads. Each step = a bounded sample: ONE guided UNet evaluation (N_s=2, 64x64);
+    """`--impl reference`: the reference's CPU implementation of the path (oracle port: the reference
+    itself need not be installed where the GPU is) on all host threads. Each step = a bounded sample: ONE guided UNet evaluation (N_s=2, 64x64);
     images/sec is extrapolated as 1 / (51 * t_eval + t_decode) with the VAE decode timed once."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
@@ -237,13 +214,13 @@ def run_gpu(args):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for _ in range(steps):
-            fn()
+            out = fn()
         e1.record()
         barrier()
         ms = torch.tensor([e0.elapsed_time(e1)], device=dev)
         if world > 1:
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
-        return float(ms)
+        return float(ms), out
 
     for _ in range(max(args.warmup, 3)):
         step_resident()
@@ -253,13 +230,18 @@ def run_gpu(args):
     n0 = ops.launch_count()
     if os.environ.get("SDB_PROFILE_RANGE"):   # ncu --profile-from-start off: only the timed steps are captured
         torch.cuda.profiler.start()
-    ms_total = timed(step_resident, args.steps)
+    ms_total, last_img = timed(step_resident, args.steps)
     if os.environ.get("SDB_PROFILE_RANGE"):
         torch.cuda.profiler.stop()
     launches = (ops.launch_count() - n0) // args.steps
     clk = clocks.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:   # what the timed path returned in its last step (before anything reuses it)
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "images.npy"), last_img.float().cpu().numpy())
+    del last_img
     step_e2e()
-    ms_e2e = timed(step_e2e, args.steps)
+    ms_e2e, _ = timed(step_e2e, args.steps)
     # sanity of what was timed (outside the timed region): the latent the 51 evaluations produce is finite and the
     # decoded image is not constant — a NaN anywhere in the UNet would show here
     lat = pipe(ids_d, un_d, x_T=xT_d, return_latent=True)
@@ -281,7 +263,7 @@ def run_gpu(args):
         ts.append(e0.elapsed_time(e1))
     unet_ms = sorted(ts)[len(ts) // 2]
 
-    # roofline of the dominant kernel family (tcgen05 GEMM / implicit conv): record every sdb_gemm descriptor of one
+    # roofline of the dominant kernel family (wgmma GEMM / implicit conv): record every sdb_gemm descriptor of one
     # UNet evaluation, then replay exactly those launches back to back through the C ABI between two CUDA events on the
     # launching stream (no Python op overhead in between), L2 flushed before each replay
     roof = None
@@ -315,13 +297,9 @@ def run_gpu(args):
         n = len(recs)
         pk = peaks()
         ach = fl / (ms * 1e-3) / 1e12
-        traffic, traffic_src, traffic_n = gemm_dram_traffic()
-        roof = {"kernel": "gemm_tc_kernel (tcgen05 GEMM / implicit 3x3 conv, all tile shapes) + its split-K epilogue",
+        roof = {"kernel": "gemm_tc_kernel (wgmma GEMM / implicit 3x3 conv, all tile shapes) + its split-K epilogue",
                 "bound": "tensor", "achieved": ach, "peak": pk["tensor_sustained"], "unit": "TFLOP/s",
-                "frac": ach / pk["tensor_sustained"], "traffic": traffic,
-                "traffic_note": f"ncu dram__bytes_read+write summed over the {traffic_n} gemm_tc launches of one UNet evaluation "
-                                f"/ {traffic_n}, read at run time from {traffic_src}; algorithmic bytes per launch ~9.1 MB "
-                                "(weights 1.72 GB + operands)",
+                "frac": ach / pk["tensor_sustained"],
                 "peak_source": pk["source"] + ", sustained bf16", "launches_per_unet_eval": n,
                 "kernels_per_unet_eval": int(gemm_kernels),
                 "algorithmic_gflop_per_launch": fl / n / 1e9, "avg_launch_us": 1000.0 * ms / n,
@@ -372,7 +350,7 @@ def run_gpu(args):
             "warmup": max(args.warmup, 3), "ms_per_step": ms_total / args.steps, "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None, "dtype": "fp16", "data": "synthetic",
             "config": {"workload": f"txt2img SD-v1-4 random-init, 512x512, 50 PLMS steps (51 UNet evals), CFG 7.5, "
-                                   f"batch {B} per GPU", "parallelism": f"dp{world}", "l2": "weights 2.1 GB > 126 MB L2; "
+                                   f"batch {B} per GPU", "parallelism": f"dp{world}", "l2": "weights 2.1 GB > 50 MB L2; "
                                    "no explicit flush inside a step (UNet-only timing flushes L2)",
                        "arithmetic": "fp16 tensor-core operands, fp32 accumulate / residual stream / norms / softmax",
                        "algorithmic_tflop_per_image": (51 * 2 * UNET_GF_PER_SAMPLE + VAE_DEC_GF + 2 * CLIP_GF_PER_PROMPT) / 1e3},
@@ -395,6 +373,8 @@ def main():
     ap.add_argument("--impl", default="sdb200", choices=["sdb200", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--extra-batch", type=int, default=8, help="also time one step at this per-GPU batch (0: skip)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the images of the last timed step as DIR/images.npy (float32)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

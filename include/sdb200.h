@@ -1,5 +1,5 @@
 /*
- * sdb200 — C ABI of the B200-native latent-diffusion kernels.
+ * sdb200 — C ABI of the H100-native latent-diffusion kernels.
  *
  * The reference (CompVis/stable-diffusion) has no FFI: its plug-in boundary is `instantiate_from_config`
  * (ldm/util.py:78-93) plus the duck-typed nn.Module contracts around the denoising loop. This header is the
@@ -40,7 +40,7 @@ enum {
 };
 
 /*
- * Tensor-core GEMM / implicit-GEMM convolution (tcgen05 + TMA), fp16 operands, fp32 accumulate:
+ * Tensor-core GEMM / implicit-GEMM convolution (wgmma + TMA), fp16 operands, fp32 accumulate:
  *
  *   acc[m, n] = sum_k A[m, k] * B[n, k]
  *   v         = alpha * acc + bias[n] + film[m / rows_per_sample, n] + residual[m, n]
@@ -94,7 +94,7 @@ typedef struct sdb_gemm_desc {
                               on every side (UNet), 1 = pad only right/bottom (the VAE's asymmetric F.pad, model.py:73) */
   int32_t in_h, in_w;      /* input height / width when they differ from the output's h / w (stride 2); 0 = h, w */
   int32_t pair;            /* 0 auto, 1 single CTAs, 2 CTA pairs: two CTAs of a cluster compute one 256 x block_n tile
-                              with tcgen05.mma.cta_group::2, each loading half of the weight tile (block_n 128/160/256) */
+                              as a 2-CTA cluster, each loading half of the weight tile and multicasting it to both (block_n 128/160/256) */
   int32_t splitk_mode;     /* how split-K partials meet. 0 auto, 1 fp32 planes in `workspace` + a second kernel,
                               2 inside a thread-block cluster through distributed shared memory (2 or 4 slices, no
                               workspace traffic, fused epilogue in the same kernel) */
@@ -108,7 +108,7 @@ int sdb_gemm(const sdb_gemm_desc* d, sdb_stream_t stream);
 int sdb_gemm_plan(const sdb_gemm_desc* d, int32_t* out);
 
 /*
- * Fused multi-head attention (flash-style, S/P/O in TMEM), replaces CrossAttention.forward's
+ * Fused multi-head attention (flash-style, S/P/O in registers), replaces CrossAttention.forward's
  * einsum -> scale -> softmax -> einsum (ldm/modules/attention.py:178-192) without materialising N x N.
  *   q  : fp16 [batch, nq,  heads*dpad]   (row stride ldq elements; head h at column h*dpad)
  *   k  : fp16 [batch, nkv, heads*dpad]   (row stride ldk)

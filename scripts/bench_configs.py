@@ -1,4 +1,4 @@
-"""Timings of the other BASELINE.json configurations on one B200 (not the headline bench line):
+"""Timings of the other BASELINE.json configurations on one H100 (not the headline bench line):
 C3 txt2img DDIM-50 batch 32, C4-per-GPU txt2img PLMS-50 batch 8, C5 img2img 768x768 strength 0.75 batch 4."""
 import json, sys, time, torch
 sys.path.insert(0, ".")

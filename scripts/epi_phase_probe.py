@@ -1,5 +1,5 @@
 """Sub-phase stamps of ONE epilogue chunk (SDB_DBG bit 6, sdb_debug_trace): epilogue warp 0, first chunk of the first
-tile. Columns are SM clocks relative to accumulator-ready: TMEM load done, fused math done, staging stored + proxy
+tile. Columns are SM clocks relative to accumulator-ready: accumulator load done, fused math done, staging stored + proxy
 fence done, chunk finished (TMA store issued + statistics), whole epilogue finished (all chunks, stores read)."""
 import ctypes as C, os, statistics, sys, torch
 sys.path.insert(0, ".")

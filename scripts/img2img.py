@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""img2img on the B200 engine with the reference script's flags (scripts/img2img.py:60-289):
+"""img2img on the H100 engine with the reference script's flags (scripts/img2img.py:60-289):
 encode_first_stage -> get_first_stage_encoding -> DDIM stochastic_encode(t_enc) -> decode -> decode_first_stage."""
 import argparse
 import os

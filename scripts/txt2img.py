@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""txt2img on the B200 engine with the reference script's flags (scripts/txt2img.py:98-235 of CompVis/stable-diffusion).
+"""txt2img on the H100 engine with the reference script's flags (scripts/txt2img.py:98-235 of CompVis/stable-diffusion).
 
   python scripts/txt2img.py --prompt "a photograph of an astronaut riding a horse" --plms --ckpt sd-v1-4.ckpt
 

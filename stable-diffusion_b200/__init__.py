@@ -1,4 +1,4 @@
-"""sdb200 — Blackwell-native (sm_100a) kernels and host mirror for the CompVis/stable-diffusion denoising loop.
+"""sdb200 — Hopper-native (sm_90a) kernels and host mirror for the CompVis/stable-diffusion denoising loop.
 
 The directory name carries a hyphen (as the project layout prescribes); import it through the `sdb200`
 alias module at the repo root, or `importlib.import_module("stable-diffusion_b200")`.

@@ -1,4 +1,4 @@
-"""Build the sm_100a C-ABI library in-tree: stable-diffusion_b200/csrc/libsdb200.so.
+"""Build the sm_90a (H100) C-ABI library in-tree: stable-diffusion_b200/csrc/libsdb200.so.
 
 nvcc cross-compiles without a GPU. Objects are rebuilt only when a source (or header) is newer.
 """
@@ -14,7 +14,7 @@ CSRC = Path(__file__).resolve().parent / "csrc"
 LIB = CSRC / "libsdb200.so"
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -56,7 +56,7 @@ def build(verbose: bool = False, force: bool = False) -> Path:
                 if verbose and out:
                     print(out, file=sys.stderr)
     if force or jobs or _newer(LIB, objs):
-        cmd = [NVCC, "-shared", "-o", str(LIB), *map(str, objs), "-gencode", "arch=compute_100a,code=sm_100a"]
+        cmd = [NVCC, "-shared", "-o", str(LIB), *map(str, objs), "-gencode", "arch=compute_90a,code=sm_90a"]
         run(cmd)
     return LIB
 

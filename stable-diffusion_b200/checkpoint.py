@@ -1,5 +1,5 @@
 """Checkpoint ingest (SURVEY 8f-1): the reference's `load_model_from_config(config, ckpt)` (scripts/txt2img.py:49-66,
-scripts/img2img.py:28-45) for the B200 engine — a `.ckpt` (pickled {"state_dict": ..., "global_step": ...}, what
+scripts/img2img.py:28-45) for the H100 engine — a `.ckpt` (pickled {"state_dict": ..., "global_step": ...}, what
 `torch.save` of a Lightning checkpoint holds) or a `.safetensors` file with the reference key names goes through
 `LatentDiffusion.load_state_dict(strict=False)`; `.cuda()` then packs the tensors into kernel-native fp16 layouts.
 

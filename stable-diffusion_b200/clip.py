@@ -1,10 +1,10 @@
-"""B200-native CLIP ViT-L/14 text encoder: drop-in for `ldm.modules.encoders.modules.FrozenCLIPEmbedder`
+"""H100-native CLIP ViT-L/14 text encoder: drop-in for `ldm.modules.encoders.modules.FrozenCLIPEmbedder`
 (modules.py:137-162: `encode(text) -> (B, 77, 768)` = CLIPTextModel(...).last_hidden_state).
 
 The arithmetic the reference delegates to third-party `transformers` (CLIPTextModel: token+position embedding,
 12 pre-LN causal self-attention layers with quick-GELU MLP, final LayerNorm) runs on the same kernel family as the
-UNet: fp32 LayerNorm -> fp16 operand, tcgen05 GEMMs with fused bias / quick-GELU / residual epilogues, the fused
-tcgen05 attention kernel with a causal mask. The value bias is folded through out_proj at pack time
+UNet: fp32 LayerNorm -> fp16 operand, wgmma GEMMs with fused bias / quick-GELU / residual epilogues, the fused
+wgmma attention kernel with a causal mask. The value bias is folded through out_proj at pack time
 (softmax rows sum to 1). State-dict keys are transformers' (`text_model.*`), found under
 `cond_stage_model.transformer.` in an SD checkpoint.
 

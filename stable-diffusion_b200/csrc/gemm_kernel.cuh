@@ -1,25 +1,25 @@
-// tcgen05 GEMM / implicit-GEMM 3x3 convolution for sm_100a — persistent, warp-specialised, optionally on CTA pairs
-// (cta_group::2) and with split-K reduced inside a thread-block cluster through distributed shared memory.
+// wgmma GEMM / implicit-GEMM 3x3 convolution for sm_90a — warp-specialised, one output tile per CTA, optionally on CTA
+// pairs (2-CTA clusters sharing the weight tile by TMA multicast) and with split-K reduced inside a thread-block
+// cluster through distributed shared memory.
 //
-//   grid        : persistent CTAs (or CTA pairs), static round-robin tile schedule (M fastest, so CTAs running side by
-//                 side read the same weight tile from L2). Cluster split-K: one cluster per output tile instead.
-//   warp 0      : TMA producer (one elected lane) — A tile [128 rows x 64 ch] via 4-D NHWC tensor maps (3x3 taps are
+//   grid        : one CTA (or CTA pair) per 128 x BN output tile, M fastest, so CTAs running side by side read the same
+//                 weight tile from L2. Cluster split-K: one cluster per output tile, one CTA (pair) per K slice.
+//   warp 8      : A producer (one elected lane) — A tile [128 rows x 64 ch] via 4-D NHWC tensor maps (3x3 taps are
 //                 shifted boxes; out-of-image reads are zero-filled by TMA = conv padding; stride-2 convs traverse the
 //                 input with element strides {1,2,2,1}; up to four A sources are concatenated along K: UNet skip
-//                 concat, or hi/lo fp16 splits of one fp32 activation), B tile [BN x 64] from the K-major weight
-//                 matrix. STAGES-deep mbarrier ring that runs across tiles.
-//   warp 1      : TMEM allocation + single-thread tcgen05.mma issue (M=128, N=BN, K=16), two accumulator buffers in
-//                 TMEM so the epilogue of tile i overlaps the main loop of tile i+1.
-//   warps 2..9  : epilogue (two warps per TMEM lane group, alternating 32-column chunks) — tcgen05.ld accumulator
-//                 rows (one row per thread), fused alpha/bias/FiLM/residual/activation in registers, 16-byte stores
-//                 into a swizzled staging tile, TMA store (cp.async.bulk.tensor) of each 32x32 block to the NHWC
-//                 output: fp16 (optionally a hi+lo pair) and/or fp32. Outputs whose row pitch TMA cannot address
-//                 (N = 3, 4 ...) take a scalar transposed path.
+//                 concat, or hi/lo fp16 splits of one fp32 activation). STAGES-deep mbarrier ring.
+//   warp 9      : B producer — B tile [BN x 64] from the K-major weight matrix.
+//   warps 0..7  : two consumer warpgroups. Main loop: warpgroup g issues wgmma (M = 64, N = BN, K = 16) for rows
+//                 64 g .. 64 g + 63 straight from the swizzled stage buffers, fp32 accumulators in registers. Epilogue:
+//                 the accumulators go to a shared-memory tile (the idle ring), then each warp takes accumulator rows
+//                 (one row per thread, 32-column chunks), fused alpha/bias/FiLM/residual/activation in registers,
+//                 16-byte stores into a swizzled staging tile, TMA store (cp.async.bulk.tensor) of each 32x32 block
+//                 to the NHWC output: fp16 (optionally a hi+lo pair) and/or fp32. Outputs whose row pitch TMA cannot
+//                 address (N = 3, 4 ...) take a scalar transposed path.
 //
-//   CTA pair (CG = 2): two CTAs of a cluster compute one 256 x BN tile. Each loads its own 128 rows of A and HALF of the
-//   B tile (BN/2 weight rows); the leader's single thread issues tcgen05.mma.cta_group::2 (M = 256), which reads both
-//   CTAs' shared memory and writes 128 accumulator rows into each CTA's tensor memory. Per CTA and K step the L2 -> SM
-//   traffic drops from (128 + BN) to (128 + BN/2) rows - the binding resource of these GEMMs (profiles/r02_*).
+//   CTA pair (CG = 2): the two CTAs of a cluster compute the two 128-row halves of a 256 x BN tile. Each loads its own
+//   A rows and HALF of the B tile (BN/2 weight rows), multicast into the shared memory of both CTAs, so the L2 -> SM
+//   weight traffic per CTA and K step drops from BN to BN/2 rows.
 //
 //   Cluster split-K: the S (x CG) CTAs of a cluster take K slices of one tile, exchange fp32 partials through
 //   distributed shared memory (rows scattered to their owner CTA), and each owner reduces its rows in a fixed order and
@@ -44,14 +44,12 @@ constexpr int BM = 128;
 constexpr int BK = 64;
 constexpr int A_BYTES = BM * BK * 2;
 constexpr int MAX_SRC = 4;
-constexpr int EPI_WARPS = 8;
+constexpr int EPI_WARPS = 8;          // the two consumer warpgroups (MMA, then epilogue)
 constexpr int STG_WARP_BYTES = 8192;  // per epilogue warp: 2 x 4 KB fp32 tiles, or 2 x (2 KB hi + 2 KB lo) fp16 tiles
 constexpr int STAGING_BYTES = EPI_WARPS * STG_WARP_BYTES;
-constexpr int GEMM_THREADS = 64 + 32 * EPI_WARPS + 32;   // + warp 10: weight (B) tile producer
-constexpr int B_WARP = 2 + EPI_WARPS;
-// single-tile (DEEP) epilogue: every epilogue warp stages ALL its chunks (<= 4) in a private 24 KB slice of the idle
-// operand ring: 4 x 4 KB fp32 tiles + 4 x 2 KB fp16 tiles (or 4 x (2 KB hi + 2 KB lo) when there is no fp32 output)
-constexpr int DEEP_WARP_STG = 24576;
+constexpr int A_WARP = EPI_WARPS;      // activation (A) tile producer
+constexpr int B_WARP = EPI_WARPS + 1;  // weight (B) tile producer
+constexpr int GEMM_THREADS = 32 * (EPI_WARPS + 2);
 
 struct TmapPack {
   CUtensorMap a[MAX_SRC];
@@ -60,7 +58,6 @@ struct TmapPack {
   CUtensorMap o16;   // fp16 output, same geometry, SWIZZLE_64B
   CUtensorMap o16lo; // fp16 low half
   CUtensorMap ows;   // split-K fp32 partial planes [C, W, H, NB, splits]
-  CUtensorMap res;   // fp32 residual, geometry of o32 (loaded into the staging tiles by the single-tile epilogue)
 };
 
 struct GemmArgs {
@@ -95,7 +92,6 @@ struct GemmArgs {
   int n_samples;
   int b_static;     // B is a weight matrix: safe to prefetch before griddepcontrol.wait
   int fast;         // outputs go through the TMA-store epilogue
-  int res_tma;      // the residual has a tensor map (tm.res): the single-tile epilogue loads it by TMA
   int bw, bh;       // store box: bw x bh x (32 / (bw*bh)) output pixels per epilogue warp
   int cstride, cshift;   // 3x3 conv: input pixel = cstride * o + tap - 1 + cshift (per axis)
   int film_table;   // 1: rows 0-63 / 64-127 of every tile belong to one sample each, so bias + FiLM fold into a
@@ -174,7 +170,7 @@ __device__ __forceinline__ void store_elem(const GemmArgs& p, float x, int orow,
   }
 }
 
-// Drain one 32x32 fp32 chunk that sits in the warp's padded staging tile (row = TMEM lane, col = chunk column) to
+// Drain one 32x32 fp32 chunk that sits in the warp's padded staging tile (row = accumulator row, col = chunk column) to
 // global memory with row-contiguous accesses: 16 lanes x 2 columns per row, two rows per instruction.
 //   mode 0: fused epilogue (alpha, bias, FiLM, residual, activation)   mode 1: raw split-K partial   mode 2: values
 //   already final (GEGLU computed in row layout)
@@ -260,24 +256,19 @@ __device__ __forceinline__ unsigned long long gtimer() {
     if (SDB_TRACE_ENABLED && trace && blockIdx.x < 160) trace[8 + blockIdx.x * 8 + (w)] = (val);   \
   } while (0)
 
-// DEEP: every CTA computes exactly ONE tile (grid <= resident CTAs, or cluster split-K). The epilogue then starts only
-// after the last MMA has retired, so its staging tiles alias the tail of the operand ring and the whole shared memory
-// (~210 KB) is pipeline: the main loop of these GEMMs is bound by the load round trip (TMA issue -> L2 -> MMA -> commit
-// -> slot free, ~2300 clk), i.e. by the bytes in flight per SM (profiles/r02_epilogue_probe.txt). Persistent multi-tile
-// CTAs keep a separate staging area (the epilogue of tile i overlaps the main loop of tile i+1) and fewer stages.
-template <int BN, int CG, bool DEEP>
+// Every CTA computes exactly ONE tile (the grid is one CTA per tile, or per tile and K slice). Once both consumer
+// warpgroups are past their last MMA the operand ring is idle, so the fp32 accumulator tile (ring head) and the
+// epilogue's staging tiles (ring tail) alias it and the whole shared memory is pipeline during the main loop.
+template <int BN, int CG>
 struct GemmCfg {
-  static constexpr int B_ROWS = BN / CG;            // weight rows of the tile this CTA loads
-  static constexpr int B_BYTES = B_ROWS * BK * 2;
+  static constexpr int B_ROWS = BN / CG;            // weight rows of the tile this CTA loads (multicast to the pair)
+  static constexpr int B_BYTES = BN * BK * 2;       // every CTA holds the whole B tile
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = DEEP ? (CG == 2 ? (BN <= 128 ? 9 : BN <= 160 ? 8 : 6)
-                                                : (BN <= 32 ? 10 : BN <= 64 ? 9 : BN <= 160 ? 6 : 4))
-                                     : (CG == 2 ? (BN <= 128 ? 6 : BN <= 160 ? 5 : 4) : (BN <= 64 ? 6 : BN <= 160 ? 4 : 3));
-  static constexpr int TMEM_COLS = BN <= 32 ? 64 : BN <= 64 ? 128 : BN <= 128 ? 256 : 512;  // two accumulators
+  static constexpr int ACC_BYTES = BN * BM * 4;
+  static constexpr int STAGES = (200 * 1024) / STAGE_BYTES < 10 ? (200 * 1024) / STAGE_BYTES : 10;
   static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
-  static constexpr int SMEM = RING_BYTES + (DEEP ? 0 : STAGING_BYTES) + 1024;
-  static_assert(!DEEP || RING_BYTES >= BN * 512 + STAGING_BYTES, "cluster split-K receive area + staging must fit the ring");
-  static_assert(!DEEP || RING_BYTES >= EPI_WARPS * DEEP_WARP_STG, "whole-tile staging must fit the ring");
+  static constexpr int SMEM = RING_BYTES + 1024;
+  static_assert(RING_BYTES >= ACC_BYTES + STAGING_BYTES, "accumulator tile (or cluster split-K receive area) + staging must fit the ring");
 };
 
 struct EpiRows {   // the output rows one epilogue warp handles: row per lane + the TMA store box origin
@@ -287,39 +278,37 @@ struct EpiRows {   // the output rows one epilogue warp handles: row per lane + 
 };
 
 // KIND selects what is compiled into an instantiation. Every instruction of an epilogue runs once per CTA from a cold
-// instruction cache, and the unrolled activation / GEGLU / scalar-store code of the general kernel tripled its size: with
-// it compiled out of the instantiations the UNet actually launches, one evaluation got 4.7 % faster.
+// instruction cache, so the activation / GEGLU / scalar-store code of the general kernel is compiled out of the
+// instantiations the UNet launches most.
 //   0 lean   : no activation, TMA-store epilogue, bias / FiLM through the column table  (almost every UNet GEMM)
 //   1 geglu  : GEGLU with fp16 output only (the feed-forward up-projection)
 //   2 general: everything (activations, scalar-store epilogue for odd widths, per-row FiLM, fp32 + fp16 hi/lo outputs)
 //   3 lean + cluster split-K (kind 0 is compiled without the cluster exchange, kind 3 without the single-CTA epilogue)
-template <int BN, int CG, bool DEEP, int KIND>
+template <int BN, int CG, int KIND>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_constant__ TmapPack tm, const GemmArgs p) {
   // compile-time specialisation of the descriptor fields the KIND fixes (dead branches fold away)
   const int act = (KIND == 0 || KIND == 3) ? SDB_ACT_NONE : (KIND == 1 ? SDB_ACT_GEGLU : p.act);
   const bool fast = KIND == 2 ? (p.fast != 0) : true;
   const bool film_row = KIND == 2 && p.film && !p.film_table;
-  // debug hooks (phase stamps, SDB_DBG switches) exist only in a -DSDB_TRACE build (SDB_BUILD_TRACE=1 python build.py):
-  // in the production kernel they were 8 % of the code every launch fetches
+  // debug hooks (phase stamps, SDB_DBG switches) exist only in a -DSDB_TRACE build (SDB_BUILD_TRACE=1 python build.py)
   const int dbg = SDB_TRACE_ENABLED ? p.dbg : 0;
   unsigned long long* const trace = SDB_TRACE_ENABLED ? p.trace : nullptr;
   const int csk = KIND == 0 ? 0 : (KIND == 3 ? 1 : p.csk);   // lean kinds: 0 = no cluster split-K, 3 = cluster split-K
-  using Cfg = GemmCfg<BN, CG, DEEP>;
+  using Cfg = GemmCfg<BN, CG>;
   constexpr int STAGES = Cfg::STAGES;
   constexpr int B_ROWS = Cfg::B_ROWS;
   constexpr int STAGE_BYTES = Cfg::STAGE_BYTES;
-  constexpr int TMEM_COLS = Cfg::TMEM_COLS;
+  constexpr int NCH = BN / 32;   // 32-column chunks of the accumulator
 
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment by offset (keeps the shared address space visible to the compiler: LDS/STS, not generic)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* staging = smem + Cfg::RING_BYTES - (DEEP ? STAGING_BYTES : 0);   // DEEP: aliases the last stages (idle by then)
+  uint8_t* staging = smem + Cfg::RING_BYTES - STAGING_BYTES;   // aliases the last stages (idle by then)
+  // accumulator tile after the main loop, ring head: 4 KB blocks [lane group][chunk] of 32 rows x 32 fp32, row r at
+  // r * 128 bytes, 16-byte granule q at (q ^ (r & 7)) << 4 (row-per-lane reads and fragment writes stay conflict-light)
+  uint8_t* accbuf = smem;
   __shared__ uint64_t full_bar[STAGES];
   __shared__ uint64_t empty_bar[STAGES];
-  __shared__ uint64_t acc_full[2];
-  __shared__ uint64_t acc_empty[2];
-  __shared__ uint64_t res_bar[EPI_WARPS];   // single-tile epilogue: residual tiles of one warp have landed
-  __shared__ uint32_t tmem_base_smem;
   // fused GroupNorm statistics: [lane group][column][sum, sum of squares]; one writer per slot per tile, fixed-order
   // fold at the flush, plain stores of the per-tile partials (deterministic)
   __shared__ __align__(16) float colsum[4 * BN * 2];
@@ -338,16 +327,17 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
   const uint32_t pr = CG == 2 ? (crank & 1u) : 0u;
   const uint32_t lead = crank - pr;
   const int csplit = csk ? static_cast<int>(crank) / CG : 0;
-  const int n_units = p.m_units * p.n_tiles * (csk ? 1 : p.splits);
   const int unit0 = csk ? static_cast<int>(blockIdx.x) / (p.splits * CG) : static_cast<int>(blockIdx.x) / CG;
-  const int ustride = csk ? (1 << 30) : static_cast<int>(gridDim.x) / CG;
-  auto decode = [&](int u, int& m_tile, int& n_tile, int& split) {
-    const int mu = u % p.m_units;
-    const int rest = u / p.m_units;
+  int m_tile, n_tile, split;
+  {
+    const int mu = unit0 % p.m_units;
+    const int rest = unit0 / p.m_units;
     n_tile = rest % p.n_tiles;
     split = csk ? csplit : rest / p.n_tiles;
     m_tile = mu * CG + static_cast<int>(pr);
-  };
+  }
+  const int it_begin = split * p.iters_per_split;
+  const int it_end = min(p.k_iters, it_begin + p.iters_per_split);
   if (trace && threadIdx.x == 0) {
     SDB_TR(0, gtimer());
     if (blockIdx.x == 0) {
@@ -358,11 +348,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
       trace[4] = p.M;
       trace[5] = p.N;
       trace[6] = p.taps;
-      trace[7] = n_units;
+      trace[7] = p.m_units * p.n_tiles * (csk ? 1 : p.splits);
     }
   }
 
-  if (warp == 0 && lane == 0) {
+  if (warp == A_WARP && lane == 0) {
     for (int i = 0; i < p.nsrc; ++i) tma_prefetch_desc(&tm.a[i]);
     tma_prefetch_desc(&tm.b);
     if (fast) {
@@ -370,43 +360,25 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
       if (p.out_f32) tma_prefetch_desc(&tm.o32);
       if (p.out_f16) tma_prefetch_desc(&tm.o16);
       if (p.out_f16_lo) tma_prefetch_desc(&tm.o16lo);
-      if (p.res_tma) tma_prefetch_desc(&tm.res);
     }
     for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);      // CTA pair: armed by the leader alone, with the bytes of BOTH CTAs
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], EPI_WARPS * CG);   // CTA pair: a slot is refilled once the consumers of BOTH CTAs freed it
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&acc_full[i], 1);
-      mbar_init(&acc_empty[i], EPI_WARPS * CG);
-    }
-    for (int i = 0; i < EPI_WARPS; ++i) mbar_init(&res_bar[i], 1);
     fence_barrier_init();
-  }
-  if (warp == 1) {
-    if (CG == 2) {
-      tmem_alloc_cg2(&tmem_base_smem, TMEM_COLS);
-      tmem_relinquish_cg2();
-    } else {
-      tmem_alloc(&tmem_base_smem, TMEM_COLS);
-      tmem_relinquish();
-    }
   }
   if (csk && p.stats) {   // lane groups this CTA does not own contribute zeros to its statistics
     for (int i = threadIdx.x; i < 4 * BN * 2; i += GEMM_THREADS) colsum[i] = 0.f;
   }
-  tc_fence_before();
-  if (clustered) cluster_sync_all();   // barrier inits visible to the peer before any remote arrive
+  if (clustered) cluster_sync_all();   // barrier inits visible to the peer before any remote arrive / multicast
   else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_d = tmem_base_smem;
   if (threadIdx.x == 0 && !(dbg & 64)) SDB_TR(2, clock64() - clk0);
 
-  // ---------------------------------------------------------------- epilogue state and helpers (warps 2..9)
-  const int ew = (warp - 2) & 7;
-  const int lg = warp & 3;       // TMEM lane group of this warp
-  const int par = ew >> 2;       // the two warps of a lane group alternate chunks
-  const int et = threadIdx.x - 64;
+  // ---------------------------------------------------------------- epilogue state and helpers (warps 0..7)
+  const int ew = warp & 7;
+  const int lg = warp >> 1;      // 32-row lane group of the tile: the rows of warps 2 lg, 2 lg + 1 in the MMA layout
+  const int par = warp & 1;      // the two warps of a lane group alternate chunks
+  const int et = threadIdx.x;
   uint8_t* stg = staging + ew * STG_WARP_BYTES;
   const bool geglu = (KIND == 0 || KIND == 3) ? false : (KIND == 1 ? true : ((p.act == SDB_ACT_GEGLU) && !p.ws));
   constexpr int HALF = BN / 2;
@@ -440,8 +412,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
     return rw;
   };
   // column table of a tile: bias (+ FiLM of the sample each row half belongs to); all epilogue warps take part
-  auto fill_coltab = [&](int m_tile, int n_tile, bool first) {
-    if (!first) asm volatile("bar.sync 1, %0;" ::"n"(32 * EPI_WARPS) : "memory");   // readers of the previous tile's table
+  auto fill_coltab = [&](int m_tile, int n_tile) {
     const TileGeo geo = tile_geo(p, m_tile);
     for (int i = et; i < 2 * BN; i += 32 * EPI_WARPS) {
       const int hsel = i / BN, cl = i - hsel * BN;
@@ -469,6 +440,18 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
     } else {
 #pragma unroll
       for (int q = 0; q < 8; ++q) r[q] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+  };
+  // one 32-column chunk of this warp's lane group from the accumulator tile: row lg * 32 + lane, columns c*32 .. +31
+  auto acc_ld32 = [&](int c, uint32_t (&r)[32]) {
+    const uint8_t* blk = accbuf + (lg * NCH + c) * 4096 + lane * 128;
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      const uint4 t = *reinterpret_cast<const uint4*>(blk + ((q ^ (lane & 7)) << 4));
+      r[4 * q] = t.x;
+      r[4 * q + 1] = t.y;
+      r[4 * q + 2] = t.z;
+      r[4 * q + 3] = t.w;
     }
   };
   // fused epilogue + staging + TMA store of one 32x32 chunk held in registers (row per thread); lgx = lane group of
@@ -651,430 +634,238 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
         p.stats[(static_cast<size_t>(s) * p.stats_T + t) * E + col0 / sg] = make_float2(a, b);
       }
     }
-    asm volatile("bar.sync 1, %0;" ::"n"(32 * EPI_WARPS) : "memory");   // slots consumed before the next tile rewrites them
   };
 
   // ---------------------------------------------------------------- roles
-  if (warp == 0 || warp == B_WARP) {
-    // Two single-thread producers: warp 0 streams the activation (A) tiles and arms the stage barriers, warp 10 streams
-    // the weight (B) tiles. One thread issuing both was the bottleneck of the whole main loop (~590 clk per K step of
-    // wait + index arithmetic + two TMA issues against a 320 clk MMA budget, profiles/r02_mainloop_probe.txt); all loop
-    // state is advanced incrementally (no division in the loop). Static weights do not depend on the previous kernel:
-    // their producer never executes griddepcontrol.wait and runs ahead under programmatic dependent launch.
+  if (warp == A_WARP || warp == B_WARP) {
+    // Two single-thread producers: warp 8 streams the activation (A) tiles and arms the stage barriers, warp 9 streams
+    // the weight (B) tiles. All loop state is advanced incrementally (no division in the loop). Static weights do not
+    // depend on the previous kernel: their producer never executes griddepcontrol.wait and runs ahead under
+    // programmatic dependent launch.
     if (elect_one()) {
-      // CTA pair: the loads of both CTAs complete on the LEADER's full barrier (its MMA thread consumes both halves).
-      // Only the leader arms it - locally, with the bytes of both CTAs; completions of the peer's loads that overtake the
-      // arming just drive the transaction count negative for a moment (a remote arrive per stage would put a cluster
-      // round trip into the producer's issue loop).
-      const bool is_a = warp == 0;
-      const uint32_t full_base = CG == 2 ? mapa_shared(smem_u32(&full_bar[0]), lead) : smem_u32(&full_bar[0]);
-      const uint32_t arm_bytes = (((dbg & 8) ? 0u : Cfg::B_BYTES) + ((dbg & 32) ? 0u : A_BYTES)) * CG;
-      const uint32_t smem_base = smem_u32(smem) + (is_a ? 0u : static_cast<uint32_t>(A_BYTES));
-      // the dependency wait sits right before this thread's first load: the tile decode / tap geometry below (cold code with
-      // integer divisions) overlaps the predecessor's tail instead of following it
-      bool need_wait = is_a || !p.b_static;
+      // CTA pair: each CTA loads its own 128 A rows and HALF of the B tile, multicast into both CTAs' rings; every CTA
+      // arms its own full barrier with the bytes of its A tile and of the whole B tile. Completions of the peer's
+      // multicast that overtake the arming just drive the transaction count negative for a moment.
+      const bool is_a = warp == A_WARP;
+      const uint32_t full_base = smem_u32(&full_bar[0]);
+      const uint32_t arm_bytes = ((dbg & 8) ? 0u : Cfg::B_BYTES) + ((dbg & 32) ? 0u : A_BYTES);
+      const uint32_t smem_base =
+          smem_u32(smem) + (is_a ? 0u : static_cast<uint32_t>(A_BYTES) + pr * static_cast<uint32_t>(B_ROWS * BK * 2));
+      const uint16_t mc_mask = static_cast<uint16_t>(3u << lead);   // the two CTAs of this pair
       int s = 0;
       uint32_t ph = 0;
       bool ring_pass = false;
       uint32_t dst = smem_base, bar = full_base;
       const int cpt = p.cb[p.nsrc];
-      for (int u = unit0; u < n_units; u += ustride) {
-        int m_tile, n_tile, split;
-        decode(u, m_tile, n_tile, split);
-        const int it_begin = split * p.iters_per_split;
-        const int it_end = min(p.k_iters, it_begin + p.iters_per_split);
-        // A: position inside the (tap, source, 64-channel chunk) sequence, advanced per K step
-        int x0 = 0, y0 = 0, n0 = 0;
-        if (p.taps == 1) {
-          x0 = m_tile * BM;
-        } else {
-          int tx = m_tile % p.tiles_x;
-          int t2 = m_tile / p.tiles_x;
-          x0 = tx * p.TW * p.cstride + p.cshift;
-          y0 = (t2 % p.tiles_y) * p.TH * p.cstride + p.cshift;
-          n0 = (t2 / p.tiles_y) * p.TN;
-        }
-        int tap = it_begin / cpt, cc = it_begin - tap * cpt;
-        int dx = 0, dy = 0;
-        if (p.taps == 9) {
-          dy = tap / 3 - 1;
-          dx = tap - (tap / 3) * 3 - 1;
-        }
-        int src = 0;
-        while (src + 1 < p.nsrc && cc >= p.cb[src + 1]) ++src;
-        int cend = p.cb[src + 1];
-        int c0 = (cc - p.cb[src]) * BK;
-        const CUtensorMap* amap = &tm.a[src];
-        int kb = it_begin * BK;
-        const int nrow = n_tile * BN + static_cast<int>(pr) * B_ROWS;
-        if (need_wait) {
-          pdl_wait();
-          need_wait = false;
-          if (is_a && !(dbg & 64)) SDB_TR(3, clock64() - clk0);
-        }
-        for (int it = it_begin; it < it_end; ++it) {
-          if (ring_pass) mbar_wait(&empty_bar[s], ph ^ 1);   // (first pass over the ring: every slot is free)
-          if (is_a) {
-            if (pr == 0) mbar_arrive_expect_tx(&full_bar[s], arm_bytes);
-            if (!(dbg & 32)) {
-              if (CG == 2) tma_load_4d_cg2_addr(dst, amap, bar, c0, x0 + dx, y0 + dy, n0);
-              else tma_load_4d_addr(dst, amap, bar, c0, x0 + dx, y0 + dy, n0);
-            }
-            // next K step: chunk -> source -> tap
-            c0 += BK;
-            if (++cc == cend) {
-              if (cc == cpt) {
-                cc = 0;
-                src = 0;
-                if (++dx == 2) {
-                  dx = -1;
-                  ++dy;
-                }
-              } else {
-                ++src;
+      // A: position inside the (tap, source, 64-channel chunk) sequence, advanced per K step
+      int x0 = 0, y0 = 0, n0 = 0;
+      if (p.taps == 1) {
+        x0 = m_tile * BM;
+      } else {
+        int tx = m_tile % p.tiles_x;
+        int t2 = m_tile / p.tiles_x;
+        x0 = tx * p.TW * p.cstride + p.cshift;
+        y0 = (t2 % p.tiles_y) * p.TH * p.cstride + p.cshift;
+        n0 = (t2 / p.tiles_y) * p.TN;
+      }
+      int tap = it_begin / cpt, cc = it_begin - tap * cpt;
+      int dx = 0, dy = 0;
+      if (p.taps == 9) {
+        dy = tap / 3 - 1;
+        dx = tap - (tap / 3) * 3 - 1;
+      }
+      int src = 0;
+      while (src + 1 < p.nsrc && cc >= p.cb[src + 1]) ++src;
+      int cend = p.cb[src + 1];
+      int c0 = (cc - p.cb[src]) * BK;
+      const CUtensorMap* amap = &tm.a[src];
+      int kb = it_begin * BK;
+      const int nrow = n_tile * BN + static_cast<int>(pr) * B_ROWS;
+      // the dependency wait sits right before this thread's first load: the tile decode / tap geometry above (cold
+      // code with integer divisions) overlaps the predecessor's tail instead of following it
+      if (is_a || !p.b_static) {
+        pdl_wait();
+        if (is_a && !(dbg & 64)) SDB_TR(3, clock64() - clk0);
+      }
+      for (int it = it_begin; it < it_end; ++it) {
+        if (ring_pass) mbar_wait_mma(&empty_bar[s], ph ^ 1);   // (first pass over the ring: every slot is free)
+        if (is_a) {
+          mbar_arrive_expect_tx(&full_bar[s], arm_bytes);
+          if (!(dbg & 32)) tma_load_4d_addr(dst, amap, bar, c0, x0 + dx, y0 + dy, n0);
+          // next K step: chunk -> source -> tap
+          c0 += BK;
+          if (++cc == cend) {
+            if (cc == cpt) {
+              cc = 0;
+              src = 0;
+              if (++dx == 2) {
+                dx = -1;
+                ++dy;
               }
-              c0 = 0;
-              cend = p.cb[src + 1];
-              amap = &tm.a[src];
+            } else {
+              ++src;
             }
-          } else {
-            if (!(dbg & 8)) {
-              if (CG == 2) tma_load_2d_cg2_addr(dst, &tm.b, bar, kb, nrow);
-              else tma_load_2d_addr(dst, &tm.b, bar, kb, nrow);
-            }
-            kb += BK;
+            c0 = 0;
+            cend = p.cb[src + 1];
+            amap = &tm.a[src];
           }
-          dst += STAGE_BYTES;
-          bar += 8;
-          if (++s == STAGES) {
-            s = 0;
-            ph ^= 1;
-            dst = smem_base;
-            bar = full_base;
-            ring_pass = true;
+        } else {
+          if (!(dbg & 8)) {
+            if (CG == 2) tma_load_2d_mc_addr(dst, &tm.b, bar, kb, nrow, mc_mask);
+            else tma_load_2d_addr(dst, &tm.b, bar, kb, nrow);
           }
+          kb += BK;
+        }
+        dst += STAGE_BYTES;
+        bar += 8;
+        if (++s == STAGES) {
+          s = 0;
+          ph ^= 1;
+          dst = smem_base;
+          bar = full_base;
+          ring_pass = true;
         }
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (pr == 0 && elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_f16(BM * CG, BN);
-      const uint16_t cmask = static_cast<uint16_t>(3u << lead);   // the two CTAs of this pair
-      // descriptor low words advance with the stage (start address >> 4); the high word is constant
-      const uint32_t desc_lo0 = (smem_u32(smem) & 0x3FFFFu) >> 4;
-      constexpr uint32_t DESC_HI = (1024u >> 4) | (1u << 14) | (2u << 29);   // SBO 1024 B, version 1, SWIZZLE_128B
-      uint32_t local = 0;
-      int s = 0;
-      uint32_t ph = 0, dlo = desc_lo0;
-      bool first_data = true;
-      for (int u = unit0; u < n_units; u += ustride, ++local) {
-        int m_tile, n_tile, split;
-        decode(u, m_tile, n_tile, split);
-        const int it_begin = split * p.iters_per_split;
-        const int it_end = min(p.k_iters, it_begin + p.iters_per_split);
-        const uint32_t ab = local & 1;
-        mbar_wait(&acc_empty[ab], ((local >> 1) & 1) ^ 1);  // epilogue(s) have drained this accumulator
-        tc_fence_after();
-        const uint32_t d_addr = tmem_d + ab * BN;
-        uint32_t acc = 0;
-        for (int it = it_begin; it < it_end; ++it) {
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after();
-          if (first_data) {
-            if (!(dbg & 64)) SDB_TR(4, clock64() - clk0);
-            first_data = false;
-          }
-          if (!(dbg & 16)) {
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k) {
-              // advance 32 bytes (16 fp16) along K inside the 128-byte swizzle atom: +2 in the (addr>>4) field
-              if (CG == 2) umma_f16_cg2_w(d_addr, dlo + 2 * k, dlo + (A_BYTES >> 4) + 2 * k, DESC_HI, idesc, acc);
-              else umma_f16_w(d_addr, dlo + 2 * k, dlo + (A_BYTES >> 4) + 2 * k, DESC_HI, idesc, acc);
-              acc = 1;
-            }
-          }
-          if (CG == 2) umma_commit_cg2(&empty_bar[s], cmask);
-          else umma_commit(&empty_bar[s]);
-          dlo += STAGE_BYTES >> 4;
-          if (++s == STAGES) {
-            s = 0;
-            ph ^= 1;
-            dlo = desc_lo0;
-          }
-        }
-        if (CG == 2) umma_commit_cg2(&acc_full[ab], cmask);
-        else umma_commit(&acc_full[ab]);
-      }
-      if (!(dbg & 64)) SDB_TR(5, clock64() - clk0);
+    if (csk) {   // the consumers' two cluster barriers around the split-K exchange
+      cluster_sync_all();
+      cluster_sync_all();
     }
-    __syncwarp();
-  } else if (!csk && warp < B_WARP) {
-    // epilogue warps 2..9 : TMEM lane group = warp % 4; the two warps of a lane group alternate chunks.
-    // Latency plan: everything the fused epilogue reads from global memory is requested BEFORE the accumulator is
-    // ready - bias (+ FiLM) of the tile's columns go to a shared-memory table, the residual rows of a chunk are
-    // prefetched into registers one chunk ahead (the first one while the main loop still runs) - so the chunk loop is
-    // TMEM load -> FMAs -> staging -> TMA store with no exposed L2 round trip.
+  } else {
+    // ---- main loop: two consumer warpgroups, warpgroup g computes rows 64 g .. 64 g + 63 of the tile with wgmma
+    // (M = 64, N = BN, K = 16) straight from the swizzled stage buffers; one MMA group stays in flight while the
+    // previous stage is handed back to the producers
     pdl_wait();   // residual / FiLM reads and all output writes come after the previous kernel has completed
-    float* stage = reinterpret_cast<float*>(stg);  // scalar path: [32][33] floats
-    const uint32_t acc_empty_lead = CG == 2 ? mapa_shared(smem_u32(&acc_empty[0]), lead) : 0u;
-    auto release_acc = [&](uint32_t ab) {   // accumulator fully read by this warp: hand it back to the (leader's) MMA warp
-      tc_fence_before();
+    float acc[BN / 2];   // rows 16 warp + lane / 4 (+ 8) of the tile, wgmma fragment layout (see wgmma.cuh)
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    const uint32_t a_off = static_cast<uint32_t>((warp >> 2) * 64 * 128);
+    const uint32_t peer_empty = CG == 2 ? mapa_shared(smem_u32(&empty_bar[0]), crank ^ 1u) : 0u;
+    auto release = [&](int s) {
       __syncwarp();
       if (lane == 0) {
-        if (CG == 2 && pr != 0) mbar_arrive_cluster(acc_empty_lead + 8u * ab);
-        else mbar_arrive(&acc_empty[ab]);
+        mbar_arrive(&empty_bar[s]);
+        if (CG == 2) mbar_arrive_cluster(peer_empty + 8u * s);
       }
     };
-    bool whole_tile_done = false;
-    if constexpr (DEEP) {
-      if (fast && !geglu && (KIND == 0 || KIND == 3 || !(st32 && st16 && p.out_f16_lo))) {
-        // ---- single-tile epilogue. The CTA owns exactly one tile and the operand ring is idle once the accumulator is
-        // complete, so every warp stages ALL its chunks in a private slice of it: the TMEM loads of two chunks are in
-        // flight together, the residual tile arrives by TMA (in the swizzled layout of the store boxes - a row-per-thread
-        // global read costs 32 L1 wavefronts per instruction) straight into the fp32 staging tile and is summed in place,
-        // nothing waits for a staging buffer to be recycled, and there is one proxy fence + one bulk group per batch.
-        // (Plain 16-byte global stores from a second row-contiguous pass were measured 30-90 % slower than the bulk
-        // stores: the epilogue of a one-wave GEMM moves the whole output through the SM <-> L2 path at once.)
-        whole_tile_done = true;
-        int m_tile, n_tile, split;
-        decode(unit0, m_tile, n_tile, split);
-        const EpiRows rw = rows_of(m_tile, lg);
-        if (use_tab) fill_coltab(m_tile, n_tile, true);
-        uint8_t* wstg = smem + ew * DEEP_WARP_STG;
-        const int my_n = (n_chunks - par + 1) / 2;   // chunks par, par + 2, ... of this lane group
-        const bool fuse = !split_fast;
-        const bool res_smem = fuse && p.residual && p.res_tma;
-        mbar_wait(&acc_full[0], 0);
-        tc_fence_after();
-        if (threadIdx.x == 64) SDB_TR(6, clock64() - clk0);
-        if (res_smem && lane == 0) {
-          int nload = 0;
-          for (int k = 0; k < my_n; ++k)
-            if (n_tile * BN + (par + 2 * k) * 32 < n_lim) ++nload;
-          if (nload) mbar_arrive_expect_tx(&res_bar[ew], nload * 4096);
-          for (int k = 0; k < my_n; ++k) {
-            const int oc = n_tile * BN + (par + 2 * k) * 32;
-            if (oc < n_lim) tma_load_5d(wstg + k * 4096, &tm.res, &res_bar[ew], oc, rw.sx, rw.sy, rw.sn, 0);
-          }
-        }
-        const uint32_t taddr = tmem_d + (static_cast<uint32_t>(lg * 32) << 16);
-        const bool w32 = split_fast || p.out_f32;
-        const bool w16 = !split_fast && p.out_f16;
-        const bool w16lo = w16 && p.out_f16_lo;
-        const uint32_t vmask = __ballot_sync(0xffffffffu, rw.valid);
-        bool res_ready = false;
-        // one chunk: registers -> fused epilogue -> staging tiles (k = index of the chunk inside this warp)
-        auto process = [&](uint32_t (&rr)[32], int k) {
-          const int c = par + 2 * k;
-          const int ocol0 = n_tile * BN + c * 32;
-          if (ocol0 >= n_lim) return;
-          float v[32];
+    int s = 0, prev = -1;
+    uint32_t ph = 0;
+    wgmma_hold(acc);
+    for (int it = it_begin; it < it_end; ++it) {
+      mbar_wait_mma(&full_bar[s], ph);
+      if (it == it_begin && threadIdx.x == 0 && !(dbg & 64)) SDB_TR(4, clock64() - clk0);
+      const uint32_t base = smem_u32(smem) + static_cast<uint32_t>(s * STAGE_BYTES);
+      wgmma_fence();
+      if (!(dbg & 16)) {
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(rr[j]);
-          uint8_t* s32 = wstg + k * 4096;
-          uint8_t* s16 = st32 ? wstg + 16384 + k * 2048 : wstg + k * 4096;
-          uint8_t* s16l = s16 + 2048;
-          if (fuse) {
-            const float4* tp = reinterpret_cast<const float4*>(coltab + (lg >= 2 ? BN : 0) + c * 32);
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              const float4 t = tp[q];
-              v[4 * q] = fmaf(v[4 * q], p.alpha, t.x);
-              v[4 * q + 1] = fmaf(v[4 * q + 1], p.alpha, t.y);
-              v[4 * q + 2] = fmaf(v[4 * q + 2], p.alpha, t.z);
-              v[4 * q + 3] = fmaf(v[4 * q + 3], p.alpha, t.w);
-            }
-            if (film_row) {
-              const float4* fp = reinterpret_cast<const float4*>(p.film + static_cast<size_t>(rw.sample) * p.ldf + ocol0);
-#pragma unroll
-              for (int q = 0; q < 8; ++q) {
-                float4 t = __ldg(fp + q);
-                v[4 * q] += t.x;
-                v[4 * q + 1] += t.y;
-                v[4 * q + 2] += t.z;
-                v[4 * q + 3] += t.w;
-              }
-            }
-            if (p.residual) {
-              if (res_smem) {
-                if (!res_ready) {
-                  mbar_wait(&res_bar[ew], 0);
-                  res_ready = true;
-                }
-#pragma unroll
-                for (int q = 0; q < 8; ++q) {
-                  const float4 t = *reinterpret_cast<const float4*>(s32 + lane * 128 + ((q ^ (lane & 7)) << 4));
-                  v[4 * q] += t.x;
-                  v[4 * q + 1] += t.y;
-                  v[4 * q + 2] += t.z;
-                  v[4 * q + 3] += t.w;
-                }
-              } else if (rw.valid) {
-                const float4* rp = reinterpret_cast<const float4*>(p.residual + static_cast<size_t>(rw.row) * p.ldr + ocol0);
-#pragma unroll
-                for (int q = 0; q < 8; ++q) {
-                  const float4 t = rp[q];
-                  v[4 * q] += t.x;
-                  v[4 * q + 1] += t.y;
-                  v[4 * q + 2] += t.z;
-                  v[4 * q + 3] += t.w;
-                }
-              }
-            }
-            if (act != SDB_ACT_NONE) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) v[j] = apply_act(v[j], act);
-            }
-          }
-          if (w32) {
-#pragma unroll
-            for (int q = 0; q < 8; ++q)
-              *reinterpret_cast<float4*>(s32 + lane * 128 + ((q ^ (lane & 7)) << 4)) =
-                  make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-          }
-          if (w16) {
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              __half2 h[4];
-              uint4 u, ul;
-#pragma unroll
-              for (int e = 0; e < 4; ++e) h[e] = __floats2half2_rn(v[8 * q + 2 * e], v[8 * q + 2 * e + 1]);
-              u.x = *reinterpret_cast<uint32_t*>(&h[0]);
-              u.y = *reinterpret_cast<uint32_t*>(&h[1]);
-              u.z = *reinterpret_cast<uint32_t*>(&h[2]);
-              u.w = *reinterpret_cast<uint32_t*>(&h[3]);
-              const uint32_t off = lane * 64 + ((q ^ ((lane >> 1) & 3)) << 4);
-              *reinterpret_cast<uint4*>(s16 + off) = u;
-              if (w16lo) {
-                __half2 l[4];
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  float2 hf = __half22float2(h[e]);
-                  l[e] = __floats2half2_rn(v[8 * q + 2 * e] - hf.x, v[8 * q + 2 * e + 1] - hf.y);
-                }
-                ul.x = *reinterpret_cast<uint32_t*>(&l[0]);
-                ul.y = *reinterpret_cast<uint32_t*>(&l[1]);
-                ul.z = *reinterpret_cast<uint32_t*>(&l[2]);
-                ul.w = *reinterpret_cast<uint32_t*>(&l[3]);
-                *reinterpret_cast<uint4*>(s16l + off) = ul;
-              }
-            }
-          }
-        };
-        // GroupNorm partial sums of one staged fp32 chunk (see emit() for the access pattern)
-        auto chunk_stats = [&](int k) {
-          const int c = par + 2 * k;
-          if (n_tile * BN + c * 32 >= n_lim) return;
-          const uint8_t* s32 = wstg + k * 4096;
-          const int gq = lane & 7, rb = lane >> 3;
-          float cs[4] = {0.f, 0.f, 0.f, 0.f}, cq[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk) {
-            const int r = rb + 4 * kk;
-            float4 x = *reinterpret_cast<const float4*>(s32 + r * 128 + ((gq ^ (r & 7)) << 4));
-            const float keep = ((vmask >> r) & 1u) ? 1.0f : 0.0f;
-            x.x *= keep;
-            x.y *= keep;
-            x.z *= keep;
-            x.w *= keep;
-            cs[0] += x.x;
-            cs[1] += x.y;
-            cs[2] += x.z;
-            cs[3] += x.w;
-            cq[0] = fmaf(x.x, x.x, cq[0]);
-            cq[1] = fmaf(x.y, x.y, cq[1]);
-            cq[2] = fmaf(x.z, x.z, cq[2]);
-            cq[3] = fmaf(x.w, x.w, cq[3]);
-          }
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            cs[j] += __shfl_xor_sync(0xffffffffu, cs[j], 8);
-            cq[j] += __shfl_xor_sync(0xffffffffu, cq[j], 8);
-            cs[j] += __shfl_xor_sync(0xffffffffu, cs[j], 16);
-            cq[j] += __shfl_xor_sync(0xffffffffu, cq[j], 16);
-          }
-          if (lane < 8) {
-            const int cl = c * 32 + 4 * gq;
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-              *reinterpret_cast<float2*>(&colsum[(lg * BN + cl + j) * 2]) = make_float2(cs[j], cq[j]);
-          }
-        };
-        const bool do_stats = fuse && p.stats && w32 && !(dbg & 1);
-#pragma unroll 1
-        for (int k0 = 0; k0 < my_n; k0 += 2) {
-          const bool two = k0 + 1 < my_n;
-          uint32_t ra[32], rb2[32];
-          tmem_ld32(taddr + (par + 2 * k0) * 32, ra);
-          if (two) tmem_ld32(taddr + (par + 2 * k0 + 2) * 32, rb2);
-          tmem_ld_wait();
-          const bool stamp = trace && (dbg & 64) && threadIdx.x == 64 && k0 == 0;
-          if (stamp) SDB_TR(3, clock64() - clk0);
-          process(ra, k0);
-          if (two) process(rb2, k0 + 1);
-          if (stamp) SDB_TR(4, clock64() - clk0);
-          fence_proxy_async();
-          __syncwarp();
-          if (stamp) SDB_TR(5, clock64() - clk0);
-          if (lane == 0 && !(dbg & 4)) {
-            for (int k = k0; k < k0 + (two ? 2 : 1); ++k) {
-              const int oc = n_tile * BN + (par + 2 * k) * 32;
-              if (oc >= n_lim) continue;
-              const uint8_t* s32 = wstg + k * 4096;
-              const uint8_t* s16 = st32 ? wstg + 16384 + k * 2048 : wstg + k * 4096;
-              if (split_fast) {
-                tma_store_5d(&tm.ows, s32, oc, rw.sx, rw.sy, rw.sn, split);
-              } else {
-                if (w32) tma_store_5d(&tm.o32, s32, oc, rw.sx, rw.sy, rw.sn, 0);
-                if (w16) tma_store_5d(&tm.o16, s16, oc, rw.sx, rw.sy, rw.sn, 0);
-                if (w16lo) tma_store_5d(&tm.o16lo, s16 + 2048, oc, rw.sx, rw.sy, rw.sn, 0);
-              }
-            }
-            tma_store_commit();
-          }
-          if (do_stats) {
-            chunk_stats(k0);
-            if (two) chunk_stats(k0 + 1);
-          }
-          if (stamp) SDB_TR(2, clock64() - clk0);
-        }
-        tc_fence_before();
-        if (p.stats && !p.ws && !(dbg & 2)) flush_stats(m_tile, n_tile);
+        for (int k = 0; k < BK / 16; ++k)
+          WgmmaSS<BN>::mma(acc, wg_desc(base + a_off + 32 * k), wg_desc(base + A_BYTES + 32 * k), 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0) release(prev);
+      prev = s;
+      if (++s == STAGES) {
+        s = 0;
+        ph ^= 1;
       }
     }
-    uint32_t local = 0;
-    constexpr bool GENERIC_LOOP = !(DEEP && (KIND == 0 || KIND == 3));   // lean single-tile CTAs always take the path above
-    for (int u = unit0; GENERIC_LOOP && u < n_units && !whole_tile_done; u += ustride, ++local) {
-      int m_tile, n_tile, split;
-      decode(u, m_tile, n_tile, split);
-      const uint32_t ab = local & 1;
-      const EpiRows rw = rows_of(m_tile, lg);
-      if (use_tab) fill_coltab(m_tile, n_tile, local == 0);
-      float4 rcur[8];
-      if (pre_res && par < n_chunks) load_res(rw, n_tile, par, rcur);
+    wgmma_wait<0>();
+    wgmma_hold(acc);
+    if (prev >= 0) release(prev);
+    if (threadIdx.x == 0 && !(dbg & 64)) SDB_TR(5, clock64() - clk0);
+    // both warpgroups are past their last MMA and every load of the tile has landed: the ring is free
+    asm volatile("bar.sync 1, %0;" ::"n"(32 * EPI_WARPS) : "memory");
 
-      mbar_wait(&acc_full[ab], (local >> 1) & 1);
-      tc_fence_after();
-      if (local == 0 && threadIdx.x == 64) SDB_TR(6, clock64() - clk0);
-      const uint32_t taddr = tmem_d + ab * BN + (static_cast<uint32_t>(lg * 32) << 16);
-      int last_c = -1;
-      for (int c = par; c < n_chunks; c += 2) last_c = c;
-      if (last_c < 0) release_acc(ab);  // BN = 32: the odd-parity warps own no chunk but still take part in the hand-off
-      if (KIND == 1 || (geglu && fast && !p.out_f32 && !p.out_f16_lo)) {
-        // GEGLU tiles (fp16 output): value and gate halves of a chunk are two TMEM loads. The loads of this warp's NEXT
-        // chunk are issued as soon as the current chunk is packed to fp16 (16 registers): they are in flight during the
-        // staging, fence and bulk store of the current one - and while the tensor pipe, which owns the TMEM port while it
-        // accumulates the next tile (K is short here: 5-20 steps), keeps them waiting.
-        uint32_t xr[32], gr[32];
-        if (par < n_chunks) {
-          tmem_ld32(taddr + par * 32, xr);
-          tmem_ld32(taddr + HALF + par * 32, gr);
+    if (csk) {
+      // ---- cluster split-K: exchange + owner epilogue. S K-slices of ONE tile sit in the registers of the cluster's
+      // CTAs. Rows are scattered to their owner (K slice o owns lane groups [o * 4/S, (o+1) * 4/S) of its pair-rank's
+      // 128 rows) through distributed shared memory into the (now idle) stage ring; the owner sums the S partials in
+      // slice order and runs the fused epilogue. The producer warps take part in the two cluster barriers.
+      const int S = p.splits;
+      const int lgs_per = 4 / S;
+      const int n_tasks = lgs_per * n_chunks;   // (owned lane group, chunk) pairs; <= 2 per epilogue warp
+      EpiRows rw0{}, rw1{};
+      float4 r0[8], r1[8];
+      {
+        fill_coltab(m_tile, n_tile);
+        if (ew < n_tasks) {
+          rw0 = rows_of(m_tile, csplit * lgs_per + ew / n_chunks);
+          if (p.residual) load_res(rw0, n_tile, ew % n_chunks, r0);
         }
+        if (ew + 8 < n_tasks) {
+          rw1 = rows_of(m_tile, csplit * lgs_per + (ew + 8) / n_chunks);
+          if (p.residual) load_res(rw1, n_tile, (ew + 8) % n_chunks, r1);
+        }
+      }
+      __syncwarp();
+      cluster_sync_all();   // every CTA of the cluster is past its main loop: the stage rings are free
+      {
+        const int owner = lg / lgs_per, lgsub = lg - owner * lgs_per;
+        const int rl = 16 * (warp & 1) + (lane >> 2);
+        const uint32_t dst = mapa_shared(smem_u32(smem), static_cast<uint32_t>(owner * CG) + pr) +
+                             static_cast<uint32_t>((csplit * lgs_per + lgsub) * NCH) * 4096u + rl * 128u + (lane & 1) * 8u;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int q = 2 * (j & 3) + ((lane & 3) >> 1);
+          const uint32_t a = dst + static_cast<uint32_t>(j >> 2) * 4096u + ((q ^ (lane >> 2)) << 4);
+          st_cluster_f32x2(a, acc[4 * j], acc[4 * j + 1]);
+          st_cluster_f32x2(a + 8u * 128u, acc[4 * j + 2], acc[4 * j + 3]);
+        }
+      }
+      __syncwarp();
+      cluster_sync_all();   // partials have landed (release / acquire at cluster scope)
+      {
+#pragma unroll 1
+        for (int k = 0; k < 2; ++k) {
+          const int t = ew + 8 * k;
+          if (t >= n_tasks) break;
+          const int lgsub = t / n_chunks, c = t - lgsub * n_chunks;
+          float v[32];
+#pragma unroll
+          for (int j = 0; j < 32; ++j) v[j] = 0.f;
+          for (int src = 0; src < S; ++src) {   // fixed order: deterministic
+            const uint8_t* rp = smem + static_cast<size_t>((src * lgs_per + lgsub) * n_chunks + c) * 4096 + lane * 128;
+#pragma unroll
+            for (int q = 0; q < 8; ++q) {
+              const float4 t4 = *reinterpret_cast<const float4*>(rp + ((q ^ (lane & 7)) << 4));
+              v[4 * q] += t4.x;
+              v[4 * q + 1] += t4.y;
+              v[4 * q + 2] += t4.z;
+              v[4 * q + 3] += t4.w;
+            }
+          }
+          const int ocol0 = n_tile * BN + c * 32;
+          if (ocol0 < n_lim) emit(v, ocol0, n_tile, 0, k ? rw1 : rw0, csplit * lgs_per + lgsub, true, false, k ? r1 : r0);
+        }
+        if (p.stats) flush_stats(m_tile, n_tile);
+      }
+    } else {
+      // accumulator fragments -> accumulator tile in shared memory (see accbuf), then the row-per-lane epilogue
+      {
+        const int rl = 16 * (warp & 1) + (lane >> 2);
+        uint8_t* blk = accbuf + lg * NCH * 4096 + rl * 128 + (lane & 1) * 8;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int q = 2 * (j & 3) + ((lane & 3) >> 1);
+          uint8_t* a = blk + (j >> 2) * 4096 + ((q ^ (lane >> 2)) << 4);
+          *reinterpret_cast<float2*>(a) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(a + 8 * 128) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+      }
+      const EpiRows rw = rows_of(m_tile, lg);
+      if (use_tab) fill_coltab(m_tile, n_tile);   // (its barrier also publishes the accumulator tile)
+      else asm volatile("bar.sync 1, %0;" ::"n"(32 * EPI_WARPS) : "memory");
+      if (threadIdx.x == 0) SDB_TR(6, clock64() - clk0);
+      float* stage = reinterpret_cast<float*>(stg);  // scalar path: [32][33] floats
+      if (KIND == 1 || (geglu && fast && !p.out_f32 && !p.out_f16_lo)) {
+        // GEGLU tiles (fp16 output): value and gate halves of a chunk are two accumulator reads
 #pragma unroll 1
         for (int c = par; c < n_chunks; c += 2) {
-          uint32_t hp[16];
-          tmem_ld_wait();
+          uint32_t xr[32], gr[32], hp[16];
+          acc_ld32(c, xr);
+          acc_ld32(HALF / 32 + c, gr);
           const float* tb = coltab + c * 32;   // bias of the value half; gate half at +HALF
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
@@ -1084,12 +875,6 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
             const float g1 = fmaf(__uint_as_float(gr[2 * j + 1]), p.alpha, tb[HALF + 2 * j + 1]);
             const __half2 h = __floats2half2_rn(x0 * gelu_erf(g0), x1 * gelu_erf(g1));
             hp[j] = *reinterpret_cast<const uint32_t*>(&h);
-          }
-          if (c == last_c) {
-            release_acc(ab);
-          } else {
-            tmem_ld32(taddr + (c + 2) * 32, xr);
-            tmem_ld32(taddr + HALF + (c + 2) * 32, gr);
           }
           const int ocol0 = n_tile * HALF + c * 32;
           if (ocol0 < n_lim) {
@@ -1109,150 +894,66 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
             ++flip;
           }
         }
-        continue;
-      }
+      } else {
+        float4 rcur[8];
+        if (pre_res && par < n_chunks) load_res(rw, n_tile, par, rcur);
 #pragma unroll 1
-      for (int c = par; c < n_chunks; c += 2) {
-        float v[32];
-        float4 rnxt[8];
-        int ocol0;
-        const bool has_next = pre_res && (c + 2 < n_chunks);
-        if (geglu) {
-          uint32_t xr[32], gr[32];
-          tmem_ld32(taddr + c * 32, xr);
-          tmem_ld32(taddr + HALF + c * 32, gr);
-          tmem_ld_wait();
-          const float* tb = coltab + c * 32;   // bias of the value half; gate half at +HALF
+        for (int c = par; c < n_chunks; c += 2) {
+          float v[32];
+          float4 rnxt[8];
+          int ocol0;
+          const bool has_next = pre_res && (c + 2 < n_chunks);
+          if (geglu) {
+            uint32_t xr[32], gr[32];
+            acc_ld32(c, xr);
+            acc_ld32(HALF / 32 + c, gr);
+            const float* tb = coltab + c * 32;   // bias of the value half; gate half at +HALF
 #pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const float x = fmaf(__uint_as_float(xr[j]), p.alpha, tb[j]);
-            const float g = fmaf(__uint_as_float(gr[j]), p.alpha, tb[HALF + j]);
-            v[j] = x * gelu_erf(g);
+            for (int j = 0; j < 32; ++j) {
+              const float x = fmaf(__uint_as_float(xr[j]), p.alpha, tb[j]);
+              const float g = fmaf(__uint_as_float(gr[j]), p.alpha, tb[HALF + j]);
+              v[j] = x * gelu_erf(g);
+            }
+            ocol0 = n_tile * HALF + c * 32;
+          } else {
+            uint32_t rr[32];
+            if (has_next) load_res(rw, n_tile, c + 2, rnxt);   // next chunk's residual rows: in flight across this chunk's work
+            acc_ld32(c, rr);
+#pragma unroll
+            for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(rr[j]);
+            ocol0 = n_tile * BN + c * 32;
           }
-          ocol0 = n_tile * HALF + c * 32;
-        } else {
-          uint32_t rr[32];
-          tmem_ld32(taddr + c * 32, rr);
-          if (has_next) load_res(rw, n_tile, c + 2, rnxt);   // next chunk's residual rows: in flight across this chunk's work
-          tmem_ld_wait();
+          tr_chunk = trace && (dbg & 64) && threadIdx.x == 0 && c == par;
+          if (tr_chunk) SDB_TR(3, clock64() - clk0);
+          if (!fast) {
+            // scalar transposed path (row pitch not TMA-addressable); split-K partials are finished by
+            // splitk_epilogue_kernel on this path
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(rr[j]);
-          ocol0 = n_tile * BN + c * 32;
-        }
-        tr_chunk = trace && (dbg & 64) && threadIdx.x == 64 && local == 0 && c == par;
-        if (tr_chunk) SDB_TR(3, clock64() - clk0);
-        if (c == last_c) release_acc(ab);
-        if (!fast) {
-          // scalar transposed path (row pitch not TMA-addressable); split-K partials are finished by
-          // splitk_epilogue_kernel on this path
+            for (int j = 0; j < 32; ++j) stage[lane * 33 + j] = v[j];
+            __syncwarp();
+            drain_chunk(p, stage, lane, rw.row, rw.sample, rw.valid, ocol0, geglu ? p.N / 2 : p.N,
+                        geglu ? 2 : (p.ws ? 1 : 0), split);
+            __syncwarp();
+            continue;
+          }
+          if (ocol0 < n_lim) emit(v, ocol0, n_tile, split, rw, lg, !geglu && !split_fast, split_fast, rcur);
+          if (has_next) {
 #pragma unroll
-          for (int j = 0; j < 32; ++j) stage[lane * 33 + j] = v[j];
-          __syncwarp();
-          drain_chunk(p, stage, lane, rw.row, rw.sample, rw.valid, ocol0, geglu ? p.N / 2 : p.N,
-                      geglu ? 2 : (p.ws ? 1 : 0), split);
-          __syncwarp();
-          continue;
-        }
-        if (ocol0 < n_lim) emit(v, ocol0, n_tile, split, rw, lg, !geglu && !split_fast, split_fast, rcur);
-        if (has_next) {
-#pragma unroll
-          for (int q = 0; q < 8; ++q) rcur[q] = rnxt[q];
+            for (int q = 0; q < 8; ++q) rcur[q] = rnxt[q];
+          }
         }
       }
       if (p.stats && !p.ws && !(dbg & 2)) flush_stats(m_tile, n_tile);
     }
   }
 
-  // ---------------------------------------------------------------- cluster split-K: exchange + owner epilogue
-  if (csk) {
-    // S K-slices of ONE tile sit in the tensor memories of the cluster's CTAs. Rows are scattered to their owner
-    // (K slice o owns lane groups [o * 4/S, (o+1) * 4/S) of its pair-rank's 128 rows) through distributed shared
-    // memory into the (now idle) stage ring; the owner sums the S partials in slice order and runs the fused epilogue.
-    const int S = p.splits;
-    const int lgs_per = 4 / S;
-    int m_tile = 0, n_tile = 0, split = 0;
-    decode(unit0, m_tile, n_tile, split);
-    const int n_tasks = lgs_per * n_chunks;   // (owned lane group, chunk) pairs; <= 2 per epilogue warp
-    EpiRows rw0{}, rw1{};
-    float4 r0[8], r1[8];
-    if (warp >= 2 && warp < B_WARP) {
-      pdl_wait();
-      fill_coltab(m_tile, n_tile, true);
-      if (ew < n_tasks) {
-        rw0 = rows_of(m_tile, csplit * lgs_per + ew / n_chunks);
-        if (p.residual) load_res(rw0, n_tile, ew % n_chunks, r0);
-      }
-      if (ew + 8 < n_tasks) {
-        rw1 = rows_of(m_tile, csplit * lgs_per + (ew + 8) / n_chunks);
-        if (p.residual) load_res(rw1, n_tile, (ew + 8) % n_chunks, r1);
-      }
-      mbar_wait(&acc_full[0], 0);   // this CTA's (pair's) MMAs have completed
-      tc_fence_after();
-      if (threadIdx.x == 64) SDB_TR(6, clock64() - clk0);
-    }
-    __syncwarp();
-    cluster_sync_all();   // every CTA of the cluster is past its main loop: the stage rings are free
-    if (warp >= 2 && warp < B_WARP) {
-      const int owner = lg / lgs_per, lgsub = lg - owner * lgs_per;
-      const uint32_t dst = mapa_shared(smem_u32(smem), static_cast<uint32_t>(owner * CG) + pr) +
-                           static_cast<uint32_t>((csplit * lgs_per + lgsub) * n_chunks) * 4096u + lane * 128u;
-      const uint32_t taddr = tmem_d + (static_cast<uint32_t>(lg * 32) << 16);
-#pragma unroll 1
-      for (int c = par; c < n_chunks; c += 2) {
-        uint32_t rr[32];
-        tmem_ld32(taddr + c * 32, rr);
-        tmem_ld_wait();
-        const uint32_t a = dst + static_cast<uint32_t>(c) * 4096u;
-#pragma unroll
-        for (int q = 0; q < 8; ++q)
-          st_cluster_f32x4(a + ((q ^ (lane & 7)) << 4), __uint_as_float(rr[4 * q]), __uint_as_float(rr[4 * q + 1]),
-                           __uint_as_float(rr[4 * q + 2]), __uint_as_float(rr[4 * q + 3]));
-      }
-      tc_fence_before();
-    }
-    __syncwarp();
-    cluster_sync_all();   // partials have landed (release / acquire at cluster scope)
-    if (warp >= 2 && warp < B_WARP) {
-#pragma unroll 1
-      for (int k = 0; k < 2; ++k) {
-        const int t = ew + 8 * k;
-        if (t >= n_tasks) break;
-        const int lgsub = t / n_chunks, c = t - lgsub * n_chunks;
-        float v[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = 0.f;
-        for (int src = 0; src < S; ++src) {   // fixed order: deterministic
-          const uint8_t* rp = smem + static_cast<size_t>((src * lgs_per + lgsub) * n_chunks + c) * 4096 + lane * 128;
-#pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            const float4 t4 = *reinterpret_cast<const float4*>(rp + ((q ^ (lane & 7)) << 4));
-            v[4 * q] += t4.x;
-            v[4 * q + 1] += t4.y;
-            v[4 * q + 2] += t4.z;
-            v[4 * q + 3] += t4.w;
-          }
-        }
-        const int ocol0 = n_tile * BN + c * 32;
-        if (ocol0 < n_lim) emit(v, ocol0, n_tile, 0, k ? rw1 : rw0, csplit * lgs_per + lgsub, true, false, k ? r1 : r0);
-      }
-      if (p.stats) flush_stats(m_tile, n_tile);
-    }
-  }
-
-  if (warp >= 2 && warp < B_WARP) {
+  if (warp < EPI_WARPS) {
     // smem may be released once the bulk stores have READ it; their global writes complete with the grid
     if (lane == 0) tma_store_wait_read<0>();
-    if (threadIdx.x == 64) SDB_TR(7, clock64() - clk0);
+    if (threadIdx.x == 0) SDB_TR(7, clock64() - clk0);
   }
-  tc_fence_before();
   __syncwarp();
-  if (clustered) cluster_sync_all();   // the peer's tensor-core reads of this CTA's shared memory / remote arrives are done
-  else __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    if (CG == 2) tmem_dealloc_cg2(tmem_d, TMEM_COLS);
-    else tmem_dealloc(tmem_d, TMEM_COLS);
-  }
+  if (clustered) cluster_sync_all();   // the peer's multicast writes / remote arrives into this CTA are done
   if (threadIdx.x == 0) SDB_TR(1, gtimer());
 }
 
@@ -1388,24 +1089,18 @@ static __global__ void __launch_bounds__(256) splitk_epilogue_scalar_kernel(cons
   }
 }
 
-template <int BN, int CG, bool DEEP, int KIND>
-static int launch_gemm_cfg(const TmapPack& tm, const GemmArgs& p, cudaStream_t st) {
-  using Cfg = GemmCfg<BN, CG, DEEP>;
-  auto kern = gemm_tc_kernel<BN, CG, DEEP, KIND>;
+// one CTA per tile (and K slice); CTA pairs and cluster split-K launch as thread-block clusters
+template <int BN, int CG, int KIND>
+static int launch_gemm(const TmapPack& tm, const GemmArgs& p, cudaStream_t st) {
+  using Cfg = GemmCfg<BN, CG>;
+  auto kern = gemm_tc_kernel<BN, CG, KIND>;
   static bool configured = false;
   if (!configured) {
     SDB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM));
     configured = true;
   }
-  const int units = p.m_units * p.n_tiles * p.splits;
-  int grid, cluster = 1;
-  if (p.csk) {
-    cluster = p.splits * CG;
-    grid = p.m_units * p.n_tiles * cluster;
-  } else {
-    cluster = CG;
-    grid = std::min(units, sm_count() / CG) * CG;
-  }
+  const int grid = p.m_units * p.n_tiles * p.splits * CG;
+  const int cluster = p.csk ? p.splits * CG : CG;
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(grid);
   cfg.blockDim = dim3(GEMM_THREADS);
@@ -1431,20 +1126,6 @@ static int launch_gemm_cfg(const TmapPack& tm, const GemmArgs& p, cudaStream_t s
   SDB_LAUNCH_CHECK();
   return 0;
 }
-
-// one tile per CTA (all of them resident at once, or cluster split-K) -> the deep-pipeline instantiation
-template <int BN, int CG, int KIND>
-static int launch_gemm(const TmapPack& tm, const GemmArgs& p, cudaStream_t st) {
-  const int units = p.m_units * p.n_tiles * p.splits;
-  const bool deep = p.csk || units <= sm_count() / CG;
-  if constexpr (KIND == 3) {
-    SDB_CHECK(deep, "sdb_gemm: cluster split-K launches are single-tile");
-    return launch_gemm_cfg<BN, CG, true, KIND>(tm, p, st);
-  } else {
-    return deep ? launch_gemm_cfg<BN, CG, true, KIND>(tm, p, st) : launch_gemm_cfg<BN, CG, false, KIND>(tm, p, st);
-  }
-}
-
 
 // all tile shapes of one KIND (one translation unit per KIND: gemm_k0.cu, gemm_k1.cu, gemm_k2.cu)
 template <int KIND>

@@ -75,9 +75,10 @@ static bool choice_valid(const sdb_gemm_desc* d, const Geometry& g, const Choice
   return true;
 }
 
-// Tile model used to pick (block_n, CTA pair, split-K). These GEMMs are bound by L2 -> SM operand traffic (chip-wide
-// ~4600 B/clk, ~64 B/clk per SM), by the tensor pipe (2*bn clk per 64-deep K step of a 128-row CTA tile) and by fixed
-// per-launch cost; a CTA pair halves the B bytes per CTA, split-K keeps tiles large at small M.
+// Tile model used to pick (block_n, CTA pair, split-K). Every CTA computes one tile with its main loop and epilogue in
+// sequence, one CTA per SM, so a launch is waves of (main loop + epilogue + pipeline fill). A main loop is bound by the
+// tensor pipe (4*bn clk per 64-deep K step of a 128-row tile on an H100 SM) or by L2 -> SM operand traffic (~64 B/clk
+// per SM, ~3000 B/clk chip-wide); a CTA pair halves the B bytes per CTA, split-K keeps tiles large at small M.
 static double choice_cost(const sdb_gemm_desc* d, const Geometry& g, const Choice& c) {
   const int sms = sm_count();
   const long nt = (d->n + c.bn - 1) / c.bn;
@@ -88,13 +89,10 @@ static double choice_cost(const sdb_gemm_desc* d, const Geometry& g, const Choic
   const double stage_bytes = 16384.0 + (c.bn / c.cg) * 128.0;
   long slots = c.csk ? std::max(1, sms / (c.splits * c.cg)) * (c.splits * c.cg) : (sms / c.cg) * c.cg;
   const long rounds = (ctas + slots - 1) / slots;
-  const double cta_iters = static_cast<double>(iters) * rounds;
-  const double t_mma = cta_iters * 2.0 * c.bn;
-  const double t_l2_cta = cta_iters * stage_bytes / 64.0;
-  const double t_l2_chip = static_cast<double>(ctas) * iters * stage_bytes / 4600.0;
-  double t = std::max(t_mma, std::max(t_l2_cta, t_l2_chip));
-  t += 1800.0 + 14.0 * c.bn;                    // epilogue of the last tile (not overlapped)
-  t += 7000.0;                                  // launch, prologue, pipeline fill
+  const double t_tile = std::max(iters * 4.0 * c.bn, iters * stage_bytes / 64.0) + 1800.0 + 14.0 * c.bn + 3000.0;
+  const double t_l2_chip = static_cast<double>(ctas) * iters * stage_bytes / 3000.0;
+  double t = std::max(rounds * t_tile, t_l2_chip);
+  t += 4000.0;                                  // launch
   if (c.csk) t += 2500.0 + 128.0 * c.bn * 4.0 * (c.splits - 1) / c.splits / 20.0;
   else if (c.splits > 1) t += 14000.0 + 8.0 * c.splits * g.M * d->n / (sms * 256.0);
   const long pad = nt * c.bn - d->n;             // zero-padded columns still cost MMA + B traffic
@@ -339,7 +337,7 @@ extern "C" int sdb_gemm(const sdb_gemm_desc* d, sdb_stream_t stream) {
     uint64_t K = static_cast<uint64_t>(d->taps) * ctot;
     uint64_t dims[2] = {K, static_cast<uint64_t>(d->n)};
     uint64_t str[1] = {K * 2};
-    uint32_t box[2] = {64, static_cast<uint32_t>(bn / ch.cg)};   // a CTA of a pair loads half of the weight tile
+    uint32_t box[2] = {64, static_cast<uint32_t>(bn / ch.cg)};   // a CTA of a pair loads (and multicasts) half of the weight tile
     if (make_tmap_f16(&tm.b, d->b, 2, dims, str, box)) return 1;
   }
   // output maps for the TMA-store epilogue (fast path); otherwise the scalar transposed path is used
@@ -353,8 +351,6 @@ extern "C" int sdb_gemm(const sdb_gemm_desc* d, sdb_stream_t stream) {
   tm.o16 = tm.b;
   tm.o16lo = tm.b;
   tm.ows = tm.b;
-  tm.res = tm.b;
-  p.res_tma = 0;
   if (fast) {
     const uint32_t bnn = static_cast<uint32_t>(32 / (p.bw * p.bh));
     auto make_out = [&](CUtensorMap* m, const void* base, int elem, int ncols, long ld, int nsplit) -> int {
@@ -386,10 +382,6 @@ extern "C" int sdb_gemm(const sdb_gemm_desc* d, sdb_stream_t stream) {
     if (p.out_f32 && make_out(&tm.o32, p.out_f32, 4, n_out, p.ldo, 1)) return 1;
     if (p.out_f16 && make_out(&tm.o16, p.out_f16, 2, n_out, p.ldo, 1)) return 1;
     if (p.out_f16_lo && make_out(&tm.o16lo, p.out_f16_lo, 2, n_out, p.ldo, 1)) return 1;
-    if (p.residual && !geglu) {
-      if (make_out(&tm.res, p.residual, 4, d->n, p.ldr, 1)) return 1;
-      p.res_tma = 1;
-    }
   }
   // fused GroupNorm statistics: per-tile partial sums of the fp32 output, stored by the epilogue
   p.stats = nullptr;

@@ -1,6 +1,6 @@
 """Tensor-level wrappers over the C ABI: PyTorch tensors in/out (device memory + current stream only).
 
-Every function enqueues hand-written sm_100a kernels from libsdb200.so on the current CUDA stream; none of
+Every function enqueues hand-written sm_90a kernels from libsdb200.so on the current CUDA stream; none of
 them computes with torch. Shapes follow the engine's layouts: activations NHWC, fp32 residual stream,
 fp16 tensor-core operands.
 """
@@ -234,7 +234,7 @@ def _tune_gemm(d, M, n, rps, stats_ok, stats_group):
                 if mode == 1 and not d.workspace:
                     continue
                 tiles = ((M + 127) // 128) * ((n + bn - 1) // bn) * sp
-                if sp > 1 and tiles > 3 * 148:
+                if sp > 1 and tiles > 3 * lib.sdb_sm_count():
                     continue
                 d.block_n, d.pair, d.splits, d.splitk_mode = bn, cg, sp, mode
                 if lib.sdb_gemm_plan(C.byref(d), plan) != 0:

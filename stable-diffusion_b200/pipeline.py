@@ -1,5 +1,5 @@
 """Script-level call sequences of the reference (scripts/txt2img.py:289-327, scripts/img2img.py:225-270) as callable
-pipelines over the B200 engine: conditioning -> sampler -> first-stage decode -> uint8 image.
+pipelines over the H100 engine: conditioning -> sampler -> first-stage decode -> uint8 image.
 
 Inputs are token ids (the tokenizer vocabulary is a host-side, third-party asset; see clip.py) and, optionally, the
 start noise x_T so results do not depend on batch size or world size (SURVEY.md Appendix D).
@@ -19,7 +19,7 @@ V1_PARAMS = dict(linear_start=0.00085, linear_end=0.0120, num_timesteps_cond=1, 
 
 def v1_model_config(unet_cfg=None, vae_cfg=None, clip_cfg=None):
     """The `model:` node of configs/stable-diffusion/v1-inference.yaml as a dict, with the reference's target names
-    (sdb200.checkpoint / LatentDiffusion map them onto the B200 classes)."""
+    (sdb200.checkpoint / LatentDiffusion map them onto the sdb200 classes)."""
     return {"target": "ldm.models.diffusion.ddpm.LatentDiffusion", "params": dict(
         V1_PARAMS,
         unet_config={"target": "ldm.modules.diffusionmodules.openaimodel.UNetModel", "params": dict(unet_cfg or arch.SD_V1_UNET)},

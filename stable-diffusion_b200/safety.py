@@ -1,11 +1,11 @@
-"""B200-native safety checker: drop-in for what `scripts/txt2img.py:26-29, 88-95` builds from third-party packages -
+"""H100-native safety checker: drop-in for what `scripts/txt2img.py:26-29, 88-95` builds from third-party packages -
 transformers' CLIPFeatureExtractor (`safety_feature_extractor`) and diffusers' StableDiffusionSafetyChecker
 (`safety_checker`): `check_safety(x_image)` -> (x_checked_image, has_nsfw_concept).
 
 Everything runs on the GPU, on the same kernel family as the UNet: PIL's 8-bit bicubic resample restated in its own
 fixed-point arithmetic (sdb_resample_u8; the coefficient tables are computed on the host as PIL's precompute_coeffs
-does), normalisation, ViT patch extraction, the CLIP ViT-L/14 vision tower (fp32 LayerNorm -> fp16 operands, tcgen05
-GEMMs with fused bias / quick-GELU / residual epilogues, tcgen05 attention), the visual projection and the concept
+does), normalisation, ViT patch extraction, the CLIP ViT-L/14 vision tower (fp32 LayerNorm -> fp16 operands, wgmma
+GEMMs with fused bias / quick-GELU / residual epilogues, wgmma attention), the visual projection and the concept
 decision (sdb_safety_scores). State-dict keys are diffusers' (`vision_model.vision_model.*`, `visual_projection.weight`,
 `concept_embeds`, `special_care_embeds`, `*_weights`). There is no CPU fallback.
 """

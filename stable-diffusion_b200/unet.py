@@ -1,8 +1,8 @@
-"""B200-native UNet for the SD-v1 denoising loop: drop-in for the reference's
+"""H100-native UNet for the SD-v1 denoising loop: drop-in for the reference's
 `ldm.modules.diffusionmodules.openaimodel.UNetModel` (constructor kwargs openaimodel.py:443-469,
 `forward(x, timesteps, context)` openaimodel.py:710-742, state-dict keys unchanged).
 
-Nothing here computes with torch: forward() only sequences the hand-written sm_100a kernels of libsdb200.so
+Nothing here computes with torch: forward() only sequences the hand-written sm_90a kernels of libsdb200.so
 (ops.py). torch provides device memory and the current stream. nn.Module is used solely so that the reference's
 `load_state_dict` / `instantiate_from_config` plumbing (ldm/util.py:78-93, scripts/txt2img.py:49-66) sees this
 object; there are no nn layers and no parameters.
@@ -94,7 +94,7 @@ class UNetModel(nn.Module):
             context_dim = list(context_dim) if isinstance(context_dim, (list, tuple)) else context_dim
         if num_heads == -1:
             assert num_head_channels != -1, "Either num_heads or num_head_channels has to be set"
-        # the B200 path covers the configuration SD v1 ships (v1-inference.yaml:29-44)
+        # the sdb200 path covers the configuration SD v1 ships (v1-inference.yaml:29-44)
         unsupported = dict(dims=dims != 2, num_classes=num_classes is not None, resblock_updown=resblock_updown,
                            use_scale_shift_norm=use_scale_shift_norm, n_embed=n_embed is not None,
                            no_spatial_transformer=not use_spatial_transformer, transformer_depth=transformer_depth != 1,
@@ -512,7 +512,7 @@ class UNetModel(nn.Module):
         assert y is None, "must specify y if and only if the model is class-conditional"
         assert self.W is not None, "weights not loaded (load_state_dict / load_weights, then .cuda())"
         if not x.is_cuda:
-            raise RuntimeError("sdb200.UNetModel runs on CUDA (sm_100a) only; there is no CPU fallback")
+            raise RuntimeError("sdb200.UNetModel runs on CUDA (sm_90a) only; there is no CPU fallback")
         assert x.dim() == 4 and x.shape[1] == self.in_channels
         assert context is not None and context.shape[0] == x.shape[0] and context.shape[2] == self.context_dim
         nb, _, H, Wd = x.shape

@@ -19,7 +19,7 @@ def instantiate_from_config(config):
     return get_obj_from_str(config["target"])(**config.get("params", dict()))
 
 
-# reference targets -> B200 engine classes (used by LatentDiffusion when handed an unmodified reference config)
+# reference targets -> sdb200 engine classes (used by LatentDiffusion when handed an unmodified reference config)
 TARGET_MAP = {
     "ldm.models.diffusion.ddpm.LatentDiffusion": "sdb200.diffusion.LatentDiffusion",
     "ldm.modules.diffusionmodules.openaimodel.UNetModel": "sdb200.unet.UNetModel",

@@ -1,10 +1,9 @@
-"""B200-native AutoencoderKL (SD first stage): drop-in for `ldm.models.autoencoder.AutoencoderKL`
+"""H100-native AutoencoderKL (SD first stage): drop-in for `ldm.models.autoencoder.AutoencoderKL`
 (`encode(x) -> posterior`, `decode(z) -> image`; autoencoder.py:285-333) over the VAE Encoder/Decoder of
 ldm/modules/diffusionmodules/model.py:368-568. State-dict keys unchanged (`encoder.*`, `decoder.*`, `quant_conv.*`,
-`post_quant_conv.*`). Same kernels as the UNet: tcgen05 implicit-GEMM convs, fp32 GroupNorm (eps 1e-6) + SiLU
+`post_quant_conv.*`). Same kernels as the UNet: wgmma implicit-GEMM convs, fp32 GroupNorm (eps 1e-6) + SiLU
 producing the fp16 operand, fp32 residual stream. The single-head mid-block attention (c=512, N=h*w;
-model.py:178-202) runs as QK^T GEMM -> fp32 row softmax -> PV GEMM per image (head dim 512 exceeds the flash
-kernel's TMEM budget), with the value bias folded through proj_out (softmax rows sum to 1).
+model.py:178-202) runs in the d = 512 flash kernel (sdb_attention, dpad 512; other widths: QK^T GEMM -> fp32 row softmax -> PV GEMM per image), with the value bias folded through proj_out (softmax rows sum to 1).
 """
 from __future__ import annotations
 

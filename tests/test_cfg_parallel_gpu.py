@@ -1,4 +1,4 @@
-"""CFG-parallel latency mode (SURVEY 8f-2) on two B200s: the guidance halves of every UNet evaluation run on two
+"""CFG-parallel latency mode (SURVEY 8f-2) on two GPUs: the guidance halves of every UNet evaluation run on two
 GPUs and meet in the fused step kernel (NCCL all_gather, or peer loads over NVLink inside the kernel). Both ranks must
 end with identical latents that match the reference PLMS / DPM-Solver outputs like the single-GPU path does.
 Skipped on boxes with fewer than two GPUs (`gpurun --gpus 2 -- python -m pytest tests/test_cfg_parallel_gpu.py`)."""

@@ -1,4 +1,4 @@
-"""Checkpoint ingest on the B200: a reference-format checkpoint (fp16 safetensors and pickled .ckpt) loaded through
+"""Checkpoint ingest on the H100: a reference-format checkpoint (fp16 safetensors and pickled .ckpt) loaded through
 `load_model_from_config` evaluates like the oracle on the very tensors the file holds."""
 import pytest
 import torch

@@ -119,7 +119,7 @@ def _check_stats(o32, nb, rps, n):
     (256, 512, 128, 256, 1), (4096, 320, 960, 160, 10), (384, 320, 64, 160, 2),
 ])
 def test_gemm_cta_pair(S, cuda_dev, M, N, K, bn, sg):
-    """cta_group::2: two CTAs per 256 x block_n tile, each loading half of the weight tile (odd tile counts included)."""
+    """CTA pairs: two CTAs per 256 x block_n tile, each loading half of the weight tile (odd tile counts included)."""
     g = torch.Generator().manual_seed(M + N + K)
     a = _rand16((M, K), cuda_dev, g)
     b = _rand16((N, K), cuda_dev, g, K ** -0.5)
@@ -410,7 +410,7 @@ def test_gemm_hilo_split_recovers_fp32_operands(S, cuda_dev):
 
 
 def test_gemm_many_tiles_persistent(S, cuda_dev):
-    """More tiles than SMs: every persistent CTA walks several tiles through both TMEM accumulators."""
+    """More tiles than SMs: several waves of one-tile CTAs."""
     g = torch.Generator().manual_seed(22)
     for (M, N, K, bn) in [(128 * 40, 1280, 192, 128), (128 * 37 + 5, 640, 320, 64), (128 * 9, 2560, 128, 256),
                           (4096, 4096, 512, 0)]:
@@ -424,7 +424,7 @@ def test_gemm_many_tiles_persistent(S, cuda_dev):
 
 
 def test_gemm_narrow_tiles_many_per_cta(S, cuda_dev):
-    """block_n 32/64 with more than two tiles per persistent CTA (accumulator hand-off with idle epilogue warps)."""
+    """block_n 32/64 with many more tiles than SMs (and a scalar-store width)."""
     g = torch.Generator().manual_seed(23)
     for (M, N, K, bn) in [(128 * 500, 32, 128, 32), (128 * 300, 96, 64, 32), (128 * 450, 64, 192, 64), (128 * 700, 3, 128, 0)]:
         a = _rand16((M, K), cuda_dev, g)

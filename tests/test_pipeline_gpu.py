@@ -1,4 +1,4 @@
-"""Samplers and the LatentDiffusion facade on the B200 against the reference (golden) and the oracle."""
+"""Samplers and the LatentDiffusion facade on the H100 against the reference (golden) and the oracle."""
 import numpy as np
 import pytest
 import torch

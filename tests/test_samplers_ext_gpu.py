@@ -1,4 +1,4 @@
-"""SURVEY 8(f) rows on the B200: DPM-Solver++ sampler and the inpainting (mask) branch of PLMS / DDIM — the fused
+"""SURVEY 8(f) rows on the H100: DPM-Solver++ sampler and the inpainting (mask) branch of PLMS / DDIM — the fused
 step kernels bit for bit against the oracle on replayed eps, and the whole loop on the tiny model against the
 reference's own outputs (tests/golden/samplers_ext.pt)."""
 import pytest
@@ -93,7 +93,7 @@ def test_mask_blend_full_channel_mask(cuda_dev):
 
 
 def test_dpm_solver_and_inpainting_vs_reference_tiny(cuda_dev):
-    """Whole loops on the tiny LatentDiffusion (B200 UNet) against the reference run: fp16-operand error accumulated
+    """Whole loops on the tiny LatentDiffusion (sdb200 UNet) against the reference run: fp16-operand error accumulated
     over the trajectory, same bounds as the PLMS / DDIM rows in test_pipeline_gpu.py."""
     import sdb200
     g = golden("samplers_ext.pt")

@@ -1,4 +1,4 @@
-"""eps parity of the B200 UNet against the reference's outputs (golden fixtures from the unmodified reference)
+"""eps parity of the sdb200 UNet against the reference's outputs (golden fixtures from the unmodified reference)
 and against the oracle on fresh seeded inputs. Tolerance: north_star's 1e-3 rel-L2 (fp16 operands, fp32 accumulate)."""
 import pytest
 import torch

@@ -1,4 +1,4 @@
-"""AutoencoderKL decode/encode and CLIP text encoder on the B200 against the reference's outputs (golden fixtures)."""
+"""AutoencoderKL decode/encode and CLIP text encoder on the H100 against the reference's outputs (golden fixtures)."""
 import pytest
 import torch
 
