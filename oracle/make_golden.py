@@ -330,10 +330,70 @@ def fullsize_goldens():
     save("fullsize.pt", out)
 
 
+@torch.no_grad()
+def nonsquare_goldens():
+    """Non-square latents from the UNMODIFIED reference: every other fixture is square, so a swapped H/W axis or a
+    transposed tile walk could cancel out there. SD-v1 (2,4,24,40) walks 24x40 -> 12x20 -> 6x10 -> 3x5 (60 tokens at
+    the third level), (1,4,8,64) reaches a 1x8 deepest level. Contexts are regenerated from their seeds by the tests
+    (gen(shape, ctx_seed)); everything else is stored."""
+    out = dict(unet=[], vae=[])
+    for tag, cfg, shapes in (
+        ("tiny", arch.TINY_UNET, [((2, 4, 8, 24), [981, 1]), ((3, 4, 24, 16), [500, 21, 981])]),
+        ("sdv1", arch.SD_V1_UNET, [((2, 4, 24, 40), [981, 261]), ((1, 4, 8, 64), [501])]),
+    ):
+        sd = arch.random_state_dict(arch.unet_param_shapes(cfg), UNET_SEED)
+        net = R.build_unet(cfg)
+        net.load_state_dict(sd, strict=True)
+        for i, (xs, ts) in enumerate(shapes):
+            x = gen(xs, 700 + i)
+            t = torch.tensor(ts, dtype=torch.long)
+            ctx_seed = 710 + i
+            ctx = gen((xs[0], 77, cfg["context_dim"]), ctx_seed)
+            eps = net(x, t, context=ctx)
+            mine = O.unet_forward(sd, x, t, ctx, num_heads=cfg["num_heads"])
+            print(f"nonsquare unet {tag} {xs} t={ts}: eps std {float(eps.std()):.3f}  oracle rel-L2 {rel(mine, eps):.2e}")
+            out["unet"].append(dict(cfg=tag, x=x, t=t, ctx_seed=ctx_seed, eps=eps, seed=UNET_SEED))
+        del net
+    for tag, cfg, zshape, ishape in (("tiny", arch.TINY_VAE, (2, 4, 8, 12), (2, 3, 32, 48)),
+                                     ("sdv1", arch.SD_V1_VAE, (1, 4, 8, 12), (1, 3, 96, 64))):
+        sd = arch.random_state_dict(arch.vae_param_shapes(cfg), VAE_SEED)
+        vae = R.build_vae(cfg)
+        vae.load_state_dict(sd, strict=True)
+        z = gen(zshape, 720)
+        img = gen(ishape, 721).clamp(-1, 1)
+        dec = vae.decode(z)
+        raw_moments = vae.quant_conv(vae.encoder(img))
+        print(f"nonsquare vae {tag} z {zshape} img {ishape}: decode oracle rel {rel(O.vae_decode(sd, z), dec):.2e}; "
+              f"encode oracle rel {rel(O.vae_encode_moments(sd, img), raw_moments):.2e}")
+        out["vae"].append(dict(cfg=tag, z=z, img=img, dec=dec, moments=raw_moments, seed=VAE_SEED))
+    # PLMS S=10, CFG 7.5 through the reference's LatentDiffusion facade at a 8x24 latent, then decode_first_stage
+    import contextlib
+    import io
+    ld = R.build_latent_diffusion(arch.TINY_UNET, arch.TINY_VAE)
+    usd = arch.random_state_dict(arch.unet_param_shapes(arch.TINY_UNET), UNET_SEED)
+    vsd = arch.random_state_dict(arch.vae_param_shapes(arch.TINY_VAE), VAE_SEED)
+    ld.model.diffusion_model.load_state_dict(usd, strict=True)
+    ld.first_stage_model.load_state_dict(vsd, strict=True)
+    plms, _ = R.build_samplers(ld)
+    B, shape = 2, [4, 8, 24]
+    c, uc, x_T = gen((B, 77, 64), 730), gen((B, 77, 64), 731), gen((B, *shape), 732)
+    buf = io.StringIO()
+    with contextlib.redirect_stdout(buf), contextlib.redirect_stderr(buf):
+        s_plms, _ = plms.sample(S=10, conditioning=c, batch_size=B, shape=shape, verbose=False,
+                                unconditional_guidance_scale=7.5, unconditional_conditioning=uc, eta=0.0, x_T=x_T)
+    x_dec = ld.decode_first_stage(s_plms)
+    model_fn = lambda x, t, cc: O.unet_forward(usd, x, t, cc, num_heads=arch.TINY_UNET["num_heads"])
+    mine = O.plms_sample(model_fn, x_T, c, uc, 7.5, S=10)
+    print(f"nonsquare plms S=10 latent {tuple(x_T.shape)}: oracle rel {rel(mine, s_plms):.2e}; "
+          f"decode_first_stage oracle rel {rel(O.decode_first_stage(vsd, s_plms), x_dec):.2e}")
+    out["pipeline"] = dict(c=c, uc=uc, x_T=x_T, plms10=s_plms, x_dec=x_dec, unet_seed=UNET_SEED, vae_seed=VAE_SEED)
+    save("nonsquare.pt", out)
+
+
 if __name__ == "__main__":
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(os.cpu_count())
-    which = sys.argv[1:] or ["unet", "vae", "pipeline", "clip", "samplers_ext", "safety"]
+    which = sys.argv[1:] or ["unet", "vae", "pipeline", "clip", "samplers_ext", "safety", "nonsquare"]
     if "unet" in which:
         unet_goldens()
     if "vae" in which:
@@ -348,3 +408,5 @@ if __name__ == "__main__":
         samplers_ext_goldens()
     if "fullsize" in which:   # slow (minutes, ~20 GB of host memory): not part of the default set
         fullsize_goldens()
+    if "nonsquare" in which:
+        nonsquare_goldens()

@@ -207,7 +207,12 @@ class AutoencoderKL(nn.Module):
             p = ops.softmax_rows(s, float(int(c) ** -0.5))
             if npad != n:
                 raise NotImplementedError("VAE attention needs h*w % 8 == 0")
-            ops.gemm(p, vt.contiguous(), out_f16=o[b], b_dynamic=True)
+            vt = vt.contiguous()
+            if n % 64:   # the token axis is the K of P . V: zero-pad it to the GEMM's 64-wide K step (e.g. 8x12 = 96)
+                kp = (n + 63) // 64 * 64
+                p = torch.nn.functional.pad(p, (0, kp - n))
+                vt = torch.nn.functional.pad(vt, (0, kp - n))
+            ops.gemm(p, vt, out_f16=o[b], b_dynamic=True)
         _, out = ops.gemm(o.view(-1, c), a["w_o"], bias=a["b_o"], residual=x.view(-1, c), want_f32=True,
                           rows_per_sample=n, want_stats=True, stats_group=_sg(c))
         return out.view(nb, H, Wd, c)

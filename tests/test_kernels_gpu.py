@@ -488,3 +488,281 @@ def test_c_abi_rejects_bad_arguments(S, cuda_dev):
                         nq=64, nkv=64, scale=1.0)
     with pytest.raises(RuntimeError, match="GEGLU"):
         S.ops.gemm(a, torch.zeros(96, 64, dtype=torch.float16, device=cuda_dev), act=S.ops.ACT_GEGLU, want_f16=True)
+
+
+# ------------------------------------------------------------------------------------------------ non-square geometry
+# Every model runs non-square latents (512x768 is the most common SD v1 size), and the 3x3-conv path treats the two axes
+# differently: the tile is TW x TH x TN output pixels with TW = largest power of two dividing w (<= 128), TH = largest
+# power of two dividing h (<= 128 / TW), TN = 128 / (TW * TH) samples. A swapped axis or a transposed tile walk can cancel
+# out in a square test, so each test below also checks that its comparison can tell H from W: the result must be far
+# from the H/W-transposed reference (the same op on the transposed image, read back in the untransposed layout).
+def _tile_geometry(h, w):
+    p2 = lambda v, cap: max(q for q in (1, 2, 4, 8, 16, 32, 64, 128) if q <= cap and v % q == 0)
+    tw = p2(w, 128)
+    th = p2(h, 128 // tw)
+    return tw, th, 128 // (tw * th)
+
+
+def _conv_ref(x, wt, bias, stride=1, shift=0, transposed=False):
+    """fp64 3x3 conv of NHWC fp16 x -> [nb*ho*wo, n] rows in NHWC order. transposed=True: the conv of the H/W-transposed
+    image, laid out as (nb, wo, ho, n) and read back as rows."""
+    xin = x.double().permute(0, 3, 1, 2)
+    if transposed:
+        xin = xin.transpose(2, 3)
+    if shift:
+        ref = F.conv2d(F.pad(xin, (0, 1, 0, 1)), wt.double(), bias.double(), stride=2, padding=0)
+    else:
+        ref = F.conv2d(xin, wt.double(), bias.double(), stride=stride, padding=1)
+    return ref.permute(0, 2, 3, 1).reshape(-1, wt.shape[0])
+
+
+def _stats_expected(h, w):
+    """Tile classes whose conv epilogue can produce fused GroupNorm statistics (gemm_tc.cu stats_slots)."""
+    tw, th, tn = _tile_geometry(h, w)
+    return tn == 1 or (tw * th == 64 and tn == 2)
+
+
+NONSQUARE = [(2, 64, 96), (2, 96, 64), (2, 8, 12), (2, 12, 8), (2, 5, 7), (3, 7, 5), (2, 1, 16), (2, 16, 1), (1, 10, 14),
+             (2, 3, 128), (3, 4, 16), (3, 16, 4), (2, 24, 40), (2, 3, 5), (1, 1, 8)]
+
+
+@pytest.mark.parametrize("nb,h,w", NONSQUARE)
+def test_conv3x3_nonsquare_fused_epilogue(S, cuda_dev, nb, h, w):
+    """Stride-1 3x3 conv over every (TW, TH, TN) tile class in both orientations, with the full fused epilogue of
+    UNetModel._res: bias, FiLM as a strided column slice of the wider all-ResBlocks FiLM matrix, residual, fp16 + fp32
+    outputs and the fused statistics (where the tile class grants them)."""
+    c, n, sg = 64, 160, 5
+    g = torch.Generator().manual_seed(nb * 1000 + h * 37 + w)
+    x = _rand16((nb, h, w, c), cuda_dev, g)
+    wt = _rand16((n, c, 3, 3), cuda_dev, g, (9 * c) ** -0.5)
+    bias = torch.randn(n, generator=g).to(cuda_dev)
+    film_all = torch.randn(nb, n + 96, generator=g).to(cuda_dev)
+    film = film_all[:, 32: 32 + n]                     # ldf = n + 96, as UNetModel._res slices the FiLM matrix
+    res = torch.randn(nb * h * w, n, generator=g).to(cuda_dev)
+    wk = wt.permute(0, 2, 3, 1).reshape(n, 9 * c).contiguous()
+    o16, o32 = S.ops.gemm(x, wk, taps=9, bias=bias, film=film, residual=res, want_f32=True, want_f16=True,
+                          want_stats=True, stats_group=sg)
+    torch.cuda.synchronize()
+    add = film.double().cpu().repeat_interleave(h * w, 0) + res.double().cpu()
+    ref = _conv_ref(x.cpu(), wt.cpu(), bias.cpu()) + add
+    ref_t = _conv_ref(x.cpu(), wt.cpu(), bias.cpu(), transposed=True) + add
+    assert rel_l2(o32.cpu(), ref) < 1e-5, rel_l2(o32.cpu(), ref)
+    assert rel_l2(o16.float().cpu(), ref) < 6e-4
+    assert rel_l2(o32.cpu(), ref_t) > 0.1
+    assert hasattr(o32, "_sdb_stats") == _stats_expected(h, w), _tile_geometry(h, w)
+    if hasattr(o32, "_sdb_stats"):
+        _check_stats(o32, nb, h * w, n)
+
+
+@pytest.mark.parametrize("nb,h,w,c,n", [
+    (2, 12, 8, 64, 128), (2, 8, 12, 64, 128), (2, 9, 14, 64, 64), (2, 14, 9, 64, 64), (3, 7, 5, 64, 96),
+    (2, 5, 7, 128, 64), (2, 10, 34, 64, 64), (2, 34, 10, 64, 64), (2, 2, 32, 64, 64), (2, 48, 80, 128, 128),
+])
+@pytest.mark.parametrize("shift", [0, 1])
+def test_conv3x3_stride2_nonsquare(S, cuda_dev, nb, h, w, c, n, shift):
+    """Stride-2 convs (strided 2*TW x 2*TH input box) on odd and even non-square inputs, symmetric pad (shift 0) and the
+    VAE's pad-right/bottom variant (shift 1), with bias + FiLM + residual."""
+    g = torch.Generator().manual_seed(nb * 17 + h * 5 + w + c + shift)
+    x = _rand16((nb, h, w, c), cuda_dev, g)
+    wt = _rand16((n, c, 3, 3), cuda_dev, g, (9 * c) ** -0.5)
+    bias = torch.randn(n, generator=g).to(cuda_dev)
+    ho, wo = (h + 1 - shift) // 2, (w + 1 - shift) // 2
+    film = torch.randn(nb, n, generator=g).to(cuda_dev)
+    res = torch.randn(nb * ho * wo, n, generator=g).to(cuda_dev)
+    wk = wt.permute(0, 2, 3, 1).reshape(n, 9 * c).contiguous()
+    _, o32 = S.ops.gemm(x, wk, taps=9, conv_stride=2, conv_shift=shift, bias=bias, film=film, residual=res,
+                        want_f32=True, splits=-1)
+    torch.cuda.synchronize()
+    assert o32.shape == (nb * ho * wo, n)
+    add = film.double().cpu().repeat_interleave(ho * wo, 0) + res.double().cpu()
+    ref = _conv_ref(x.cpu(), wt.cpu(), bias.cpu(), stride=2, shift=shift) + add
+    ref_t = _conv_ref(x.cpu(), wt.cpu(), bias.cpu(), stride=2, shift=shift, transposed=True) + add
+    assert rel_l2(o32.cpu(), ref) < 1e-5, rel_l2(o32.cpu(), ref)
+    assert rel_l2(o32.cpu(), ref_t) > 0.1
+
+
+@pytest.mark.parametrize("nb,h,w,c,n,bn,pair,sp,mode", [
+    (2, 64, 96, 128, 256, 128, 2, 1, 0),     # CTA pair, TN = 1
+    (2, 96, 64, 128, 320, 160, 2, 2, 2),     # CTA pair + cluster split-K, TN = 1 (statistics per K slice)
+    (2, 12, 8, 320, 640, 160, 1, 4, 2),      # cluster split-K, TN = 4
+    (3, 7, 5, 128, 256, 128, 2, 2, 2),       # CTA pair + cluster split-K, TN = 128
+    (3, 16, 4, 128, 256, 128, 2, 1, 0),      # CTA pair, two-sample 64-pixel tiles
+    (2, 8, 12, 320, 640, 0, 1, 3, 1),        # workspace split-K (second kernel)
+    (2, 24, 40, 128, 320, 0, 1, 4, 1),       # workspace split-K, TN = 1
+])
+def test_conv3x3_nonsquare_pair_and_splitk(S, cuda_dev, nb, h, w, c, n, bn, pair, sp, mode):
+    g = torch.Generator().manual_seed(nb * 131 + h * 7 + w + c + sp)
+    x = _rand16((nb, h, w, c), cuda_dev, g)
+    wt = _rand16((n, c, 3, 3), cuda_dev, g, (9 * c) ** -0.5)
+    bias = torch.randn(n, generator=g).to(cuda_dev)
+    film = torch.randn(nb, n, generator=g).to(cuda_dev)
+    res = torch.randn(nb * h * w, n, generator=g).to(cuda_dev)
+    wk = wt.permute(0, 2, 3, 1).reshape(n, 9 * c).contiguous()
+    o16, o32 = S.ops.gemm(x, wk, taps=9, bias=bias, film=film, residual=res, want_f32=True, want_f16=True, block_n=bn,
+                          pair=pair, splits=sp, splitk_mode=mode, want_stats=True, stats_group=n // 32)
+    torch.cuda.synchronize()
+    add = film.double().cpu().repeat_interleave(h * w, 0) + res.double().cpu()
+    ref = _conv_ref(x.cpu(), wt.cpu(), bias.cpu()) + add
+    ref_t = _conv_ref(x.cpu(), wt.cpu(), bias.cpu(), transposed=True) + add
+    assert rel_l2(o32.cpu(), ref) < 1e-5, rel_l2(o32.cpu(), ref)
+    assert rel_l2(o16.float().cpu(), ref) < 6e-4
+    assert rel_l2(o32.cpu(), ref_t) > 0.1
+    assert hasattr(o32, "_sdb_stats") == (mode == 1 or _stats_expected(h, w)), _tile_geometry(h, w)
+    if hasattr(o32, "_sdb_stats"):
+        _check_stats(o32, nb, h * w, n)
+
+
+@pytest.mark.parametrize("nb,h,w,c,n", [(2, 64, 96, 64, 320), (2, 24, 40, 128, 320), (3, 4, 16, 64, 128),
+                                         (3, 16, 4, 64, 128), (2, 8, 16, 64, 640)])
+def test_groupnorm_nonsquare_from_fused_statistics(S, cuda_dev, nb, h, w, c, n):
+    """groupnorm() fed by the conv epilogue's per-tile statistics at h != w (one slot per spatial tile position)."""
+    g = torch.Generator().manual_seed(nb + h * 3 + w + n)
+    x = _rand16((nb, h, w, c), cuda_dev, g)
+    wt = _rand16((n, c, 3, 3), cuda_dev, g, (9 * c) ** -0.5)
+    bias = torch.randn(n, generator=g).to(cuda_dev)
+    res = (torch.randn(nb * h * w, n, generator=g) * 2 + 0.7).to(cuda_dev)
+    wk = wt.permute(0, 2, 3, 1).reshape(n, 9 * c).contiguous()
+    _, o32 = S.ops.gemm(x, wk, taps=9, bias=bias, residual=res, want_f32=True, want_stats=True, stats_group=n // 32)
+    assert S.ops.channel_stats(o32) is not None, _tile_geometry(h, w)
+    gamma = (1 + 0.1 * torch.randn(n, generator=g)).to(cuda_dev)
+    beta = (0.1 * torch.randn(n, generator=g)).to(cuda_dev)
+    y, _ = S.ops.groupnorm(o32.view(nb, h, w, n), gamma, beta, eps=1e-5, silu=True)
+    torch.cuda.synchronize()
+    gn = lambda r: F.silu(F.group_norm(r.float().reshape(nb, h, w, n).permute(0, 3, 1, 2), 32, gamma.cpu(), beta.cpu(),
+                                       1e-5)).permute(0, 2, 3, 1)
+    ref = _conv_ref(x.cpu(), wt.cpu(), bias.cpu()) + res.double().cpu()
+    ref_t = _conv_ref(x.cpu(), wt.cpu(), bias.cpu(), transposed=True) + res.double().cpu()
+    assert rel_l2(y.float().cpu(), gn(ref)) < 6e-4, rel_l2(y.float().cpu(), gn(ref))
+    assert rel_l2(y.float().cpu(), gn(ref_t)) > 0.1
+
+
+@pytest.mark.parametrize("nb,h,w,c", [(2, 8, 12, 4), (2, 12, 8, 4), (1, 5, 7, 8), (3, 16, 24, 320), (2, 1, 16, 64)])
+def test_elementwise_nonsquare(S, cuda_dev, nb, h, w, c):
+    """Layout conversion, nearest 2x upsample and im2col at h != w."""
+    g = torch.Generator().manual_seed(nb + h + w + c)
+    x = torch.randn(nb, c, h, w, generator=g).to(cuda_dev)
+    o32, o16 = S.ops.nchw_to_nhwc(x, want_f16=True)
+    assert torch.equal(o32, x.permute(0, 2, 3, 1).contiguous())
+    assert torch.equal(o16, x.permute(0, 2, 3, 1).contiguous().half())
+    assert torch.equal(S.ops.nhwc_to_nchw(o32), x)
+    xt = x.transpose(2, 3)                      # [nb, c, w, h]: the H/W-transposed image
+    if h > 1:
+        assert rel_l2(o32, xt.permute(0, 2, 3, 1).reshape(o32.shape)) > 0.1
+    up = S.ops.upsample2x(o32)
+    ref_up = F.interpolate(x, scale_factor=2, mode="nearest").permute(0, 2, 3, 1)
+    assert up.shape == (nb, 2 * h, 2 * w, c)
+    assert torch.allclose(up.float(), ref_up, atol=2e-3)
+    assert rel_l2(up.float(), F.interpolate(xt, scale_factor=2, mode="nearest").permute(0, 2, 3, 1).reshape(up.shape)) > 0.1
+    if c > 8:
+        return
+    kpad = (9 * c + 63) // 64 * 64
+    for stride, pad_lo in [(1, 1), (2, 1), (2, 0)]:
+        ho = (h + 2 * pad_lo - 3) // stride + 1 if pad_lo else (h + 1 - 3) // stride + 1
+        wo = (w + 2 * pad_lo - 3) // stride + 1 if pad_lo else (w + 1 - 3) // stride + 1
+        col = S.ops.im2col3x3(o32, stride, pad_lo, ho, wo, kpad)
+
+        def unfold(img):
+            xp = F.pad(img, (0, 1, 0, 1)) if pad_lo == 0 else F.pad(img, (1, 1, 1, 1))
+            un = F.unfold(xp, 3, stride=stride)           # [nb, c*9, L]; index c*9 + tap -> ours tap*c + ch
+            return un.reshape(nb, c, 9, -1).permute(0, 3, 2, 1).reshape(-1, 9 * c)
+        ref = unfold(x)
+        assert col.shape == (nb * ho * wo, kpad) and ref.shape[0] == col.shape[0]
+        assert torch.allclose(col[:, :9 * c].float(), ref, atol=2e-3), (stride, pad_lo)
+        assert float(col[:, 9 * c:].abs().max()) == 0.0
+        assert rel_l2(col[:, :9 * c].float(), unfold(xt)) > 0.1
+
+
+def _attn_ref_gpu(q, k, v, scale):
+    """fp64 softmax(q k^T * scale) v per batch ([B, H, n, d] fp16 on the device), for token counts whose logits would not
+    fit comfortably on the host."""
+    out = torch.empty(q.shape, dtype=torch.float64, device=q.device)
+    for b in range(q.shape[0]):
+        s = torch.einsum("hid,hjd->hij", q[b].double(), k[b].double()) * scale
+        out[b] = torch.einsum("hij,hjd->hid", s.softmax(-1), v[b].double())
+    return out
+
+
+def _heads_padded(t, dpad, fill):
+    """[B, H, n, d] -> [B, n, H*dpad] with `fill` in the head-dim padding d..dpad."""
+    B, H, n, d = t.shape
+    p = torch.full((B, n, H, dpad), fill, dtype=t.dtype, device=t.device)
+    p[..., :d] = t.permute(0, 2, 1, 3)
+    return p.reshape(B, n, H * dpad)
+
+
+@pytest.mark.parametrize("nb,ntok,d,dpad", [
+    (2, 6144, 40, 64), (2, 1536, 80, 128), (2, 384, 160, 192),       # 512x768: 64x96, 32x48, 16x24 latent levels
+    (2, 960, 40, 64), (2, 240, 80, 128), (2, 60, 160, 192),          # 192x320: 24x40, 12x20, 6x10
+    (2, 140, 160, 192), (2, 140, 40, 64), (3, 15, 160, 192),          # 10x14 and 3x5: ntok % 8 != 0
+])
+def test_attention_unet_views(S, cuda_dev, nb, ntok, d, dpad):
+    """The attention kernel through exactly the views UNetModel._st passes (unet.py, self- and cross-attention), at
+    SD v1 head widths (8 heads) and the token counts of non-square latents.
+
+    Self-attention: q / k are the column halves qk3[:, :, :hd] / qk3[:, :, hd:] of the fused [M, 2*hd] QK output; V^T is
+    the permuted view of the [hd, nb*ntok] operand-swapped GEMM output when ntok % 8 == 0, else the [nb, hd, ceil8(ntok)]
+    output of transpose_f16. Cross-attention: q [M, hd], K [nb, 77, hd] and an ld-padded V^T [nb, hd, 80].
+    The Q / K head-dim padding columns d..dpad must be zero (the packed weights have zero rows there): the kernel reads
+    them up to ceil16(d). Memory the kernel must not use holds NaN: V^T columns past nkv, the V head-dim padding
+    d..dpad, and the columns of a wider output buffer beyond heads*d."""
+    H = 8
+    hd = H * dpad
+    scale = d ** -0.5
+    g = torch.Generator().manual_seed(ntok + d)
+    rnd = lambda *s: torch.randn(*s, generator=g).half().to(cuda_dev)
+    nan = float("nan")
+    # ---- self-attention
+    q, k, v = rnd(nb, H, ntok, d), rnd(nb, H, ntok, d), rnd(nb, H, ntok, d)
+    qk = torch.cat([_heads_padded(q, dpad, 0.0), _heads_padded(k, dpad, 0.0)], -1).reshape(nb * ntok, 2 * hd)
+    qk3 = qk.view(nb, ntok, 2 * hd)
+    vp = _heads_padded(v, dpad, nan)                                         # [nb, ntok, hd], NaN head padding
+    if ntok % 8 == 0:
+        vt = vp.reshape(nb * ntok, hd).t().contiguous()                      # [hd, nb*ntok]
+        vt3 = vt.view(hd, nb, ntok).permute(1, 0, 2)
+    else:
+        ld = (ntok + 7) // 8 * 8
+        vt3 = torch.full((nb, hd, ld), nan, dtype=torch.float16, device=cuda_dev)
+        vt3[:, :, :ntok] = vp.transpose(1, 2)
+    wide = torch.full((nb, ntok, H * d + 64), nan, dtype=torch.float16, device=cuda_dev)
+    out = wide[:, :, :H * d]
+    S.ops.attention(qk3[:, :, :hd], qk3[:, :, hd:], vt3, heads=H, d=d, dpad=dpad, nq=ntok, nkv=ntok, scale=scale, out=out)
+    torch.cuda.synchronize()
+    ref = _attn_ref_gpu(q, k, v, scale).permute(0, 2, 1, 3).reshape(nb, ntok, H * d)
+    assert bool(torch.isfinite(out).all()), "NaN from memory the kernel must not read reached the output"
+    assert bool(torch.isnan(wide[:, :, H * d:]).all()), "output columns beyond heads*d were written"
+    err = rel_l2(out, ref)
+    assert err < 2e-3, err
+    # ---- cross-attention, nkv = 77
+    nkv = 77
+    q2, k2, v2 = rnd(nb, H, ntok, d), rnd(nb, H, nkv, d), rnd(nb, H, nkv, d)
+    qv = _heads_padded(q2, dpad, 0.0).reshape(nb * ntok, hd).view(nb, ntok, hd)
+    kv = _heads_padded(k2, dpad, 0.0)
+    vt2 = torch.full((nb, hd, 80), nan, dtype=torch.float16, device=cuda_dev)
+    vt2[:, :, :nkv] = _heads_padded(v2, dpad, nan).transpose(1, 2)
+    o2 = S.ops.attention(qv, kv, vt2, heads=H, d=d, dpad=dpad, nq=ntok, nkv=nkv, scale=scale)
+    torch.cuda.synchronize()
+    ref2 = _attn_ref_gpu(q2, k2, v2, scale).permute(0, 2, 1, 3).reshape(nb, ntok, H * d)
+    assert bool(torch.isfinite(o2).all())
+    err2 = rel_l2(o2, ref2)
+    assert err2 < 2e-3, err2
+
+
+@pytest.mark.parametrize("nb,n", [(1, 96), (2, 96), (1, 6144), (2, 384)])
+def test_attention_vae_d512_batch_strided_view(S, cuda_dev, nb, n):
+    """The d = 512 VAE kernel through the views AutoencoderKL._attn passes (vae.py): q / k [nb, n, 512] and V^T as the
+    batch-strided permuted view of the [512, nb*n] operand-swapped GEMM output. 96 tokens = the 8x12 latent of a 64x96
+    image (ragged against the 128-row CTA), 6144 = 64x96 (512x768 image)."""
+    c = 512
+    g = torch.Generator().manual_seed(n + nb)
+    q = torch.randn(nb, n, c, generator=g).half().to(cuda_dev)
+    k = torch.randn(nb, n, c, generator=g).half().to(cuda_dev)
+    v = torch.randn(nb, n, c, generator=g).half().to(cuda_dev)
+    vt = v.reshape(nb * n, c).t().contiguous()                          # [c, nb*n]
+    vt3 = vt.view(c, nb, n).permute(1, 0, 2)
+    scale = float(c ** -0.5)
+    o = S.ops.attention(q, k, vt3, heads=1, d=c, dpad=c, nq=n, nkv=n, scale=scale)
+    torch.cuda.synchronize()
+    ref = _attn_ref_gpu(q[:, None], k[:, None], v[:, None], scale)[:, 0]
+    assert bool(torch.isfinite(o).all())
+    err = rel_l2(o, ref)
+    assert err < 2e-3, err

@@ -38,6 +38,36 @@ def test_vae_oracle_matches_reference(idx):
     assert rel_l2(mean, case["mean"]) < 1e-5 and rel_l2(logvar.clamp(-30, 20), case["logvar"]) < 1e-5
 
 
+def _gen(shape, seed):
+    return torch.randn(shape, generator=torch.Generator().manual_seed(seed))
+
+
+@pytest.mark.parametrize("idx", range(4))
+def test_unet_oracle_matches_reference_nonsquare(idx):
+    """Non-square latents (tests/golden/nonsquare.pt): lets the GPU tests trust the oracle where H != W."""
+    case = golden("nonsquare.pt")["unet"][idx]
+    cfg = CFGS["unet"][case["cfg"]]
+    ctx = _gen((case["x"].shape[0], 77, cfg["context_dim"]), case["ctx_seed"])
+    eps = O.unet_forward(weights("unet", case["cfg"], case["seed"]), case["x"], case["t"], ctx, num_heads=cfg["num_heads"])
+    assert rel_l2(eps, case["eps"]) < 1e-5
+
+
+@pytest.mark.parametrize("idx", range(2))
+def test_vae_oracle_matches_reference_nonsquare(idx):
+    case = golden("nonsquare.pt")["vae"][idx]
+    sd = weights("vae", case["cfg"], case["seed"])
+    assert rel_l2(O.vae_decode(sd, case["z"]), case["dec"]) < 1e-5
+    assert rel_l2(O.vae_encode_moments(sd, case["img"]), case["moments"]) < 1e-5
+
+
+def test_plms_oracle_matches_reference_nonsquare():
+    g = golden("nonsquare.pt")["pipeline"]
+    usd = weights("unet", "tiny", g["unet_seed"])
+    model_fn = lambda x, t, c: O.unet_forward(usd, x, t, c, num_heads=CFGS["unet"]["tiny"]["num_heads"])
+    assert rel_l2(O.plms_sample(model_fn, g["x_T"], g["c"], g["uc"], 7.5, S=10), g["plms10"]) < 1e-5
+    assert rel_l2(O.decode_first_stage(weights("vae", "tiny", g["vae_seed"]), g["plms10"]), g["x_dec"]) < 1e-5
+
+
 @pytest.mark.parametrize("idx", range(2))
 def test_clip_oracle_matches_transformers(idx):
     case = golden("clip.pt")[idx]
