@@ -151,6 +151,21 @@ int sdb_groupnorm(const float* x0, const float* x1, int32_t c0, int32_t c1, int3
                   int32_t stats_group /* channels per entry; must divide c0, c1 and (c0 + c1) / groups */,
                   sdb_stream_t stream);
 
+/*
+ * GroupNorm(32) [+ SiLU] of one NHWC fp32 tensor [nb, h, w, c] with the two options of the attention-block UNet's
+ * ResBlock (openaimodel.py:255-275), writing the fp16 operand of the following 3x3 conv:
+ *   modulation (scale, shift non-NULL; use_scale_shift_norm, :267-271): GN(x) * (1 + scale[n, c]) + shift[n, c], with
+ *     scale / shift rows ldm floats apart (column slices of the FiLM output);
+ *   resample (up / down ResBlocks, :256-261): 0 none, 1 the activated output 2x2 average-pooled ([nb, h/2, w/2, c]),
+ *     2 nearest-2x upsampled ([nb, 2h, 2w, c]).
+ * Statistics come from chan_stats (fused GEMM statistics, as in sdb_groupnorm; groups <= 32) or, when NULL, from a
+ * reduction pass. stats_ws as in sdb_groupnorm.
+ */
+int sdb_groupnorm_mod(const float* x, int32_t c, int32_t nb, int32_t h, int32_t w, int32_t groups, const float* gamma,
+                      const float* beta, float eps, int32_t silu, const float* scale, const float* shift, int32_t ldm,
+                      int32_t resample, void* out_f16, void* stats_ws, const void* chan_stats, int32_t stats_t,
+                      int32_t stats_group, sdb_stream_t stream);
+
 /* LayerNorm over the last dim of fp32 [rows, c] -> fp16 (attention.py:203-205, eps 1e-5). */
 int sdb_layernorm(const float* x, int32_t rows, int32_t c, const float* gamma, const float* beta, float eps,
                   void* out_f16, float* out_f32 /* optional */, sdb_stream_t stream);
@@ -231,6 +246,17 @@ int sdb_mask_blend(const float* img_orig, const float* mask, int32_t mask_channe
 int sdb_vae_sample(const float* moments, const float* noise_nchw, int32_t nb, int32_t hw, float scale_factor,
                    float* z_nchw, sdb_stream_t stream);
 int sdb_to_uint8(const float* x_nhwc, int64_t n, uint8_t* out, sdb_stream_t stream);
+/* 2x2 resample of the fp32 residual stream (ResBlock.x_upd, openaimodel.py:209-214,260): NHWC [nb, h, w, c] ->
+ * mode 1: 2x2 average pool [nb, h/2, w/2, c] (summed in avg_pool2d's order, then / 4); mode 2: nearest 2x [nb, 2h, 2w, c] */
+int sdb_resample_f32(const float* x, int32_t nb, int32_t h, int32_t w, int32_t c, int32_t mode, float* out,
+                     sdb_stream_t stream);
+/* Ancestral DDPM step, LatentDiffusion.p_sample with clip_denoised=False (ddpm.py:1047-1108), one timestep per call:
+ *   x0 = sqrt_recip_ac * x - sqrt_recipm1_ac * eps;  mean = coef1 * x0 + coef2 * x;  x' = mean + sigma * noise
+ * with sigma = nonzero_mask * exp(0.5 * posterior_log_variance_clipped[t]) (noise NULL: x' = mean). fp32, rounded per
+ * operation as the reference's tensor ops; x0 optionally written (the intermediates). */
+int sdb_ddpm_step(const float* x, const float* eps, const float* noise, float sqrt_recip_alphas_cumprod,
+                  float sqrt_recipm1_alphas_cumprod, float posterior_mean_coef1, float posterior_mean_coef2, float sigma,
+                  int64_t n, float* x_out, float* x0_out, sdb_stream_t stream);
 /* out = a*x + b (latent scaling z/0.18215, ddpm.py:713) */
 int sdb_axpby(const float* x, float a, float b, int64_t n, float* out, sdb_stream_t stream);
 /* out = a*x + b*y (DDIMSampler.stochastic_encode, ddim.py:206-220; q_sample, ddpm.py:274-277) */

@@ -35,6 +35,22 @@ CLIP_IMAGE_STD = (0.26862954, 0.26130258, 0.27577711)
 TINY_UNET = dict(image_size=16, in_channels=4, out_channels=4, model_channels=64, attention_resolutions=[2, 1],
                  num_res_blocks=1, channel_mult=[1, 2], num_heads=2, use_spatial_transformer=True,
                  transformer_depth=1, context_dim=64, use_checkpoint=False, legacy=False)
+# unconditional attention-block family (openaimodel.py AttentionBlock + ResBlock with scale-shift norm / up-down):
+# the LSUN-Churches LDM (models/ldm/lsun_churches256/config.yaml) and two small members for tests. The tiny ones keep
+# every GroupNorm width a multiple of 32, every conv input width a multiple of 64, and head dims even, <= 128 and
+# partly not multiples of 16 (8 and 24; 16 and 40).
+LSUN_CHURCHES_UNET = dict(image_size=32, in_channels=4, out_channels=4, model_channels=192,
+                          attention_resolutions=[1, 2, 4, 8], num_res_blocks=2, channel_mult=[1, 2, 2, 4, 4], num_heads=8,
+                          use_scale_shift_norm=True, resblock_updown=True, use_spatial_transformer=False,
+                          context_dim=None, legacy=True)
+TINY_ATTN_UNET = dict(image_size=16, in_channels=4, out_channels=4, model_channels=64, attention_resolutions=[1, 2, 4],
+                      num_res_blocks=1, channel_mult=[1, 3, 3], num_heads=8, use_scale_shift_norm=True,
+                      resblock_updown=True, use_spatial_transformer=False, context_dim=None, legacy=True)
+# both options off: additive-FiLM ResBlocks and conv Downsample / Upsample around AttentionBlocks
+TINY_ATTN_PLAIN_UNET = dict(image_size=16, in_channels=4, out_channels=4, model_channels=64,
+                            attention_resolutions=[2, 4], num_res_blocks=1, channel_mult=[1, 2, 5], num_heads=8,
+                            use_scale_shift_norm=False, resblock_updown=False, use_spatial_transformer=False,
+                            context_dim=None, legacy=True)
 TINY_VAE = dict(embed_dim=4, ddconfig=dict(double_z=True, z_channels=4, resolution=32, in_channels=3, out_ch=3,
                                            ch=64, ch_mult=[1, 2], num_res_blocks=1, attn_resolutions=[],
                                            dropout=0.0))
@@ -46,47 +62,60 @@ TINY_CLIP = dict(vocab_size=1000, hidden_size=128, intermediate_size=512, num_hi
 def unet_plan(cfg):
     """Block list of UNetModel as (kind, prefix, params) tuples, in execution order.
 
-    kinds: conv_in, res(cin, cout), st(ch, heads, dhead), down(ch), up(ch), out. Mirrors the constructor loops
-    at openaimodel.py:512-686 for use_spatial_transformer=True, resblock_updown=False.
+    kinds: conv_in, res(cin, cout, ss, updown), st(ch, heads, dhead), attn(ch, heads, dhead), down(ch), up(ch), out.
+    Mirrors the constructor loops at openaimodel.py:512-686. Without a spatial transformer the attention layers are
+    AttentionBlocks with `num_heads` heads of ch / num_heads channels (legacy=True passes num_head_channels=-1,
+    openaimodel.py:547-549); `ss` is use_scale_shift_norm; with resblock_updown the Downsample / Upsample layers are
+    ResBlocks with updown "down" / "up" (openaimodel.py:567-582, 664-677).
     """
     mc = cfg["model_channels"]
     mult = cfg["channel_mult"]
     nrb = cfg["num_res_blocks"]
     heads = cfg["num_heads"]
     attn_res = set(cfg["attention_resolutions"])
+    st = cfg.get("use_spatial_transformer", False)
+    ss = bool(cfg.get("use_scale_shift_norm", False))
+    updown = bool(cfg.get("resblock_updown", False))
+    akind = "st" if st else "attn"
+
+    def res(pre, cin, cout, ud=None, **kw):
+        return ("res", pre, dict(cin=cin, cout=cout, ss=ss, updown=ud, **kw))
+
     plan = {"input": [], "middle": [], "output": []}
     plan["input"].append([("conv_in", "input_blocks.0.0", dict(cin=cfg["in_channels"], cout=mc))])
     chans = [mc]
     ch, ds, idx = mc, 1, 1
     for level, m in enumerate(mult):
         for _ in range(nrb):
-            layers = [("res", f"input_blocks.{idx}.0", dict(cin=ch, cout=m * mc))]
+            layers = [res(f"input_blocks.{idx}.0", ch, m * mc)]
             ch = m * mc
             if ds in attn_res:
-                layers.append(("st", f"input_blocks.{idx}.1", dict(ch=ch, heads=heads, dhead=ch // heads)))
+                layers.append((akind, f"input_blocks.{idx}.1", dict(ch=ch, heads=heads, dhead=ch // heads)))
             plan["input"].append(layers)
             chans.append(ch)
             idx += 1
         if level != len(mult) - 1:
-            plan["input"].append([("down", f"input_blocks.{idx}.0", dict(ch=ch))])
+            plan["input"].append([res(f"input_blocks.{idx}.0", ch, ch, "down") if updown else
+                                  ("down", f"input_blocks.{idx}.0", dict(ch=ch))])
             chans.append(ch)
             idx += 1
             ds *= 2
-    plan["middle"] = [("res", "middle_block.0", dict(cin=ch, cout=ch)),
-                      ("st", "middle_block.1", dict(ch=ch, heads=heads, dhead=ch // heads)),
-                      ("res", "middle_block.2", dict(cin=ch, cout=ch))]
+    plan["middle"] = [res("middle_block.0", ch, ch),
+                      (akind, "middle_block.1", dict(ch=ch, heads=heads, dhead=ch // heads)),
+                      res("middle_block.2", ch, ch)]
     idx = 0
     for level, m in list(enumerate(mult))[::-1]:
         for i in range(nrb + 1):
             ich = chans.pop()
-            layers = [("res", f"output_blocks.{idx}.0", dict(cin=ch + ich, cout=mc * m, skip_ch=ich))]
+            layers = [res(f"output_blocks.{idx}.0", ch + ich, mc * m, skip_ch=ich)]
             ch = mc * m
             sub = 1
             if ds in attn_res:
-                layers.append(("st", f"output_blocks.{idx}.{sub}", dict(ch=ch, heads=heads, dhead=ch // heads)))
+                layers.append((akind, f"output_blocks.{idx}.{sub}", dict(ch=ch, heads=heads, dhead=ch // heads)))
                 sub += 1
             if level and i == nrb:
-                layers.append(("up", f"output_blocks.{idx}.{sub}", dict(ch=ch)))
+                layers.append(res(f"output_blocks.{idx}.{sub}", ch, ch, "up") if updown else
+                              ("up", f"output_blocks.{idx}.{sub}", dict(ch=ch)))
                 ds //= 2
             plan["output"].append(layers)
             idx += 1
@@ -94,13 +123,14 @@ def unet_plan(cfg):
     return plan
 
 
-def _res_shapes(p, pre, cin, cout, temb):
+def _res_shapes(p, pre, cin, cout, temb, ss=False):
     p[f"{pre}.in_layers.0.weight"] = (cin,)
     p[f"{pre}.in_layers.0.bias"] = (cin,)
     p[f"{pre}.in_layers.2.weight"] = (cout, cin, 3, 3)
     p[f"{pre}.in_layers.2.bias"] = (cout,)
-    p[f"{pre}.emb_layers.1.weight"] = (cout, temb)
-    p[f"{pre}.emb_layers.1.bias"] = (cout,)
+    ew = 2 * cout if ss else cout      # [scale | shift] with use_scale_shift_norm (openaimodel.py:218-224)
+    p[f"{pre}.emb_layers.1.weight"] = (ew, temb)
+    p[f"{pre}.emb_layers.1.bias"] = (ew,)
     p[f"{pre}.out_layers.0.weight"] = (cout,)
     p[f"{pre}.out_layers.0.bias"] = (cout,)
     p[f"{pre}.out_layers.3.weight"] = (cout, cout, 3, 3)
@@ -133,12 +163,22 @@ def _st_shapes(p, pre, ch, ctx):
     p[f"{pre}.proj_out.bias"] = (ch,)
 
 
+def _attn_block_shapes(p, pre, ch):
+    """AttentionBlock (openaimodel.py:278-324): GroupNorm32, qkv and proj_out are 1-d 1x1 convs."""
+    p[f"{pre}.norm.weight"] = (ch,)
+    p[f"{pre}.norm.bias"] = (ch,)
+    p[f"{pre}.qkv.weight"] = (3 * ch, ch, 1)
+    p[f"{pre}.qkv.bias"] = (3 * ch,)
+    p[f"{pre}.proj_out.weight"] = (ch, ch, 1)
+    p[f"{pre}.proj_out.bias"] = (ch,)
+
+
 def unet_param_shapes(cfg):
     """OrderedDict key -> shape, keys exactly as UNetModel.state_dict() (686 tensors for SD v1)."""
     assert cfg.get("transformer_depth", 1) == 1, "SD v1 uses transformer_depth 1"
     mc = cfg["model_channels"]
     temb = 4 * mc
-    ctx = cfg["context_dim"]
+    ctx = cfg.get("context_dim")
     p = OrderedDict()
     p["time_embed.0.weight"] = (temb, mc)
     p["time_embed.0.bias"] = (temb,)
@@ -152,9 +192,11 @@ def unet_param_shapes(cfg):
                 p[f"{pre}.weight"] = (a["cout"], a["cin"], 3, 3)
                 p[f"{pre}.bias"] = (a["cout"],)
             elif kind == "res":
-                _res_shapes(p, pre, a["cin"], a["cout"], temb)
+                _res_shapes(p, pre, a["cin"], a["cout"], temb, a["ss"])
             elif kind == "st":
                 _st_shapes(p, pre, a["ch"], ctx)
+            elif kind == "attn":
+                _attn_block_shapes(p, pre, a["ch"])
             elif kind == "down":
                 p[f"{pre}.op.weight"] = (a["ch"], a["ch"], 3, 3)
                 p[f"{pre}.op.bias"] = (a["ch"],)

@@ -276,6 +276,52 @@ __global__ void embed_tokens_kernel(const long long* __restrict__ ids, int rows,
   }
 }
 
+// 2x2 resample of the fp32 residual stream (ResBlock.x_upd, openaimodel.py:209-214,260 with use_conv=False):
+// mode 1 = 2x2 average pool in avg_pool2d's order ((x00 + x01) + x10) + x11, then / 4; mode 2 = nearest 2x. NHWC.
+__global__ void resample_f32_kernel(const float* __restrict__ x, int nb, int h, int w, int c, int mode,
+                                    float* __restrict__ out) {
+  const int ho = mode == 1 ? h / 2 : 2 * h, wo = mode == 1 ? w / 2 : 2 * w;
+  const int c4 = c / 4;
+  const size_t total = static_cast<size_t>(nb) * ho * wo * c4;
+  GRID_STRIDE(i, total) {
+    const int cc = static_cast<int>(i % c4) * 4;
+    const size_t pix = i / c4;
+    const int ox = static_cast<int>(pix % wo);
+    const int oy = static_cast<int>((pix / wo) % ho);
+    const size_t n = pix / (static_cast<size_t>(wo) * ho);
+    float4 r;
+    if (mode == 1) {
+      const float* p = x + ((n * h + 2 * oy) * w + 2 * ox) * c + cc;
+      const float4 a = *reinterpret_cast<const float4*>(p), b = *reinterpret_cast<const float4*>(p + c);
+      const float4 d = *reinterpret_cast<const float4*>(p + static_cast<size_t>(w) * c);
+      const float4 e = *reinterpret_cast<const float4*>(p + static_cast<size_t>(w) * c + c);
+      r.x = __fdiv_rn(__fadd_rn(__fadd_rn(__fadd_rn(a.x, b.x), d.x), e.x), 4.0f);
+      r.y = __fdiv_rn(__fadd_rn(__fadd_rn(__fadd_rn(a.y, b.y), d.y), e.y), 4.0f);
+      r.z = __fdiv_rn(__fadd_rn(__fadd_rn(__fadd_rn(a.z, b.z), d.z), e.z), 4.0f);
+      r.w = __fdiv_rn(__fadd_rn(__fadd_rn(__fadd_rn(a.w, b.w), d.w), e.w), 4.0f);
+    } else {
+      r = *reinterpret_cast<const float4*>(x + ((n * h + oy / 2) * w + ox / 2) * c + cc);
+    }
+    *reinterpret_cast<float4*>(out + pix * c + cc) = r;
+  }
+}
+
+// Ancestral DDPM step (LatentDiffusion.p_sample with clip_denoised=False, ddpm.py:1047-1108), fp32 in the reference's
+// operation order: x0 = sqrt_recip_ac x - sqrt_recipm1_ac eps; mean = c1 x0 + c2 x; x' = mean + sigma noise, where
+// sigma = nonzero_mask * exp(0.5 posterior_log_variance_clipped) is formed on the host exactly as the reference does.
+__global__ void ddpm_step_kernel(const float* __restrict__ x, const float* __restrict__ eps,
+                                 const float* __restrict__ noise, float sqrt_recip_ac, float sqrt_recipm1_ac, float c1,
+                                 float c2, float sigma, size_t n, float* __restrict__ x_out, float* __restrict__ x0_out) {
+  GRID_STRIDE(i, n) {
+    const float xv = x[i];
+    const float x0 = __fsub_rn(__fmul_rn(sqrt_recip_ac, xv), __fmul_rn(sqrt_recipm1_ac, eps[i]));
+    float v = __fadd_rn(__fmul_rn(c1, x0), __fmul_rn(c2, xv));
+    if (noise) v = __fadd_rn(v, __fmul_rn(sigma, noise[i]));
+    x_out[i] = v;
+    if (x0_out) x0_out[i] = x0;
+  }
+}
+
 }  // namespace sdb
 
 using namespace sdb;
@@ -438,6 +484,29 @@ extern "C" int sdb_embed_tokens(const int64_t* ids, int32_t rows, int32_t n_ctx,
   SDB_CHECK(ids && tok && pos && out, "sdb_embed_tokens: null pointer");
   embed_tokens_kernel<<<grid_for(static_cast<size_t>(rows) * dim), 256, 0, ST>>>(
       reinterpret_cast<const long long*>(ids), rows, n_ctx, dim, vocab, tok, pos, out);
+  SDB_LAUNCH_CHECK();
+  return 0;
+}
+extern "C" int sdb_resample_f32(const float* x, int32_t nb, int32_t h, int32_t w, int32_t c, int32_t mode, float* out,
+                                sdb_stream_t stream) {
+  SDB_REC(sdb_resample_f32(x, nb, h, w, c, mode, out, s_));
+  SDB_CHECK(x && out && nb > 0 && h > 0 && w > 0 && c > 0 && c % 4 == 0, "sdb_resample_f32: bad arguments");
+  SDB_CHECK(mode == 1 || mode == 2, "sdb_resample_f32: mode %d (1 down, 2 up)", mode);
+  SDB_CHECK(mode != 1 || (h % 2 == 0 && w % 2 == 0), "sdb_resample_f32: 2x2 average pool needs even sides (%dx%d)", h, w);
+  const size_t total = static_cast<size_t>(nb) * h * w * (c / 4) * (mode == 1 ? 1 : 4) / (mode == 1 ? 4 : 1);
+  resample_f32_kernel<<<grid_for(total), 256, 0, ST>>>(x, nb, h, w, c, mode, out);
+  SDB_LAUNCH_CHECK();
+  return 0;
+}
+extern "C" int sdb_ddpm_step(const float* x, const float* eps, const float* noise, float sqrt_recip_alphas_cumprod,
+                             float sqrt_recipm1_alphas_cumprod, float posterior_mean_coef1, float posterior_mean_coef2,
+                             float sigma, int64_t n, float* x_out, float* x0_out, sdb_stream_t stream) {
+  SDB_REC(sdb_ddpm_step(x, eps, noise, sqrt_recip_alphas_cumprod, sqrt_recipm1_alphas_cumprod, posterior_mean_coef1,
+                        posterior_mean_coef2, sigma, n, x_out, x0_out, s_));
+  SDB_CHECK(x && eps && x_out && n > 0, "sdb_ddpm_step: bad arguments");
+  ddpm_step_kernel<<<grid_for(n), 256, 0, ST>>>(x, eps, noise, sqrt_recip_alphas_cumprod, sqrt_recipm1_alphas_cumprod,
+                                                posterior_mean_coef1, posterior_mean_coef2, sigma, static_cast<size_t>(n),
+                                                x_out, x0_out);
   SDB_LAUNCH_CHECK();
   return 0;
 }

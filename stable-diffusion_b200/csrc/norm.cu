@@ -426,6 +426,84 @@ __global__ void __launch_bounds__(256)
   for (int c = threadIdx.x; c < cols; c += blockDim.x) o[c] = __float2half_rn(__expf(p[c] * scale - m) * inv);
 }
 
+// GroupNorm(32) of an NHWC fp32 tensor -> one per-(sample, channel) affine -> SiLU -> optional 2x2 resample -> fp16.
+// Modulation (ResBlock.out_layers with use_scale_shift_norm, openaimodel.py:267-271): GN(h) * (1 + scale) + shift is
+// folded into a = rstd gamma (1 + scale), b = (beta - mean rstd gamma)(1 + scale) + shift; scale / shift are strided
+// column slices of the FiLM GEMV output (row stride ldm). Resample (ResBlock up / down, openaimodel.py:256-261, with
+// Downsample / Upsample(use_conv=False)): the activated values are written 2x2 average-pooled (1) or nearest-2x
+// upsampled (2), so the full-resolution fp16 tensor never reaches HBM. grid = (slabs of output pixels, nb).
+__global__ void __launch_bounds__(GN_THREADS)
+    gn_mod_apply_kernel(const float* __restrict__ x, int C, int h, int w, int groups, int pix_per_block,
+                        const float* __restrict__ meanrstd, const float* __restrict__ gamma,
+                        const float* __restrict__ beta, const float* __restrict__ scale, const float* __restrict__ shift,
+                        int ldm, int silu, int resample, __half* __restrict__ out) {
+  extern __shared__ float2 gn_ab[];   // [C] {a, b}
+  const int n = blockIdx.y;
+  const int cpg = C / groups;
+  pdl_launch_dependents();
+  pdl_wait();
+  for (int c = threadIdx.x; c < C; c += GN_THREADS) {
+    const int g = c / cpg;
+    const float mean = meanrstd[(static_cast<size_t>(n) * groups + g) * 2];
+    const float rstd = meanrstd[(static_cast<size_t>(n) * groups + g) * 2 + 1];
+    float a = rstd * __ldg(gamma + c);
+    float b = fmaf(-mean, a, __ldg(beta + c));
+    if (scale) {
+      const float s1 = 1.0f + scale[static_cast<size_t>(n) * ldm + c];
+      a *= s1;
+      b = fmaf(b, s1, shift[static_cast<size_t>(n) * ldm + c]);
+    }
+    gn_ab[c] = make_float2(a, b);
+  }
+  __syncthreads();
+  const int ho = resample == 1 ? h / 2 : resample == 2 ? 2 * h : h;
+  const int wo = resample == 1 ? w / 2 : resample == 2 ? 2 * w : w;
+  const int c4n = C >> 2;
+  const long p0 = static_cast<long>(blockIdx.x) * pix_per_block;
+  const long p1 = min(static_cast<long>(ho) * wo, p0 + pix_per_block);
+  const float* xs = x + static_cast<size_t>(n) * h * w * C;
+  __half* os = out + static_cast<size_t>(n) * ho * wo * C;
+  for (long i = p0 * c4n + threadIdx.x; i < p1 * c4n; i += GN_THREADS) {
+    const int c = static_cast<int>(i % c4n) * 4;
+    const long p = i / c4n;
+    const int oy = static_cast<int>(p / wo), ox = static_cast<int>(p % wo);
+    const float4 ab01 = *reinterpret_cast<const float4*>(&gn_ab[c]);
+    const float4 ab23 = *reinterpret_cast<const float4*>(&gn_ab[c + 2]);
+    auto act = [&](float4 v, float y[4]) {
+      y[0] = fmaf(v.x, ab01.x, ab01.y);
+      y[1] = fmaf(v.y, ab01.z, ab01.w);
+      y[2] = fmaf(v.z, ab23.x, ab23.y);
+      y[3] = fmaf(v.w, ab23.z, ab23.w);
+      if (silu) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) y[j] = silu_fast(y[j]);
+      }
+    };
+    float y[4];
+    if (resample == 1) {
+      float acc[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+      for (int t = 0; t < 4; ++t) {   // avg_pool2d order: rows, then columns
+        const int iy = 2 * oy + (t >> 1), ix = 2 * ox + (t & 1);
+        float yt[4];
+        act(*reinterpret_cast<const float4*>(xs + (static_cast<size_t>(iy) * w + ix) * C + c), yt);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[j] += yt[j];
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) y[j] = acc[j] * 0.25f;
+    } else {
+      const int iy = resample == 2 ? oy >> 1 : oy, ix = resample == 2 ? ox >> 1 : ox;
+      act(*reinterpret_cast<const float4*>(xs + (static_cast<size_t>(iy) * w + ix) * C + c), y);
+    }
+    __half2 h0 = __floats2half2_rn(y[0], y[1]), h1 = __floats2half2_rn(y[2], y[3]);
+    uint2 u;
+    u.x = *reinterpret_cast<uint32_t*>(&h0);
+    u.y = *reinterpret_cast<uint32_t*>(&h1);
+    *reinterpret_cast<uint2*>(os + p * C + c) = u;
+  }
+}
+
 }  // namespace sdb
 
 using namespace sdb;
@@ -540,6 +618,63 @@ extern "C" int sdb_softmax_rows(const float* x, int32_t rows, int32_t cols, floa
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   SDB_CHECK(x && out_f16, "sdb_softmax_rows: null pointer");
   softmax_rows_kernel<<<rows, 256, 0, st>>>(x, cols, scale, static_cast<__half*>(out_f16));
+  SDB_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int sdb_groupnorm_mod(const float* x, int32_t c, int32_t nb, int32_t h, int32_t w, int32_t groups,
+                                 const float* gamma, const float* beta, float eps, int32_t silu, const float* scale,
+                                 const float* shift, int32_t ldm, int32_t resample, void* out_f16, void* stats_ws,
+                                 const void* chan_stats, int32_t stats_t, int32_t stats_group, sdb_stream_t stream) {
+  SDB_REC(sdb_groupnorm_mod(x, c, nb, h, w, groups, gamma, beta, eps, silu, scale, shift, ldm, resample, out_f16, stats_ws,
+                            chan_stats, stats_t, stats_group, s_));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  SDB_CHECK(x && out_f16 && stats_ws && gamma && beta, "sdb_groupnorm_mod: null pointer");
+  SDB_CHECK(nb > 0 && h > 0 && w > 0, "sdb_groupnorm_mod: bad sizes");
+  SDB_CHECK(groups > 0 && groups <= 32 && c % groups == 0, "sdb_groupnorm_mod: C=%d not divisible by groups=%d", c, groups);
+  SDB_CHECK(c % 4 == 0 && c <= GN_THREADS * GN_MAX_CPT, "sdb_groupnorm_mod: C=%d must be a multiple of 4, <= %d", c,
+            GN_THREADS * GN_MAX_CPT);
+  SDB_CHECK((scale == nullptr) == (shift == nullptr), "sdb_groupnorm_mod: scale and shift go together");
+  SDB_CHECK(!scale || ldm >= c, "sdb_groupnorm_mod: modulation row stride %d < C %d", ldm, c);
+  SDB_CHECK(resample >= 0 && resample <= 2, "sdb_groupnorm_mod: resample %d (0 none, 1 down, 2 up)", resample);
+  SDB_CHECK(resample != 1 || (h % 2 == 0 && w % 2 == 0), "sdb_groupnorm_mod: 2x2 average pool needs even sides (%dx%d)",
+            h, w);
+  const int hw = h * w;
+  const int cpg = c / groups;
+  const int sg = stats_group > 0 ? stats_group : 1;
+  // workspace layout as sdb_groupnorm: [nb][GN_MAX_SLABS][groups][2] partials | [nb][groups][2] mean/rstd | [nb] tickets
+  float* partial = static_cast<float*>(stats_ws);
+  float* meanrstd = partial + static_cast<size_t>(nb) * GN_MAX_SLABS * groups * 2;
+  unsigned int* counter = reinterpret_cast<unsigned int*>(meanrstd + static_cast<size_t>(nb) * groups * 2);
+  if (chan_stats) {
+    SDB_CHECK(stats_t > 0 && cpg % sg == 0 && c % sg == 0,
+              "sdb_groupnorm_mod: statistics entries of %d channels do not tile the groups (C %d, %d groups)", sg, c, groups);
+    SDB_CUDA(launch_pdl(gn_fold_kernel, dim3(groups, nb), dim3(GN_THREADS), 0, st, static_cast<const float2*>(chan_stats),
+                        static_cast<int>(stats_t), static_cast<const float2*>(nullptr), 0, sg, c, 0, groups, hw, eps,
+                        meanrstd));
+    SDB_LAUNCH_CHECK();
+  } else {
+    SDB_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned int) * nb, st));
+    int cw = GN_THREADS;
+    while (cw > 32 && cw / 2 >= c) cw /= 2;
+    const int rstep = GN_THREADS / cw;
+    int slabs = std::max(1, std::min(std::min((hw + rstep - 1) / rstep, GN_MAX_SLABS), (sm_count() * 4 + nb - 1) / nb));
+    int rows_per_block = (hw + slabs - 1) / slabs;
+    slabs = (hw + rows_per_block - 1) / rows_per_block;
+    gn_stats_kernel<<<dim3(slabs, nb), GN_THREADS, 2 * c * sizeof(float), st>>>(x, nullptr, c, 0, hw, groups,
+                                                                                 rows_per_block, cw, eps, partial, counter,
+                                                                                 meanrstd);
+    SDB_LAUNCH_CHECK();
+  }
+  const long opix = resample == 1 ? static_cast<long>(hw) / 4 : resample == 2 ? static_cast<long>(hw) * 4 : hw;
+  long slabs = std::max(1L, std::min(opix, static_cast<long>((sm_count() * 4 + nb - 1) / nb)));
+  long ppb = (opix + slabs - 1) / slabs;
+  slabs = (opix + ppb - 1) / ppb;
+  SDB_CUDA(launch_pdl(gn_mod_apply_kernel, dim3(static_cast<unsigned>(slabs), nb), dim3(GN_THREADS),
+                      static_cast<size_t>(c) * sizeof(float2), st, x, static_cast<int>(c), static_cast<int>(h),
+                      static_cast<int>(w), static_cast<int>(groups), static_cast<int>(ppb), static_cast<const float*>(meanrstd),
+                      gamma, beta, scale, shift, static_cast<int>(ldm), static_cast<int>(silu), static_cast<int>(resample),
+                      static_cast<__half*>(out_f16)));
   SDB_LAUNCH_CHECK();
   return 0;
 }

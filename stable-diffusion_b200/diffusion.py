@@ -3,7 +3,10 @@ samplers use (ddpm.py): register_schedule (:117-169), apply_model (:891-992 plai
 (:1393-1421 crossattn branch), get_learned_conditioning (:551-562), encode_first_stage (:825-863),
 get_first_stage_encoding (:542-549), decode_first_stage (:705-763), q_sample (:274-277), ema_scope (:171-184).
 Sub-modules keep the reference attribute names so checkpoint prefixes resolve:
-`model.diffusion_model.*`, `first_stage_model.*`, `cond_stage_model.transformer.*`.
+`model.diffusion_model.*`, `first_stage_model.*`, `cond_stage_model.transformer.*`, `model_ema.*`.
+Unconditional models (cond_stage_config "__is_unconditional__", e.g. LSUN-Churches) sample through DDIM with no
+conditioning, or through the ancestral sampler (p_sample_loop / progressive_denoising, ddpm.py:1047-1213) whose update
+is one fused kernel per step (sdb_ddpm_step).
 Training (p_losses, training_step, optimizers, logging) is out of scope.
 """
 from __future__ import annotations
@@ -23,34 +26,70 @@ class DiffusionWrapper(nn.Module):
         super().__init__()
         self.diffusion_model = instantiate_from_config(remap_config(diff_model_config))
         self.conditioning_key = conditioning_key
-        assert self.conditioning_key in [None, "crossattn"], "SD v1 uses crossattn conditioning"
+        assert self.conditioning_key in [None, "crossattn"], "supported: crossattn (SD v1) or None (unconditional)"
 
     def forward(self, x, t, c_concat=None, c_crossattn=None):
         if self.conditioning_key is None:
-            raise NotImplementedError("unconditional UNet is not part of the SD-v1 path")
+            return self.diffusion_model(x, t)
         cc = c_crossattn[0] if len(c_crossattn) == 1 else torch.cat(c_crossattn, 1)
         return self.diffusion_model(x, t, context=cc)
+
+
+class _EmaWeights(nn.Module):
+    """Receives the `model_ema.*` tensors of a checkpoint (LitEma, ldm/modules/ema.py: buffer names are the
+    DiffusionWrapper parameter names with the dots removed, plus `decay` and `num_updates`) and hands them to the UNet
+    as its "ema" weight set. Holds no tensors of its own: the UNet packs the set it runs on."""
+
+    def __init__(self, unet):
+        super().__init__()
+        self._unet = [unet]       # not a sub-module: its tensors belong to model.diffusion_model
+        self.loaded = False
+
+    def _load_from_state_dict(self, state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
+                              error_msgs):
+        unet = self._unet[0]
+        names = {("diffusion_model." + k).replace(".", ""): k for k in unet.shapes}
+        sub = {k[len(prefix):]: v for k, v in state_dict.items() if k.startswith(prefix)}
+        unexpected_keys.extend(prefix + k for k in sub if k not in names and k not in ("decay", "num_updates"))
+        if not any(k in sub for k in names):
+            return        # a checkpoint without EMA copies: ema_scope() keeps the raw weights
+        absent = [prefix + k for k in names if k not in sub]
+        if absent:
+            missing_keys.extend(absent)
+            return
+        unet.set_weight_set("ema", {names[k]: v for k, v in sub.items() if k in names})
+        self.loaded = True
 
 
 class LatentDiffusion(nn.Module):
     def __init__(self, first_stage_config, cond_stage_config, unet_config, timesteps=1000, beta_schedule="linear",
                  linear_start=1e-4, linear_end=2e-2, cosine_s=8e-3, num_timesteps_cond=None, cond_stage_key="image",
                  cond_stage_trainable=False, concat_mode=True, cond_stage_forward=None, conditioning_key=None,
-                 scale_factor=1.0, scale_by_std=False, parameterization="eps", use_ema=False, image_size=256,
+                 scale_factor=1.0, scale_by_std=False, parameterization="eps", use_ema=True, image_size=256,
                  channels=3, first_stage_key="image", log_every_t=100, monitor=None, v_posterior=0.,
                  scheduler_config=None, **ignored):
         super().__init__()
-        assert parameterization == "eps" and beta_schedule == "linear" and not scale_by_std
+        assert parameterization == "eps" and beta_schedule == "linear"
         if conditioning_key is None:
             conditioning_key = "concat" if concat_mode else "crossattn"
+        if cond_stage_config == "__is_unconditional__":      # ddpm.py:447-448, 501-504
+            conditioning_key = None
         self.parameterization = parameterization
         self.image_size, self.channels = image_size, channels
-        self.scale_factor = float(scale_factor)
+        self.scale_by_std = scale_by_std
+        if scale_by_std:        # a buffer loaded from the checkpoint (ddpm.py:461-464)
+            self.register_buffer("scale_factor", torch.tensor(scale_factor))
+        else:
+            self.scale_factor = float(scale_factor)
         self.use_ema = use_ema
+        self.log_every_t = log_every_t
+        self.clip_denoised = False
         self.cond_stage_key, self.first_stage_key = cond_stage_key, first_stage_key
         self.model = DiffusionWrapper(unet_config, conditioning_key)
+        if use_ema:
+            self.model_ema = _EmaWeights(self.model.diffusion_model)
         self.first_stage_model = instantiate_from_config(remap_config(first_stage_config))
-        if cond_stage_config in ("__is_first_stage__", "__is_unconditional__"):
+        if cond_stage_config == "__is_first_stage__":
             raise NotImplementedError(cond_stage_config)
         self.cond_stage_model = instantiate_from_config(remap_config(cond_stage_config))
         self.register_schedule(timesteps, linear_start, linear_end)
@@ -69,6 +108,18 @@ class LatentDiffusion(nn.Module):
         self.register_buffer("alphas_cumprod_prev", to_torch(alphas_cumprod_prev))
         self.register_buffer("sqrt_alphas_cumprod", to_torch(np.sqrt(alphas_cumprod)))
         self.register_buffer("sqrt_one_minus_alphas_cumprod", to_torch(np.sqrt(1. - alphas_cumprod)))
+        # q(x_{t-1} | x_t, x_0) for the ancestral sampler (v_posterior 0); recomputed from the config, not loaded
+        nonp = dict(persistent=False)
+        self.register_buffer("sqrt_recip_alphas_cumprod", to_torch(np.sqrt(1. / alphas_cumprod)), **nonp)
+        self.register_buffer("sqrt_recipm1_alphas_cumprod", to_torch(np.sqrt(1. / alphas_cumprod - 1)), **nonp)
+        posterior_variance = betas * (1. - alphas_cumprod_prev) / (1. - alphas_cumprod)
+        self.register_buffer("posterior_variance", to_torch(posterior_variance), **nonp)
+        self.register_buffer("posterior_log_variance_clipped",
+                             to_torch(np.log(np.maximum(posterior_variance, 1e-20))), **nonp)
+        self.register_buffer("posterior_mean_coef1",
+                             to_torch(betas * np.sqrt(alphas_cumprod_prev) / (1. - alphas_cumprod)), **nonp)
+        self.register_buffer("posterior_mean_coef2",
+                             to_torch((1. - alphas_cumprod_prev) * np.sqrt(alphas) / (1. - alphas_cumprod)), **nonp)
 
     @property
     def device(self):
@@ -76,7 +127,21 @@ class LatentDiffusion(nn.Module):
 
     @contextmanager
     def ema_scope(self, context=None):
-        yield None  # use_ema False in v1-inference.yaml:18 -> the reference's scope is a no-op too
+        """ddpm.py:171-184: inside the scope the UNet runs on the checkpoint's EMA weights (use_ema, e.g. the LSUN
+        config's default); SD v1 has use_ema False and the scope is a no-op."""
+        unet = self.model.diffusion_model
+        swap = self.use_ema and unet.has_weight_set("ema")
+        if swap:
+            unet.use_weight_set("ema")
+            if context is not None:
+                print(f"{context}: Switched to EMA weights")
+        try:
+            yield None
+        finally:
+            if swap:
+                unet.use_weight_set("raw")
+                if context is not None:
+                    print(f"{context}: Restored training weights")
 
     # -- denoiser
     def apply_model(self, x_noisy, t, cond, return_ids=False):
@@ -93,7 +158,8 @@ class LatentDiffusion(nn.Module):
 
     def set_context(self, c):
         """Fast path used by sdb200 samplers: cross-attention K/V of the (guidance-doubled) context, once per batch."""
-        self.model.diffusion_model.set_context(c)
+        if c is not None:
+            self.model.diffusion_model.set_context(c)
 
     def get_learned_conditioning(self, c):
         enc = getattr(self.cond_stage_model, "encode", None)
@@ -111,14 +177,14 @@ class LatentDiffusion(nn.Module):
 
     def get_first_stage_encoding(self, encoder_posterior, noise=None):
         if hasattr(encoder_posterior, "sample"):
-            return encoder_posterior.sample(noise=noise, scale=self.scale_factor)
+            return encoder_posterior.sample(noise=noise, scale=float(self.scale_factor))
         if torch.is_tensor(encoder_posterior):
-            return self.scale_factor * encoder_posterior
+            return float(self.scale_factor) * encoder_posterior
         raise NotImplementedError(f"encoder_posterior of type '{type(encoder_posterior)}' not yet implemented")
 
     def decode_first_stage(self, z, predict_cids=False, force_not_quantize=False):
         assert not predict_cids
-        return self.first_stage_model.decode(z, scale=1. / self.scale_factor)
+        return self.first_stage_model.decode(z, scale=1. / float(self.scale_factor))
 
     def q_sample(self, x_start, t, noise=None):
         if noise is None:
@@ -128,3 +194,74 @@ class LatentDiffusion(nn.Module):
         a = float(self.sqrt_alphas_cumprod[int(t_host[0])])
         s = float(self.sqrt_one_minus_alphas_cumprod[int(t_host[0])])
         return ops.axpby2(x_start.contiguous().float(), noise.contiguous().float(), a, s)
+
+    # -- ancestral sampler (ddpm.py:1047-1213), unconditional models
+    def _p_step(self, img, t, noise):
+        """LatentDiffusion.p_sample (clip_denoised=False, one timestep for the batch) as one fused kernel; the scalars
+        are the fp32 schedule entries, and sigma is formed as the reference does: nonzero_mask * exp(0.5 * logvar)."""
+        b = img.shape[0]
+        ts = torch.full((b,), t, device=img.device, dtype=torch.long)
+        eps = self.apply_model(img, ts, None).contiguous().float()
+        cpu = lambda k: getattr(self, k)[t].detach().to("cpu", torch.float32)
+        sigma = (torch.tensor(1.0 if t != 0 else 0.0) * (0.5 * cpu("posterior_log_variance_clipped")).exp()).item()
+        return ops.ddpm_step(img, eps, noise, sqrt_recip_ac=cpu("sqrt_recip_alphas_cumprod").item(),
+                             sqrt_recipm1_ac=cpu("sqrt_recipm1_alphas_cumprod").item(),
+                             coef1=cpu("posterior_mean_coef1").item(), coef2=cpu("posterior_mean_coef2").item(),
+                             sigma=sigma)
+
+    def _check_uncond(self, cond):
+        if cond is not None or self.model.conditioning_key is not None:
+            raise NotImplementedError("the ancestral sampler runs unconditional models (cond None) only")
+
+    @torch.no_grad()
+    def p_sample_loop(self, cond, shape, return_intermediates=False, x_T=None, verbose=True, callback=None,
+                      timesteps=None, quantize_denoised=False, mask=None, x0=None, img_callback=None, start_T=None,
+                      log_every_t=None):
+        """ddpm.py:1165-1213 (no mask): ancestral steps T-1 .. 0; intermediates are the latents."""
+        self._check_uncond(cond)
+        assert mask is None and not quantize_denoised
+        log_every_t = log_every_t or self.log_every_t
+        img = torch.randn(shape, device=self.device) if x_T is None else x_T.to(self.device, torch.float32).contiguous()
+        intermediates = [img]
+        timesteps = self.num_timesteps if timesteps is None else timesteps
+        if start_T is not None:
+            timesteps = min(timesteps, start_T)
+        for i in reversed(range(0, timesteps)):
+            img, _ = self._p_step(img, i, torch.randn(img.shape, device=img.device))
+            if i % log_every_t == 0 or i == timesteps - 1:
+                intermediates.append(img)
+            if callback:
+                callback(i)
+            if img_callback:
+                img_callback(img, i)
+        return (img, intermediates) if return_intermediates else img
+
+    @torch.no_grad()
+    def progressive_denoising(self, cond, shape, verbose=True, callback=None, quantize_denoised=False, img_callback=None,
+                              mask=None, x0=None, temperature=1., noise_dropout=0., score_corrector=None,
+                              corrector_kwargs=None, batch_size=None, x_T=None, start_T=None, log_every_t=None):
+        """ddpm.py:1110-1163 (no mask): ancestral steps T-1 .. 0; intermediates are the x0 predictions."""
+        self._check_uncond(cond)
+        assert mask is None and not quantize_denoised and noise_dropout == 0. and score_corrector is None
+        log_every_t = log_every_t or self.log_every_t
+        timesteps = self.num_timesteps
+        if batch_size is not None:
+            shape = [batch_size] + list(shape)
+        img = torch.randn(shape, device=self.device) if x_T is None else x_T.to(self.device, torch.float32).contiguous()
+        if start_T is not None:
+            timesteps = min(timesteps, start_T)
+        if isinstance(temperature, float):
+            temperature = [temperature] * timesteps
+        intermediates = []
+        for i in reversed(range(0, timesteps)):
+            noise = torch.randn(img.shape, device=img.device)       # noise_like, util.py:264-267
+            if temperature[i] != 1.:
+                noise = noise * temperature[i]
+            img, x0_partial = self._p_step(img, i, noise)
+            if i % log_every_t == 0 or i == timesteps - 1:
+                intermediates.append(x0_partial)
+            if callback:
+                callback(i)
+            if img_callback:
+                img_callback(img, i)
+        return img, intermediates

@@ -84,6 +84,9 @@ SIGNATURES = {
     "sdb_gemm_plan": ([C.POINTER(GemmDesc), C.POINTER(C.c_int32)], C.c_int),
     "sdb_attention": ([C.POINTER(AttnDesc), _P], C.c_int),
     "sdb_groupnorm": ([_P, _P, _I, _I, _I, _I, _I, _P, _P, _F, _I, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P], C.c_int),
+    "sdb_groupnorm_mod": ([_P, _I, _I, _I, _I, _I, _P, _P, _F, _I, _P, _P, _I, _I, _P, _P, _P, _I, _I, _P], C.c_int),
+    "sdb_resample_f32": ([_P, _I, _I, _I, _I, _I, _P, _P], C.c_int),
+    "sdb_ddpm_step": ([_P, _P, _P, _F, _F, _F, _F, _F, _L, _P, _P, _P], C.c_int),
     "sdb_layernorm": ([_P, _I, _I, _P, _P, _F, _P, _P, _P], C.c_int),
     "sdb_softmax_rows": ([_P, _I, _I, _F, _P, _P], C.c_int),
     "sdb_nchw_to_nhwc": ([_P, _I, _I, _I, _P, _P, _P], C.c_int),

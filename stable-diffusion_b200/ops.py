@@ -340,6 +340,61 @@ def groupnorm(x0, gamma, beta, *, x1=None, groups=32, eps=1e-5, silu=False, want
     return out, raw
 
 
+def groupnorm_mod(x, gamma, beta, *, scale=None, shift=None, resample=0, groups=32, eps=1e-5, silu=True):
+    """x fp32 NHWC [nb, h, w, c] -> fp16 NHWC: SiLU(GN(x) [* (1 + scale) + shift]), optionally 2x2 average-pooled
+    (resample=1) or nearest-2x upsampled (resample=2). scale / shift: fp32 [nb, c] views with unit column stride (the
+    FiLM output's column slices). Uses the fused statistics attached to x by the producing gemm() when compatible."""
+    _chk32(x, "x")
+    nb, h, w, c = x.shape
+    ldm = 0
+    if scale is not None:
+        for t_ in (scale, shift):
+            assert t_.dtype == torch.float32 and t_.is_cuda and t_.shape == (nb, c) and t_.stride(1) == 1
+        assert scale.stride(0) == shift.stride(0)
+        ldm = scale.stride(0)
+    ho, wo = (h // 2, w // 2) if resample == 1 else (2 * h, 2 * w) if resample == 2 else (h, w)
+    out = torch.empty((nb, ho, wo, c), dtype=torch.float16, device=x.device)
+    ws = torch.empty(nb * (128 * groups * 2 + groups * 2 + 1), dtype=torch.float32, device=x.device)
+    cs = channel_stats(x)
+    if cs is not None and ((c // groups) % cs[2] or c % cs[2]):
+        cs = None
+    _l.check(_l.load().sdb_groupnorm_mod(_ptr(x), c, nb, h, w, groups, _ptr(gamma), _ptr(beta), eps, 1 if silu else 0,
+                                         _ptr(scale), _ptr(shift), ldm, resample, _ptr(out), _ptr(ws),
+                                         _ptr(cs[0]) if cs else None, cs[1] if cs else 0, cs[2] if cs else 1,
+                                         _stream()), "sdb_groupnorm_mod")
+    _count(2)
+    return out
+
+
+def resample_f32(x, mode):
+    """fp32 NHWC [nb, h, w, c] -> 2x2 average pool (mode 1) or nearest 2x (mode 2), fp32 NHWC."""
+    _chk32(x, "x")
+    nb, h, w, c = x.shape
+    ho, wo = (h // 2, w // 2) if mode == 1 else (2 * h, 2 * w)
+    out = torch.empty((nb, ho, wo, c), dtype=torch.float32, device=x.device)
+    _l.check(_l.load().sdb_resample_f32(_ptr(x), nb, h, w, c, mode, _ptr(out), _stream()), "sdb_resample_f32")
+    _count()
+    return out
+
+
+def ddpm_step(x, eps, noise, *, sqrt_recip_ac, sqrt_recipm1_ac, coef1, coef2, sigma, x_out=None, x0_out=None):
+    """One ancestral DDPM update (sdb_ddpm_step); returns (x', x0)."""
+    _chk32(x, "x")
+    _chk32(eps, "eps")
+    assert eps.numel() == x.numel()
+    if noise is not None:
+        _chk32(noise, "noise")
+        assert noise.numel() == x.numel()
+    if x_out is None:
+        x_out = torch.empty_like(x)
+    if x0_out is None:
+        x0_out = torch.empty_like(x)
+    _l.check(_l.load().sdb_ddpm_step(_ptr(x), _ptr(eps), _ptr(noise), sqrt_recip_ac, sqrt_recipm1_ac, coef1, coef2, sigma,
+                                     x.numel(), _ptr(x_out), _ptr(x0_out), _stream()), "sdb_ddpm_step")
+    _count()
+    return x_out, x0_out
+
+
 def layernorm(x, gamma, beta, eps=1e-5, want_f32=False):
     """x fp32 [rows, c] -> fp16 [rows, c]."""
     _chk32(x, "x")

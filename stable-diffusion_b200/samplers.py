@@ -74,6 +74,8 @@ class _SamplerBase:
     # -- model evaluation on the (optionally) guidance-doubled batch
     def _setup_guidance(self, cond, uc, scale, b):
         self._guided = not (uc is None or scale == 1.)
+        if cond is None and self._guided:
+            raise ValueError("classifier-free guidance needs a conditioning")
         self._scale = float(scale)
         if isinstance(cond, dict):
             raise NotImplementedError("dict conditioning (hybrid/concat) is outside the SD-v1 crossattn path")
@@ -81,7 +83,9 @@ class _SamplerBase:
         if self._split:
             self._c_in = self.cfg_parallel.select(uc, cond).contiguous()   # this GPU evaluates one half only
         else:
-            self._c_in = torch.cat([uc, cond]).contiguous() if self._guided else cond.contiguous()
+            # unconditional models (cond None, sample_diffusion.py): no context, no doubled batch
+            self._c_in = torch.cat([uc, cond]).contiguous() if self._guided else \
+                (cond.contiguous() if cond is not None else None)
         self._rep = 2 if (self._guided and not self._split) else 1
         setter = getattr(self.model, "set_context", None)
         if setter is not None:

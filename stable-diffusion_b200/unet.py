@@ -1,6 +1,10 @@
-"""H100-native UNet for the SD-v1 denoising loop: drop-in for the reference's
-`ldm.modules.diffusionmodules.openaimodel.UNetModel` (constructor kwargs openaimodel.py:443-469,
+"""H100-native UNet for the SD-v1 denoising loop and the unconditional attention-block LDMs: drop-in for the
+reference's `ldm.modules.diffusionmodules.openaimodel.UNetModel` (constructor kwargs openaimodel.py:443-469,
 `forward(x, timesteps, context)` openaimodel.py:710-742, state-dict keys unchanged).
+
+Two members of the reference's UNet family run: the SD-v1 spatial-transformer UNet (cross-attention on a context), and
+the unconditional AttentionBlock UNet (use_spatial_transformer=False, e.g. LSUN-Churches) with any combination of
+use_scale_shift_norm and resblock_updown.
 
 Nothing here computes with torch: forward() only sequences the hand-written sm_90a kernels of libsdb200.so
 (ops.py). torch provides device memory and the current stream. nn.Module is used solely so that the reference's
@@ -11,6 +15,8 @@ Data layout: activations NHWC; the residual stream is fp32, tensor-core operands
 GroupNorm/LayerNorm statistics, softmax, FiLM and residual adds are fp32 (SURVEY.md §7.3-1).
 """
 from __future__ import annotations
+
+import math
 
 import torch
 import torch.nn as nn
@@ -94,20 +100,27 @@ class UNetModel(nn.Module):
             context_dim = list(context_dim) if isinstance(context_dim, (list, tuple)) else context_dim
         if num_heads == -1:
             assert num_head_channels != -1, "Either num_heads or num_head_channels has to be set"
-        # the sdb200 path covers the configuration SD v1 ships (v1-inference.yaml:29-44)
-        unsupported = dict(dims=dims != 2, num_classes=num_classes is not None, resblock_updown=resblock_updown,
-                           use_scale_shift_norm=use_scale_shift_norm, n_embed=n_embed is not None,
-                           no_spatial_transformer=not use_spatial_transformer, transformer_depth=transformer_depth != 1,
+        # the sdb200 path covers the configuration SD v1 ships (v1-inference.yaml:29-44) and the unconditional
+        # AttentionBlock family (models/ldm/lsun_churches256/config.yaml: scale-shift norm, up/down ResBlocks)
+        unsupported = dict(dims=dims != 2, num_classes=num_classes is not None, n_embed=n_embed is not None,
                            num_head_channels=num_head_channels != -1, dropout=dropout != 0,
-                           conv_resample=not conv_resample)
+                           conv_resample=not conv_resample, use_new_attention_order=bool(use_new_attention_order),
+                           num_heads_upsample=num_heads_upsample not in (-1, num_heads))
+        if use_spatial_transformer:
+            unsupported.update(resblock_updown=resblock_updown, use_scale_shift_norm=use_scale_shift_norm,
+                               transformer_depth=transformer_depth != 1)
         bad = [k for k, v in unsupported.items() if v]
         if bad:
-            raise NotImplementedError(f"sdb200.UNetModel supports the SD-v1 UNet configuration only; unsupported: {bad}")
+            raise NotImplementedError("sdb200.UNetModel supports the SD-v1 UNet and the unconditional AttentionBlock UNet "
+                                      f"configurations only; unsupported: {bad}")
         self.cfg = dict(image_size=image_size, in_channels=in_channels, model_channels=model_channels,
                         out_channels=out_channels, num_res_blocks=num_res_blocks,
                         attention_resolutions=list(attention_resolutions), channel_mult=list(channel_mult),
-                        num_heads=num_heads, use_spatial_transformer=True, transformer_depth=1,
-                        context_dim=context_dim, legacy=legacy)
+                        num_heads=num_heads, use_spatial_transformer=bool(use_spatial_transformer), transformer_depth=1,
+                        context_dim=context_dim, legacy=legacy, use_scale_shift_norm=bool(use_scale_shift_norm),
+                        resblock_updown=bool(resblock_updown))
+        self.conditional = bool(use_spatial_transformer)   # cross-attention on a context; otherwise forward(x, t)
+        self.image_size = image_size
         self.in_channels, self.model_channels, self.out_channels = in_channels, model_channels, out_channels
         self.num_heads = num_heads
         self.context_dim = context_dim
@@ -118,6 +131,9 @@ class UNetModel(nn.Module):
         # channels per fused GroupNorm-statistics entry: every channel count of the UNet (and of its skip concats) is a
         # multiple of model_channels, so the 32 groups always tile into entries of model_channels / 32 channels
         self._sg = model_channels // 32 if model_channels % 32 == 0 else 1
+        if not self.conditional:
+            # entries must also divide every GEMM tile width (multiples of 32): 192 channels -> 6 per group -> entries of 2
+            self._sg = math.gcd(self._sg, 16)
         self.W = None           # packed weights (device)
         self._ctx_ref = None    # the context tensor whose cross-attention K/V are cached (strong reference)
         self._ctx_ver = -1
@@ -126,6 +142,9 @@ class UNetModel(nn.Module):
         self._graphs = {}
         self._arena = None
         self._side = None       # side stream of the FiLM chain (forked / joined inside every forward, graph-capturable)
+        self._alt_sd = {}       # other weight sets of the same architecture by name (the EMA copy), host tensors
+        self._packed = {}       # name -> (packed weights, captured graphs) of the sets not in use
+        self._active = "raw"
         self.use_cuda_graph = False   # replay one captured graph per UNet evaluation (set by the pipeline / bench)
         self.autotune = True          # graph mode: pick (block_n, split-K) per GEMM problem by measurement before capture
 
@@ -155,9 +174,41 @@ class UNetModel(nn.Module):
             self.pack_weights(probe.device)
         return r
 
+    def set_weight_set(self, name, sd):
+        """Register another state dict of this architecture (UNetModel keys) under `name`, e.g. the EMA weights."""
+        for k, shape in self.shapes.items():
+            assert k in sd and tuple(sd[k].shape) == tuple(shape), f"weight set {name}: {k} missing or misshapen"
+        self._alt_sd[name] = {k: sd[k] for k in self.shapes}
+        self._packed.pop(name, None)
+
+    def has_weight_set(self, name):
+        return name in self._alt_sd
+
     @torch.no_grad()
-    def pack_weights(self, device):
-        sd = {k: v.detach().to(device=device, dtype=torch.float32) for k, v in self._host_sd.items()}
+    def use_weight_set(self, name="raw"):
+        """Run on the weights registered under `name` ("raw": the loaded state dict). Each set is packed once and keeps
+        its own captured CUDA graphs, so switching back and forth costs no repacking."""
+        if name == self._active:
+            return
+        assert name == "raw" or name in self._alt_sd, f"no weight set {name}"
+        if self.W is not None:
+            self._packed[self._active] = (self.W, self._graphs)
+            dev = self.W["device"]
+            if name in self._packed:
+                self.W, self._graphs = self._packed.pop(name)
+                self._ctx_ref = None      # cross-attention K / V are recomputed with this set's weights
+            else:
+                self._active = name
+                self.pack_weights(dev, keep_sets=True)
+        self._active = name
+
+    @torch.no_grad()
+    def pack_weights(self, device, keep_sets=False):
+        if not keep_sets:       # fresh weights: every packed set is stale
+            self._packed = {}
+            self._active = "raw"
+        src = self._host_sd if self._active == "raw" else self._alt_sd[self._active]
+        sd = {k: v.detach().to(device=device, dtype=torch.float32) for k, v in src.items()}
         W = {"device": device}
         f32 = lambda k: sd[k].contiguous()
         f16 = lambda k: sd[k].half().contiguous()
@@ -173,7 +224,8 @@ class UNetModel(nn.Module):
 
         def pack_res(pre, a):
             nonlocal off
-            r = {"cin": a["cin"], "cout": a["cout"]}
+            r = {"cin": a["cin"], "cout": a["cout"], "ss": a.get("ss", False), "updown": a.get("updown")}
+            assert r["updown"] is None or a["cin"] == a["cout"]
             r["gn1"] = (f32(pre + ".in_layers.0.weight"), f32(pre + ".in_layers.0.bias"))
             r["w1"], r["b1"] = _pack_conv3(sd[pre + ".in_layers.2.weight"]), f32(pre + ".in_layers.2.bias")
             r["gn2"] = (f32(pre + ".out_layers.0.weight"), f32(pre + ".out_layers.0.bias"))
@@ -184,8 +236,30 @@ class UNetModel(nn.Module):
             emb_w.append(sd[pre + ".emb_layers.1.weight"].half())
             emb_b.append(sd[pre + ".emb_layers.1.bias"])
             r["film_off"] = off
-            off += a["cout"]
+            off += 2 * a["cout"] if r["ss"] else a["cout"]     # [scale | shift] with use_scale_shift_norm
             return r
+
+        def pack_attn(pre, a):
+            """AttentionBlock (openaimodel.py:278-324) with QKVAttentionLegacy: qkv rows are [head][q | k | v][ch]. They
+            are repacked into head-padded Q|K and V weights for the flash kernel. The V bias is folded into proj_out:
+            softmax rows sum to one, so P (V + 1 b_v^T) = P V + 1 b_v^T, and proj_out(o + b_v) = W_p o + (W_p b_v + b_p)."""
+            ch, d = a["ch"], a["dhead"]
+            hh = a["heads"]
+            dp = _dpad(d)
+            w = sd[pre + ".qkv.weight"].reshape(hh, 3, d, ch)
+            b = sd[pre + ".qkv.bias"].reshape(hh, 3, d)
+            s = {"ch": ch, "d": d, "dpad": dp, "heads": hh}
+            s["gn"] = (f32(pre + ".norm.weight"), f32(pre + ".norm.bias"))
+            s["w_qk"] = torch.cat([_pack_heads(w[:, 0].reshape(hh * d, ch), hh, d, dp),
+                                   _pack_heads(w[:, 1].reshape(hh * d, ch), hh, d, dp)], 0).contiguous()
+            bq = torch.zeros((2, hh, dp), dtype=torch.float32, device=device)
+            bq[0, :, :d], bq[1, :, :d] = b[:, 0], b[:, 1]
+            s["b_qk"] = bq.reshape(-1).contiguous()
+            s["w_v"] = _pack_heads(w[:, 2].reshape(hh * d, ch), hh, d, dp)
+            wp = sd[pre + ".proj_out.weight"].reshape(ch, ch)
+            s["w_proj"] = wp.half().contiguous()
+            s["b_proj"] = (sd[pre + ".proj_out.bias"].double() + wp.double() @ b[:, 2].reshape(-1).double()).float().contiguous()
+            return s
 
         def pack_st(pre, a):
             ch, d = a["ch"], a["dhead"]
@@ -219,6 +293,8 @@ class UNetModel(nn.Module):
                     out.append((kind, pack_res(pre, a)))
                 elif kind == "st":
                     out.append((kind, pack_st(pre, a)))
+                elif kind == "attn":
+                    out.append((kind, pack_attn(pre, a)))
                 elif kind == "down":
                     out.append((kind, {"w": _pack_conv3(sd[pre + ".op.weight"]), "b": f32(pre + ".op.bias"), "ch": a["ch"]}))
                 elif kind == "up":
@@ -251,17 +327,30 @@ class UNetModel(nn.Module):
 
     def _res(self, r, h, skip, film, emit_f16=False):
         """ResBlock._forward (openaimodel.py:255-275); `skip` is the UNet skip tensor concatenated along C.
-        emit_f16: the last GEMM also writes an fp16 copy of the block output (operand of a following stride-2 conv)."""
-        nb, H, Wd, _ = h.shape
+        emit_f16: the last GEMM also writes an fp16 copy of the block output (operand of a following stride-2 conv).
+        Up / down blocks resample inside the first GroupNorm kernel (h_upd) and through sdb_resample_f32 (x_upd); with
+        scale-shift norm the FiLM vector modulates the second GroupNorm instead of being added by the first conv."""
         x3 = self.W["x3"] and "ws" in r
-        if x3:
+        raw = raw_lo = None
+        if r["updown"] is not None:
+            assert skip is None
+            mode = 1 if r["updown"] == "down" else 2
+            hn = ops.groupnorm_mod(h, *r["gn1"], resample=mode, eps=1e-5, silu=True)
+            h = ops.resample_f32(h, mode)
+        elif x3:
             hn, raw, _, raw_lo = ops.groupnorm(h, *r["gn1"], x1=skip, eps=1e-5, silu=True, want_raw_lo=True)
         else:
             hn, raw = ops.groupnorm(h, *r["gn1"], x1=skip, eps=1e-5, silu=True, want_raw="ws" in r)
-        fv = film[:, r["film_off"]: r["film_off"] + r["cout"]]
-        _, h1 = ops.gemm(hn, r["w1"], taps=9, bias=r["b1"], film=fv, want_f32=True, splits=-1, want_stats=True, stats_group=self._sg)
-        h1 = h1.view(nb, H, Wd, r["cout"])
-        hn2, _ = ops.groupnorm(h1, *r["gn2"], eps=1e-5, silu=True)
+        nb, H, Wd, _ = h.shape
+        fo, co = r["film_off"], r["cout"]
+        _, h1 = ops.gemm(hn, r["w1"], taps=9, bias=r["b1"], film=None if r["ss"] else film[:, fo: fo + co], want_f32=True,
+                         splits=-1, want_stats=True, stats_group=self._sg)
+        h1 = h1.view(nb, H, Wd, co)
+        if r["ss"]:
+            hn2 = ops.groupnorm_mod(h1, *r["gn2"], scale=film[:, fo: fo + co], shift=film[:, fo + co: fo + 2 * co],
+                                    eps=1e-5, silu=True)
+        else:
+            hn2, _ = ops.groupnorm(h1, *r["gn2"], eps=1e-5, silu=True)
         if x3:    # skip 1x1 conv on the raw stream: [x_hi | x_lo | x_hi] . [W_hi | W_hi | W_lo]
             _, res = ops.gemm(raw, r["ws"], a1=raw_lo, a2=raw, bias=r["bs"], want_f32=True, splits=-1)
         elif "ws" in r:
@@ -326,6 +415,32 @@ class UNetModel(nn.Module):
             out._sdb_f16 = o16.view(nb, H, Wd, ch)
         return out
 
+    def _attn(self, s, x, emit_f16=False):
+        """AttentionBlock._forward (openaimodel.py:318-324) with QKVAttentionLegacy (:347-372) on the flash kernel.
+        The reference scales q and k by ch^-0.25 each; the kernel applies ch^-0.5 to the product."""
+        nb, H, Wd, ch = x.shape
+        ntok = H * Wd
+        heads, d, dp = s["heads"], s["d"], s["dpad"]
+        hd = heads * dp
+        xn, _ = ops.groupnorm(x, *s["gn"], eps=1e-5, silu=False)
+        xm = xn.view(-1, ch)
+        qk, _ = ops.gemm(xm, s["w_qk"], bias=s["b_qk"], want_f16=True)                     # [M, 2*hd]
+        qk3 = qk.view(nb, ntok, 2 * hd)
+        if ntok % 8 == 0:
+            vt, _ = ops.gemm(s["w_v"], xm, want_f16=True, b_dynamic=True)                    # V^T [hd, M]
+            vt3 = vt.view(hd, nb, ntok).permute(1, 0, 2)
+        else:  # TMA needs 16-byte aligned strides: the 4x4 / 2x2 levels go through an explicit transpose
+            v, _ = ops.gemm(xm, s["w_v"], want_f16=True)
+            vt3 = ops.transpose_f16(v.view(nb, ntok, hd))
+        o = ops.attention(qk3[:, :, :hd], qk3[:, :, hd:], vt3, heads=heads, d=d, dpad=dp, nq=ntok, nkv=ntok,
+                          scale=d ** -0.5)
+        o16, out = ops.gemm(o.view(-1, ch), s["w_proj"], bias=s["b_proj"], residual=x.view(-1, ch), want_f32=True,
+                            want_f16=emit_f16, splits=-1, rows_per_sample=ntok, want_stats=True, stats_group=self._sg)
+        out = out.view(nb, H, Wd, ch)
+        if emit_f16:
+            out._sdb_f16 = o16.view(nb, H, Wd, ch)
+        return out
+
     def context_kv(self, context, static=False):
         """Cross-attention K and V^T for all SpatialTransformers (x/t independent: once per prompt).
         static=True writes into persistent per-shape buffers so captured CUDA graphs stay valid across prompts."""
@@ -376,6 +491,8 @@ class UNetModel(nn.Module):
             elif kind == "st":
                 h = self._st(p, h, kvs[st_idx[0]], emit_f16=last)
                 st_idx[0] += 1
+            elif kind == "attn":
+                h = self._attn(p, h, emit_f16=last)
             elif kind == "down":
                 # Downsample (openaimodel.py:149-153): 3x3, stride 2, pad 1, straight from the NHWC activation through
                 # strided TMA boxes (element strides {1,2,2,1}); no im2col buffer
@@ -474,8 +591,9 @@ class UNetModel(nn.Module):
 
     # ------------------------------------------------------------------ handle-level C entry (include/sdb200.h)
     @torch.no_grad()
-    def c_handle(self, shape, context):
-        """Build the C-side handle of one guided evaluation for latents of `shape` = (n, c, h, w) and the given context:
+    def c_handle(self, shape, context=None):
+        """Build the C-side handle of one guided evaluation for latents of `shape` = (n, c, h, w) and the given context
+        (None for the unconditional model):
         walks the model once between sdb_plan_begin / sdb_plan_end (every launch is recorded with its arguments; the
         pass doubles as warm-up), then wraps the plan and its static x / t / eps buffers in an sdb_unet. Afterwards
         `sdb_unet_forward(handle, x, t, eps, stream)` and `sdb_sample_plms` run without any Python on the hot path.
@@ -484,7 +602,8 @@ class UNetModel(nn.Module):
         from . import lib as _l
         lib = _l.load()
         dev = self.W["device"]
-        kvs = self.set_context(context)
+        self._check_context(context, shape[0])
+        kvs = self.set_context(context) if self.conditional else None
         x = torch.zeros(shape, dtype=torch.float32, device=dev)
         t = torch.zeros((shape[0],), dtype=torch.float32, device=dev)
         ops.AUTOTUNE = self.autotune
@@ -507,6 +626,13 @@ class UNetModel(nn.Module):
                                      shape[0], shape[1], eps.shape[1], shape[2], shape[3], C.byref(h)), "sdb_unet_create")
         return CUNet(h, plan, pool, (x, t, eps, kvs, context), int(lib.sdb_plan_size(plan)))
 
+    def _check_context(self, context, nb):
+        if not self.conditional:
+            if context is not None:
+                raise ValueError("this UNet is unconditional (no spatial transformer): call forward(x, t) without a context")
+            return
+        assert context is not None and context.shape[0] == nb and context.shape[2] == self.context_dim
+
     @torch.no_grad()
     def forward(self, x, timesteps=None, context=None, y=None, **kwargs):
         assert y is None, "must specify y if and only if the model is class-conditional"
@@ -514,10 +640,12 @@ class UNetModel(nn.Module):
         if not x.is_cuda:
             raise RuntimeError("sdb200.UNetModel runs on CUDA (sm_90a) only; there is no CPU fallback")
         assert x.dim() == 4 and x.shape[1] == self.in_channels
-        assert context is not None and context.shape[0] == x.shape[0] and context.shape[2] == self.context_dim
+        self._check_context(context, x.shape[0])
         nb, _, H, Wd = x.shape
         lv = len(self.cfg["channel_mult"]) - 1
         assert H % (1 << lv) == 0 and Wd % (1 << lv) == 0, "latent size must be divisible by 2^(levels-1)"
+        if not self.conditional:
+            return self._forward_uncond(x, timesteps)
         cached = self._context_cached(context)
         if self.use_cuda_graph:
             if not cached:
@@ -536,6 +664,18 @@ class UNetModel(nn.Module):
         t = timesteps.to(torch.float32).contiguous()
         eps = self._forward_impl(x.contiguous().float(), t, kvs)
         return eps.to(x.dtype)
+
+    def _forward_uncond(self, x, timesteps):
+        if self.use_cuda_graph:
+            g = self._graph_for(tuple(x.shape), None)
+            if x.data_ptr() != g["x"].data_ptr():
+                g["x"].copy_(x)
+            g["t"].copy_(timesteps)
+            g["graph"].replay()
+            ops.add_graph_launches(g["launches"])
+            return g["out"].clone() if x.dtype == torch.float32 else g["out"].to(x.dtype)
+        t = timesteps.to(torch.float32).contiguous()
+        return self._forward_impl(x.contiguous().float(), t, None).to(x.dtype)
 
 
 class CUNet:
