@@ -257,6 +257,13 @@ int sdb_resample_f32(const float* x, int32_t nb, int32_t h, int32_t w, int32_t c
 int sdb_ddpm_step(const float* x, const float* eps, const float* noise, float sqrt_recip_alphas_cumprod,
                   float sqrt_recipm1_alphas_cumprod, float posterior_mean_coef1, float posterior_mean_coef2, float sigma,
                   int64_t n, float* x_out, float* x0_out, sdb_stream_t stream);
+/* Vector quantizer of a VQ first stage (taming VectorQuantizer2.forward, legacy, no remap): z fp32 NHWC [m, e_dim],
+ * first multiplied by `scale` (1 / scale_factor of decode_first_stage); codebook fp32 [n_e, e_dim] with code_sq[j] =
+ * sum(codebook[j]^2) precomputed once per weight load. Index = argmin_j sum(z^2) + code_sq[j] - 2 z.e_j, the lowest
+ * index on ties; z_q = z + (e - z) in fp32 (the straight-through value, not always e bit for bit). indices (int64 [m])
+ * may be NULL. e_dim 1 .. 8, any n_e (the codebook streams through shared memory). */
+int sdb_vq_quantize(const float* z, int64_t m, int32_t e_dim, float scale, const float* codebook, const float* code_sq,
+                    int32_t n_e, float* z_q, int64_t* indices, sdb_stream_t stream);
 /* out = a*x + b (latent scaling z/0.18215, ddpm.py:713) */
 int sdb_axpby(const float* x, float a, float b, int64_t n, float* out, sdb_stream_t stream);
 /* out = a*x + b*y (DDIMSampler.stochastic_encode, ddim.py:206-220; q_sample, ddpm.py:274-277) */

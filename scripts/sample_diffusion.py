@@ -4,6 +4,10 @@ CompVis/stable-diffusion), e.g. the LSUN-Churches KL-f8 model:
 
   python scripts/sample_diffusion.py -r models/ldm/lsun_churches256/model.ckpt -n 50 -c 50 -e 1.0 -l outputs/lsun
 
+or the VQ-f4 models (CelebA-HQ, FFHQ, LSUN-Bedrooms: configs/latent-diffusion/*-ldm-vq-4.yaml), e.g.
+
+  python scripts/sample_diffusion.py -r models/ldm/celeba256/model.ckpt -n 50 -c 50 -e 0 -l outputs/celeba
+
 -r is a checkpoint (its directory holds config.yaml) or a logdir holding model.ckpt and config.yaml. DDIM with eta
 (default 1.0) or, with -v, the ancestral sampler over all training steps (progressive_denoising). Sampling runs inside
 ema_scope(), so checkpoints with EMA copies sample with them. With --random_init no checkpoint is read: the UNet and the
@@ -39,6 +43,22 @@ def lsun_churches_config(unet_cfg=None, vae_cfg=None):
         "unet_config": {"target": "ldm.modules.diffusionmodules.openaimodel.UNetModel", "params": u},
         "first_stage_config": {"target": "ldm.models.autoencoder.AutoencoderKL",
                                "params": {**v, "monitor": "val/rec_loss", "lossconfig": {"target": "torch.nn.Identity"}}},
+        "cond_stage_config": "__is_unconditional__"}}
+
+
+def celebahq_config(unet_cfg=None, vq_cfg=None):
+    """configs/latent-diffusion/celebahq-ldm-vq-4.yaml, `model:` node (reference targets); the FFHQ and LSUN-Bedrooms
+    configs differ only in their data and first-stage ckpt_path."""
+    u = dict(unet_cfg or arch.CELEBAHQ_UNET)
+    v = dict(vq_cfg or arch.VQ_F4)
+    return {"target": "ldm.models.diffusion.ddpm.LatentDiffusion", "params": {
+        "linear_start": 0.0015, "linear_end": 0.0195, "num_timesteps_cond": 1, "log_every_t": 200, "timesteps": 1000,
+        "first_stage_key": "image", "image_size": u["image_size"], "channels": u["in_channels"],
+        "monitor": "val/loss_simple_ema",
+        "unet_config": {"target": "ldm.modules.diffusionmodules.openaimodel.UNetModel", "params": u},
+        "first_stage_config": {"target": "ldm.models.autoencoder.VQModelInterface",
+                               "params": {**v, "ckpt_path": "models/first_stage_models/vq-f4/model.ckpt",
+                                          "lossconfig": {"target": "torch.nn.Identity"}}},
         "cond_stage_config": "__is_unconditional__"}}
 
 

@@ -51,6 +51,21 @@ TINY_ATTN_PLAIN_UNET = dict(image_size=16, in_channels=4, out_channels=4, model_
                             attention_resolutions=[2, 4], num_res_blocks=1, channel_mult=[1, 2, 5], num_heads=8,
                             use_scale_shift_norm=False, resblock_updown=False, use_spatial_transformer=False,
                             context_dim=None, legacy=True)
+# the unconditional VQ-f4 LDMs (configs/latent-diffusion/celebahq-ldm-vq-4.yaml; ffhq- and lsun_bedrooms-ldm-vq-4 share
+# the UNet and the first stage): plain ResBlocks, AttentionBlocks of num_head_channels 32 (14, 21, 28 heads of d = 32).
+# Widths 224 .. 896 and the skip concats 672, 1120, 1568 are multiples of 32, not all of 64.
+CELEBAHQ_UNET = dict(image_size=64, in_channels=3, out_channels=3, model_channels=224, attention_resolutions=[8, 4, 2],
+                     num_res_blocks=2, channel_mult=[1, 2, 3, 4], num_head_channels=32)
+# a small member for tests: widths 96 / 192 / 288, concats 288 and 480; 3 and 9 channels per GroupNorm group
+TINY_VQ_UNET = dict(image_size=16, in_channels=3, out_channels=3, model_channels=96, attention_resolutions=[2, 4],
+                    num_res_blocks=1, channel_mult=[1, 2, 3], num_head_channels=32)
+# VQModelInterface first stages (models/first_stage_models/vq-f4/config.yaml) and a small member
+VQ_F4 = dict(embed_dim=3, n_embed=8192, ddconfig=dict(double_z=False, z_channels=3, resolution=256, in_channels=3, out_ch=3,
+                                                       ch=128, ch_mult=[1, 2, 4], num_res_blocks=2, attn_resolutions=[],
+                                                       dropout=0.0))
+TINY_VQ = dict(embed_dim=3, n_embed=512, ddconfig=dict(double_z=False, z_channels=3, resolution=32, in_channels=3, out_ch=3,
+                                                        ch=64, ch_mult=[1, 2], num_res_blocks=1, attn_resolutions=[],
+                                                        dropout=0.0))
 TINY_VAE = dict(embed_dim=4, ddconfig=dict(double_z=True, z_channels=4, resolution=32, in_channels=3, out_ch=3,
                                            ch=64, ch_mult=[1, 2], num_res_blocks=1, attn_resolutions=[],
                                            dropout=0.0))
@@ -65,13 +80,15 @@ def unet_plan(cfg):
     kinds: conv_in, res(cin, cout, ss, updown), st(ch, heads, dhead), attn(ch, heads, dhead), down(ch), up(ch), out.
     Mirrors the constructor loops at openaimodel.py:512-686. Without a spatial transformer the attention layers are
     AttentionBlocks with `num_heads` heads of ch / num_heads channels (legacy=True passes num_head_channels=-1,
-    openaimodel.py:547-549); `ss` is use_scale_shift_norm; with resblock_updown the Downsample / Upsample layers are
+    openaimodel.py:547-549), or, when num_head_channels is set, ch / num_head_channels heads of num_head_channels
+    (openaimodel.py:542-546); `ss` is use_scale_shift_norm; with resblock_updown the Downsample / Upsample layers are
     ResBlocks with updown "down" / "up" (openaimodel.py:567-582, 664-677).
     """
     mc = cfg["model_channels"]
     mult = cfg["channel_mult"]
     nrb = cfg["num_res_blocks"]
-    heads = cfg["num_heads"]
+    nh = cfg.get("num_heads", -1)
+    nhc = cfg.get("num_head_channels", -1)
     attn_res = set(cfg["attention_resolutions"])
     st = cfg.get("use_spatial_transformer", False)
     ss = bool(cfg.get("use_scale_shift_norm", False))
@@ -80,6 +97,10 @@ def unet_plan(cfg):
 
     def res(pre, cin, cout, ud=None, **kw):
         return ("res", pre, dict(cin=cin, cout=cout, ss=ss, updown=ud, **kw))
+
+    def att(pre, ch):
+        heads = nh if nhc == -1 else ch // nhc
+        return (akind, pre, dict(ch=ch, heads=heads, dhead=ch // heads))
 
     plan = {"input": [], "middle": [], "output": []}
     plan["input"].append([("conv_in", "input_blocks.0.0", dict(cin=cfg["in_channels"], cout=mc))])
@@ -90,7 +111,7 @@ def unet_plan(cfg):
             layers = [res(f"input_blocks.{idx}.0", ch, m * mc)]
             ch = m * mc
             if ds in attn_res:
-                layers.append((akind, f"input_blocks.{idx}.1", dict(ch=ch, heads=heads, dhead=ch // heads)))
+                layers.append(att(f"input_blocks.{idx}.1", ch))
             plan["input"].append(layers)
             chans.append(ch)
             idx += 1
@@ -101,7 +122,7 @@ def unet_plan(cfg):
             idx += 1
             ds *= 2
     plan["middle"] = [res("middle_block.0", ch, ch),
-                      (akind, "middle_block.1", dict(ch=ch, heads=heads, dhead=ch // heads)),
+                      att("middle_block.1", ch),
                       res("middle_block.2", ch, ch)]
     idx = 0
     for level, m in list(enumerate(mult))[::-1]:
@@ -111,7 +132,7 @@ def unet_plan(cfg):
             ch = mc * m
             sub = 1
             if ds in attn_res:
-                layers.append((akind, f"output_blocks.{idx}.{sub}", dict(ch=ch, heads=heads, dhead=ch // heads)))
+                layers.append(att(f"output_blocks.{idx}.{sub}", ch))
                 sub += 1
             if level and i == nrb:
                 layers.append(res(f"output_blocks.{idx}.{sub}", ch, ch, "up") if updown else
@@ -300,6 +321,22 @@ def vae_param_shapes(cfg):
     return p
 
 
+def vq_param_shapes(cfg):
+    """Keys as VQModelInterface.state_dict() (autoencoder.py:14-44, 264-282): encoder.* and decoder.* (double_z False),
+    quantize.embedding.weight [n_embed, embed_dim], quant_conv (z -> embed) and post_quant_conv (embed -> z)."""
+    dd = cfg["ddconfig"]
+    assert not dd["double_z"], "VQ first stages have double_z False"
+    kl = vae_param_shapes(dict(embed_dim=cfg["embed_dim"], ddconfig=dd))
+    zc, ed = dd["z_channels"], cfg["embed_dim"]
+    p = OrderedDict((k, v) for k, v in kl.items() if k.startswith(("encoder.", "decoder.")))
+    p["quantize.embedding.weight"] = (cfg["n_embed"], ed)
+    p["quant_conv.weight"] = (ed, zc, 1, 1)
+    p["quant_conv.bias"] = (ed,)
+    p["post_quant_conv.weight"] = (zc, ed, 1, 1)
+    p["post_quant_conv.bias"] = (zc,)
+    return p
+
+
 # ------------------------------------------------------------------------------------------------ CLIP
 def clip_param_shapes(cfg):
     """Keys as transformers CLIPTextModel.state_dict() (`text_model.*`); in an SD checkpoint they sit under
@@ -390,6 +427,8 @@ def random_state_dict(shapes, seed, prefix="", device="cpu"):
             t = 0.15 + 0.05 * rn()
         elif _is_norm_key(k):
             t = 1.0 + 0.1 * rn()
+        elif k.endswith("quantize.embedding.weight"):   # VQ codebook: unit scale, or every z_q collapses towards 0
+            t = rn()
         elif "embedding" in k:
             t = 0.02 * rn()
         else:

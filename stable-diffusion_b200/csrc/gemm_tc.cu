@@ -106,10 +106,13 @@ static int make_geometry(const sdb_gemm_desc* d, Geometry* g) {
   int nsrc = 0, chunks = 0;
   for (int i = 0; i < MAX_SRC; ++i) {
     if (srcs[i] == nullptr) break;
-    SDB_CHECK(chans[i] > 0 && chans[i] % 64 == 0, "sdb_gemm: channel count of source %d must be a positive multiple of 64 (got %d)",
+    // a width that is a multiple of 32 only takes ceil(c / 64) K steps: the A map keeps dims[0] = c, so TMA's
+    // out-of-bounds fill supplies zeros for the channels c .. ceil64(c) - 1 of the last step
+    SDB_CHECK(chans[i] > 0 && chans[i] % 32 == 0,
+              "sdb_gemm: channel count of source %d must be a positive multiple of 64, or of 32 (tail zero-filled) (got %d)",
               i, chans[i]);
     ++nsrc;
-    chunks += chans[i] / 64;
+    chunks += (chans[i] + 63) / 64;
   }
   for (int i = nsrc; i < MAX_SRC; ++i)
     SDB_CHECK(srcs[i] == nullptr && chans[i] == 0, "sdb_gemm: A sources must be contiguous (a%d/c%d)", i, i);
@@ -245,18 +248,15 @@ extern "C" int sdb_gemm(const sdb_gemm_desc* d, sdb_stream_t stream) {
   SDB_CHECK(!geglu || d->n % bn == 0, "sdb_gemm: GEGLU needs n %% block_n == 0");
 
   GemmArgs p{};
-  int nsrc = 0, ctot = 0;
-  for (int i = 0; i < MAX_SRC && srcs[i]; ++i) {
-    ++nsrc;
-    ctot += chans[i];
-  }
+  int nsrc = 0;
+  for (int i = 0; i < MAX_SRC && srcs[i]; ++i) ++nsrc;
   const long M = g.M;
   p.M = static_cast<int>(M);
   p.N = d->n;
   p.taps = d->taps;
   p.nsrc = nsrc;
   p.cb[0] = 0;
-  for (int i = 0; i < nsrc; ++i) p.cb[i + 1] = p.cb[i] + chans[i] / 64;
+  for (int i = 0; i < nsrc; ++i) p.cb[i + 1] = p.cb[i] + (chans[i] + 63) / 64;
   for (int i = nsrc; i < MAX_SRC; ++i) p.cb[i + 1] = p.cb[nsrc];
   p.k_iters = g.k_iters;
   p.H = d->h;
@@ -334,7 +334,10 @@ extern "C" int sdb_gemm(const sdb_gemm_desc* d, sdb_stream_t stream) {
   }
   for (int i = nsrc; i < MAX_SRC; ++i) tm.a[i] = tm.a[0];
   {
-    uint64_t K = static_cast<uint64_t>(d->taps) * ctot;
+    // B rows: taps * sum(ceil64(c_i)) columns, each source's padded tail zero; one source of one tap may be exactly
+    // c wide (the tail step then reads TMA's out-of-bounds zeros, as for A)
+    const uint64_t K = (nsrc == 1 && d->taps == 1) ? static_cast<uint64_t>(chans[0])
+                                                    : static_cast<uint64_t>(d->taps) * g.cpt * 64;
     uint64_t dims[2] = {K, static_cast<uint64_t>(d->n)};
     uint64_t str[1] = {K * 2};
     uint32_t box[2] = {64, static_cast<uint32_t>(bn / ch.cg)};   // a CTA of a pair loads (and multicasts) half of the weight tile

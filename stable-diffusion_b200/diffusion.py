@@ -1,7 +1,7 @@
 """LatentDiffusion facade: the inference surface of `ldm.models.diffusion.ddpm.LatentDiffusion` that the scripts and
 samplers use (ddpm.py): register_schedule (:117-169), apply_model (:891-992 plain path) through a DiffusionWrapper
 (:1393-1421 crossattn branch), get_learned_conditioning (:551-562), encode_first_stage (:825-863),
-get_first_stage_encoding (:542-549), decode_first_stage (:705-763), q_sample (:274-277), ema_scope (:171-184).
+get_first_stage_encoding (:542-549), decode_first_stage (:705-763, KL and VQ first stages), q_sample (:274-277), ema_scope (:171-184).
 Sub-modules keep the reference attribute names so checkpoint prefixes resolve:
 `model.diffusion_model.*`, `first_stage_model.*`, `cond_stage_model.transformer.*`, `model_ema.*`.
 Unconditional models (cond_stage_config "__is_unconditional__", e.g. LSUN-Churches) sample through DDIM with no
@@ -19,6 +19,7 @@ import torch.nn as nn
 
 from . import ops
 from .util import instantiate_from_config, remap_config
+from .vq import VQModelInterface
 
 
 class DiffusionWrapper(nn.Module):
@@ -183,7 +184,11 @@ class LatentDiffusion(nn.Module):
         raise NotImplementedError(f"encoder_posterior of type '{type(encoder_posterior)}' not yet implemented")
 
     def decode_first_stage(self, z, predict_cids=False, force_not_quantize=False):
-        assert not predict_cids
+        if predict_cids:
+            raise NotImplementedError("decode_first_stage(predict_cids=True): codebook-index latents are not supported")
+        if isinstance(self.first_stage_model, VQModelInterface):     # ddpm.py:753-761: quantize, then decode
+            return self.first_stage_model.decode(z, force_not_quantize=force_not_quantize,
+                                                 scale=1. / float(self.scale_factor))
         return self.first_stage_model.decode(z, scale=1. / float(self.scale_factor))
 
     def q_sample(self, x_start, t, noise=None):

@@ -87,6 +87,7 @@ SIGNATURES = {
     "sdb_groupnorm_mod": ([_P, _I, _I, _I, _I, _I, _P, _P, _F, _I, _P, _P, _I, _I, _P, _P, _P, _I, _I, _P], C.c_int),
     "sdb_resample_f32": ([_P, _I, _I, _I, _I, _I, _P, _P], C.c_int),
     "sdb_ddpm_step": ([_P, _P, _P, _F, _F, _F, _F, _F, _L, _P, _P, _P], C.c_int),
+    "sdb_vq_quantize": ([_P, _L, _I, _F, _P, _P, _I, _P, _P, _P], C.c_int),
     "sdb_layernorm": ([_P, _I, _I, _P, _P, _F, _P, _P, _P], C.c_int),
     "sdb_softmax_rows": ([_P, _I, _I, _F, _P, _P], C.c_int),
     "sdb_nchw_to_nhwc": ([_P, _I, _I, _I, _P, _P, _P], C.c_int),

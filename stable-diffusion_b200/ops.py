@@ -90,7 +90,10 @@ def gemm(a0, b, *, a1=None, a2=None, a3=None, nb=None, h=None, w=None, taps=1, b
         rows = a0.numel() // c0
         nb, h, w = 1, 1, rows
     n = b.shape[0] if n is None else n
-    assert b.shape[1] == taps * sum(chans), (b.shape, taps, chans)
+    # B rows hold taps * sum(ceil64(c_i)) columns (zero tails pad a source whose width is a multiple of 32 only to whole
+    # 64-wide K steps); one source of one tap may be exactly c wide
+    kb = chans[0] if (len(srcs) == 1 and taps == 1) else taps * sum((c_ + 63) // 64 * 64 for c_ in chans)
+    assert b.shape[1] == kb, (b.shape, taps, chans)
     M = nb * h * w
     n_out = n // 2 if act == ACT_GEGLU else n
     if out_f16 is None and (want_f16 or want_lo):
@@ -159,7 +162,7 @@ def gemm(a0, b, *, a1=None, a2=None, a3=None, nb=None, h=None, w=None, taps=1, b
         out_f32._sdb_stats = (stats, plan[4], stats_group)   # travels with the tensor object (and, through ._base, its views)
     if RECORD is not None:
         # operand-split passes ([A_hi|A_lo|A_hi]) are overhead, not algorithmic work: count K once
-        k_alg = b.shape[1] // 3 if (len(srcs) == 3 and srcs[0] is srcs[2]) else b.shape[1]
+        k_alg = taps * sum(chans) // 3 if (len(srcs) == 3 and srcs[0] is srcs[2]) else taps * sum(chans)
         RECORD.append((d, 2.0 * M * n * k_alg, (srcs, b, bias, film, residual, out_f16, out_f32, out_f16_lo, workspace, stats)))
     if PROFILE is not None:
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -393,6 +396,23 @@ def ddpm_step(x, eps, noise, *, sqrt_recip_ac, sqrt_recipm1_ac, coef1, coef2, si
                                      x.numel(), _ptr(x_out), _ptr(x0_out), _stream()), "sdb_ddpm_step")
     _count()
     return x_out, x0_out
+
+
+def vq_quantize(z, codebook, code_sq, scale=1.0, want_indices=False):
+    """Nearest-codebook quantization (sdb_vq_quantize): z fp32 NHWC [..., e_dim] (times `scale` first), codebook fp32
+    [n_e, e_dim], code_sq its squared row norms. Returns z_q (same shape), or (z_q, int64 indices [rows])."""
+    _chk32(z, "z")
+    _chk32(codebook, "codebook")
+    _chk32(code_sq, "code_sq")
+    n_e, e_dim = codebook.shape
+    assert z.shape[-1] == e_dim and code_sq.shape == (n_e,)
+    rows = z.numel() // e_dim
+    z_q = torch.empty_like(z)
+    idx = torch.empty(rows, dtype=torch.int64, device=z.device) if want_indices else None
+    _l.check(_l.load().sdb_vq_quantize(_ptr(z), rows, e_dim, scale, _ptr(codebook), _ptr(code_sq), n_e, _ptr(z_q),
+                                       _ptr(idx), _stream()), "sdb_vq_quantize")
+    _count()
+    return (z_q, idx) if want_indices else z_q
 
 
 def layernorm(x, gamma, beta, eps=1e-5, want_f32=False):

@@ -139,7 +139,7 @@ class _SamplerBase:
         if kw.get("mask") is not None:
             assert kw.get("x0") is not None   # plms.py:148 / ddim.py:145
         if kw.get("quantize_x0"):
-            raise NotImplementedError("quantize_x0 needs a VQ first stage (not SD v1)")
+            raise NotImplementedError("quantize_x0 is not implemented (it would split the fused sampler update)")
         if kw.get("noise_dropout", 0.) != 0.:
             raise NotImplementedError("noise_dropout")
 

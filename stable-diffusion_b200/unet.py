@@ -4,7 +4,7 @@ reference's `ldm.modules.diffusionmodules.openaimodel.UNetModel` (constructor kw
 
 Two members of the reference's UNet family run: the SD-v1 spatial-transformer UNet (cross-attention on a context), and
 the unconditional AttentionBlock UNet (use_spatial_transformer=False, e.g. LSUN-Churches) with any combination of
-use_scale_shift_norm and resblock_updown.
+use_scale_shift_norm and resblock_updown, or with plain ResBlocks and heads of num_head_channels (the VQ-f4 models).
 
 Nothing here computes with torch: forward() only sequences the hand-written sm_90a kernels of libsdb200.so
 (ops.py). torch provides device memory and the current stream. nn.Module is used solely so that the reference's
@@ -31,13 +31,20 @@ def _dpad(d):
     return (d + 63) // 64 * 64
 
 
-def _pack_conv3(w):  # [Cout, Cin, 3, 3] -> [Cout, 9*Cin], k = (ky*3+kx)*Cin + c
-    return w.permute(0, 2, 3, 1).reshape(w.shape[0], -1).contiguous().half()
+def _pad64(w):
+    """Zero columns up to the GEMM's 64-wide K step for a source width that is a multiple of 32 but not of 64 (the GEMM
+    reads the tail of such a source as zeros); other widths are returned unchanged."""
+    c = w.shape[-1]
+    return torch.nn.functional.pad(w, (0, 32)) if c % 64 == 32 else w
 
 
-def _pack_conv3_padk(w, kpad):  # small-Cin convs through im2col: K zero-padded to kpad
+def _pack_conv3(w):  # [Cout, Cin, 3, 3] -> [Cout, 9*Cin'], k = (ky*3+kx)*Cin' + c, Cin' = Cin padded by _pad64
+    return _pad64(w.permute(0, 2, 3, 1)).reshape(w.shape[0], -1).contiguous().half()
+
+
+def _pack_conv3_padk(w, kpad):  # small-Cin convs through im2col: k = (ky*3+kx)*Cin + c, K zero-padded to kpad
     p = torch.zeros((w.shape[0], kpad), dtype=torch.float16, device=w.device)
-    p[:, : 9 * w.shape[1]] = _pack_conv3(w)
+    p[:, : 9 * w.shape[1]] = w.permute(0, 2, 3, 1).reshape(w.shape[0], -1).half()
     return p
 
 
@@ -55,13 +62,13 @@ def _hilo(w):
 
 def _pack_hilo_1x1(w):  # [N, K] fp32 -> [N, 3K] = [W_hi | W_hi | W_lo], multiplied by A = [A_hi | A_lo | A_hi]
     hi, lo = _hilo(w)
-    return torch.cat([hi, hi, lo], dim=1).contiguous()
+    return torch.cat([_pad64(hi), _pad64(hi), _pad64(lo)], dim=1).contiguous()
 
 
 def _pack_hilo_conv3(w):  # [N, C, 3, 3] fp32 -> [N, 9 * 3C], per tap [W_hi | W_hi | W_lo]
     wk = w.permute(0, 2, 3, 1).reshape(w.shape[0], 9, w.shape[1])
     hi, lo = _hilo(wk)
-    return torch.cat([hi, hi, lo], dim=2).reshape(w.shape[0], -1).contiguous()
+    return torch.cat([_pad64(hi), _pad64(hi), _pad64(lo)], dim=2).reshape(w.shape[0], -1).contiguous()
 
 
 def _geglu_tile(inner):
@@ -101,9 +108,11 @@ class UNetModel(nn.Module):
         if num_heads == -1:
             assert num_head_channels != -1, "Either num_heads or num_head_channels has to be set"
         # the sdb200 path covers the configuration SD v1 ships (v1-inference.yaml:29-44) and the unconditional
-        # AttentionBlock family (models/ldm/lsun_churches256/config.yaml: scale-shift norm, up/down ResBlocks)
+        # AttentionBlock family (models/ldm/lsun_churches256/config.yaml: scale-shift norm, up/down ResBlocks;
+        # configs/latent-diffusion/*-ldm-vq-4.yaml: plain ResBlocks with num_head_channels)
+        plain = not (use_spatial_transformer or use_scale_shift_norm or resblock_updown)
         unsupported = dict(dims=dims != 2, num_classes=num_classes is not None, n_embed=n_embed is not None,
-                           num_head_channels=num_head_channels != -1, dropout=dropout != 0,
+                           num_head_channels=num_head_channels != -1 and not plain, dropout=dropout != 0,
                            conv_resample=not conv_resample, use_new_attention_order=bool(use_new_attention_order),
                            num_heads_upsample=num_heads_upsample not in (-1, num_heads))
         if use_spatial_transformer:
@@ -116,7 +125,8 @@ class UNetModel(nn.Module):
         self.cfg = dict(image_size=image_size, in_channels=in_channels, model_channels=model_channels,
                         out_channels=out_channels, num_res_blocks=num_res_blocks,
                         attention_resolutions=list(attention_resolutions), channel_mult=list(channel_mult),
-                        num_heads=num_heads, use_spatial_transformer=bool(use_spatial_transformer), transformer_depth=1,
+                        num_heads=num_heads, num_head_channels=num_head_channels,
+                        use_spatial_transformer=bool(use_spatial_transformer), transformer_depth=1,
                         context_dim=context_dim, legacy=legacy, use_scale_shift_norm=bool(use_scale_shift_norm),
                         resblock_updown=bool(resblock_updown))
         self.conditional = bool(use_spatial_transformer)   # cross-attention on a context; otherwise forward(x, t)

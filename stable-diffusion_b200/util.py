@@ -24,6 +24,7 @@ TARGET_MAP = {
     "ldm.models.diffusion.ddpm.LatentDiffusion": "sdb200.diffusion.LatentDiffusion",
     "ldm.modules.diffusionmodules.openaimodel.UNetModel": "sdb200.unet.UNetModel",
     "ldm.models.autoencoder.AutoencoderKL": "sdb200.vae.AutoencoderKL",
+    "ldm.models.autoencoder.VQModelInterface": "sdb200.vq.VQModelInterface",
     "ldm.modules.encoders.modules.FrozenCLIPEmbedder": "sdb200.clip.FrozenCLIPEmbedder",
 }
 

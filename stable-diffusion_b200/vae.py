@@ -51,15 +51,14 @@ class DiagonalGaussianDistribution:
         return self.mean
 
 
-class AutoencoderKL(nn.Module):
-    def __init__(self, ddconfig, lossconfig=None, embed_dim=4, ckpt_path=None, ignore_keys=(), image_key="image",
-                 colorize_nlabels=None, monitor=None):
+class ConvAutoencoder(nn.Module):
+    """The Encoder / Decoder of model.py:368-568 (attention in the mid block only) and the weight plumbing shared by the
+    first stages: AutoencoderKL below and VQModelInterface (vq.py). Both have a quant_conv and a post_quant_conv (1x1,
+    <= 16 channels, fp32), packed here; a subclass sets `shapes` and packs anything else it has (the codebook)."""
+
+    def __init__(self, shapes):
         super().__init__()
-        assert ddconfig["double_z"], "AutoencoderKL needs double_z"
-        assert not ddconfig.get("attn_resolutions"), "SD-v1 VAE: attention only in the mid block"
-        self.cfg = dict(embed_dim=embed_dim, ddconfig=dict(ddconfig))
-        self.embed_dim = embed_dim
-        self.shapes = vae_param_shapes(self.cfg)
+        self.shapes = shapes
         self.W = None
         self._host_sd = None
 
@@ -217,15 +216,9 @@ class AutoencoderKL(nn.Module):
                           rows_per_sample=n, want_stats=True, stats_group=_sg(c))
         return out.view(nb, H, Wd, c)
 
-    # ------------------------------------------------------------------ public API
-    @torch.no_grad()
-    def decode(self, z, scale=1.0, nhwc=False):
-        """AutoencoderKL.decode (autoencoder.py:330-333) on z*scale; NCHW fp32 in / out (nhwc=True keeps the
-        kernels' native NHWC output, which is what the image writer wants: txt2img.py:322)."""
-        assert self.W is not None and z.is_cuda, "sdb200.AutoencoderKL runs on CUDA only (no CPU fallback)"
-        W, D = self.W, self.W["decoder"]
-        zh, _ = ops.nchw_to_nhwc(z.contiguous().float())
-        h = ops.pointwise_small(zh, W["pq_w"], W["pq_b"], alpha=float(scale))
+    def _decoder(self, h):
+        """Decoder.forward (model.py:535-568) on the fp32 NHWC output of post_quant_conv; returns fp32 NHWC."""
+        D = self.W["decoder"]
         h = self._conv3(D["conv_in"], x32=h)
         h = self._resnet(D["mid1"], h)
         h = self._attn(D["attn"], h)
@@ -236,14 +229,11 @@ class AutoencoderKL(nn.Module):
             if lvl["resample"] is not None:   # Upsample: nearest 2x + conv (model.py:42-57)
                 h = self._conv3(lvl["resample"], x16=ops.upsample2x(h))
         hn, _ = ops.groupnorm(h, *D["gn_out"], eps=1e-6, silu=True)
-        out = self._conv3(D["conv_out"], x16=hn)
-        return out if nhwc else ops.nhwc_to_nchw(out)
+        return self._conv3(D["conv_out"], x16=hn)
 
-    @torch.no_grad()
-    def encode(self, x):
-        """AutoencoderKL.encode (autoencoder.py:324-328): returns the diagonal Gaussian posterior."""
-        assert self.W is not None and x.is_cuda, "sdb200.AutoencoderKL runs on CUDA only (no CPU fallback)"
-        W, E = self.W, self.W["encoder"]
+    def _encoder(self, x):
+        """Encoder.forward (model.py:434-459) on an NCHW image; returns the fp32 NHWC output of conv_out."""
+        E = self.W["encoder"]
         xh, _ = ops.nchw_to_nhwc(x.contiguous().float())
         h = self._conv3(E["conv_in"], x32=xh)
         for lvl in E["levels"]:
@@ -260,7 +250,36 @@ class AutoencoderKL(nn.Module):
         h = self._attn(E["attn"], h)
         h = self._resnet(E["mid2"], h)
         hn, _ = ops.groupnorm(h, *E["gn_out"], eps=1e-6, silu=True)
-        m = self._conv3(E["conv_out"], x16=hn)
+        return self._conv3(E["conv_out"], x16=hn)
+
+
+class AutoencoderKL(ConvAutoencoder):
+    def __init__(self, ddconfig, lossconfig=None, embed_dim=4, ckpt_path=None, ignore_keys=(), image_key="image",
+                 colorize_nlabels=None, monitor=None):
+        assert ddconfig["double_z"], "AutoencoderKL needs double_z"
+        assert not ddconfig.get("attn_resolutions"), "SD-v1 VAE: attention only in the mid block"
+        cfg = dict(embed_dim=embed_dim, ddconfig=dict(ddconfig))
+        super().__init__(vae_param_shapes(cfg))
+        self.cfg = cfg
+        self.embed_dim = embed_dim
+
+    # ------------------------------------------------------------------ public API
+    @torch.no_grad()
+    def decode(self, z, scale=1.0, nhwc=False):
+        """AutoencoderKL.decode (autoencoder.py:330-333) on z*scale; NCHW fp32 in / out (nhwc=True keeps the
+        kernels' native NHWC output, which is what the image writer wants: txt2img.py:322)."""
+        assert self.W is not None and z.is_cuda, "sdb200.AutoencoderKL runs on CUDA only (no CPU fallback)"
+        W = self.W
+        zh, _ = ops.nchw_to_nhwc(z.contiguous().float())
+        out = self._decoder(ops.pointwise_small(zh, W["pq_w"], W["pq_b"], alpha=float(scale)))
+        return out if nhwc else ops.nhwc_to_nchw(out)
+
+    @torch.no_grad()
+    def encode(self, x):
+        """AutoencoderKL.encode (autoencoder.py:324-328): returns the diagonal Gaussian posterior."""
+        assert self.W is not None and x.is_cuda, "sdb200.AutoencoderKL runs on CUDA only (no CPU fallback)"
+        W = self.W
+        m = self._encoder(x)
         nb, H, Wd, c2 = m.shape
         moments = ops.pointwise_small(m, W["quant_w"], W["quant_b"])
         return DiagonalGaussianDistribution(moments.view(nb * H * Wd, c2), nb, H, Wd, c2 // 2)
