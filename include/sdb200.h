@@ -110,12 +110,13 @@ int sdb_gemm_plan(const sdb_gemm_desc* d, int32_t* out);
 /*
  * Fused multi-head attention (flash-style, S/P/O in registers), replaces CrossAttention.forward's
  * einsum -> scale -> softmax -> einsum (ldm/modules/attention.py:178-192) without materialising N x N.
- *   q  : fp16 [batch, nq,  heads*dpad]   (row stride ldq elements; head h at column h*dpad)
- *   k  : fp16 [batch, nkv, heads*dpad]   (row stride ldk)
- *   vt : fp16 [batch, heads*dpad, ldvt]  (V transposed: channel-major, nkv valid columns)
+ *   q  : fp16 [batch, nq,  heads*hs]     (row stride ldq elements; head h at column h*hs)
+ *   k  : fp16 [batch, nkv, heads*hs]     (row stride ldk)
+ *   vt : fp16 [batch, heads*hs, ldvt]    (V transposed: channel-major, head h at row h*hs, nkv valid columns)
  *   out: fp16 [batch, nq, heads*d]       (row stride ldo; unpadded head dim d)
- * dpad in {64,128,192} (head dim zero-padded to a multiple of 64 by the projection weights: columns d .. dpad-1 of q / k
- * and rows d .. dpad-1 of each head of vt MUST be zero - the kernels only issue the tensor-core steps that hold real columns).
+ * hs = head_stride, the elements between consecutive heads (a multiple of 8, >= d; 0 means dpad). head_stride = d is
+ * the packed layout the projections produce; elements d .. hs-1 of a head, if any, are never read.
+ * dpad in {64,128,192}: d rounded up to the kernel's 64-column K panels (512: the single-head d = 512 kernel).
  * scale multiplies q.k before softmax (applied after the dot product, attention.py:180).
  * causal != 0 masks kv index > q index (CLIP text encoder).
  */
@@ -129,6 +130,7 @@ typedef struct sdb_attn_desc {
   int64_t q_batch_stride, k_batch_stride, vt_batch_stride, o_batch_stride; /* elements */
   float scale;
   int32_t causal;
+  int32_t head_stride;
 } sdb_attn_desc;
 
 int sdb_attention(const sdb_attn_desc* d, sdb_stream_t stream);

@@ -5,11 +5,21 @@
 //   warps 0..7  : two consumer warpgroups of 64 query rows each: wgmma S (M = 64, N = 64 keys), masking, online
 //                 softmax (a row lives in the four threads of a quad), wgmma PV (M = 64, N = DV), epilogue O / l
 //
-//   attention_tc_kernel<DPAD, DPAD>: multi-head attention with the head dim padded to DPAD = 64 / 128 / 192.
+//   attention_tc_kernel<DPAD, DV>: multi-head attention, head dim d <= DPAD (64 / 128 / 192 = the K panels of S),
+//     DV = the PV width, ceil8(d) for the head dims the engine runs, else the slot width (d <= 160 at DPAD 192). Heads are read through 4-D
+//     tensor maps whose innermost extent is d, so the panel columns d .. DPAD-1 and the V^T rows d .. DV-1 arrive as
+//     TMA zero fill whatever the head stride in memory is. The consumer loop is software-pipelined (FA3-style):
+//       window j (tensor-core issue, ping-ponged between the warpgroups by two named barriers): S_j = Q K_j^T, then
+//         O += P_{j-1} V_{j-1}
+//       after the window: wait for S_j only, softmax of tile j into the S registers while PV_{j-1} runs, wait for
+//         PV_{j-1}, rescale O, pack P_j
+//     so one warpgroup's exp work overlaps its own PV and the other warpgroup's MMAs. A quarter of the exponentials
+//     run as a polynomial on the FMA pipe (poly_exp2) next to the MUFU ones.
+//     The 288 threads x 224 registers of one CTA per SM fit the register file, so there is no setmaxnreg rebalancing.
 //   attention_tc_kernel<512, 128>  : single-head d = 512 (the AutoencoderKL mid-block AttnBlock,
 //     ldm/modules/diffusionmodules/model.py:178-202): one CTA = 128 query rows x ONE 128-column slice of the output
 //     (grid.y = 4 slices; S is recomputed per slice: a wider O does not fit the registers next to S), Q resident as
-//     eight 64-column panels, K streamed panel by panel.
+//     eight 64-column panels, K streamed panel by panel through a 4-deep ring (S and PV are not overlapped here).
 //     The N x N logits never leave the SM.
 //
 // Replaces the materialised einsum('b i d, b j d -> b i j') * scale -> softmax -> einsum('b i j, b j d -> b i d')
@@ -26,15 +36,19 @@ constexpr int AQ = 128;   // query rows per CTA
 constexpr int AKV = 64;   // kv rows per iteration
 constexpr int ATT_THREADS = 288;
 constexpr int ATT_PRODUCER_WARP = 8;
+constexpr int WIDE_D = 512;
+constexpr int WIDE_DV = 128;
 
 template <int DPAD, int DV>
 struct AttnCfg {
   static constexpr int PANELS = DPAD / 64;
   static constexpr int Q_BYTES = AQ * DPAD * 2;
-  static constexpr int KP_BYTES = AKV * 64 * 2;   // one 64-column K panel
-  static constexpr int V_BYTES = DV * AKV * 2;     // one V^T tile [DV x 64 keys]
-  static constexpr int KST = DPAD == 512 ? 4 : (2 * PANELS < 4 ? 4 : 2 * PANELS);   // K panel ring depth
-  static constexpr int VST = 2;                                                      // V^T ring depth
+  static constexpr int KP_BYTES = AKV * 64 * 2;            // one 64-column K panel
+  static constexpr int V_TX = DV * AKV * 2;                 // one V^T tile [DV x 64 keys]
+  static constexpr int V_BYTES = (V_TX + 1023) / 1024 * 1024;   // ring stage: swizzle atoms stay 1024-byte aligned
+  // multi-head: two tiles of K panels, so S_{j+1}'s panels load while S_j's are still held
+  static constexpr int KST = DPAD == WIDE_D ? 4 : (2 * PANELS < 4 ? 4 : 2 * PANELS);   // K panel ring depth
+  static constexpr int VST = DPAD == WIDE_D ? 2 : 4;   // V^T ring depth: the producer loads K_{j+1} after V_j's slot frees
   static constexpr int SMEM = Q_BYTES + KST * KP_BYTES + VST * V_BYTES + 1024;
 };
 
@@ -52,9 +66,94 @@ __device__ __forceinline__ float fast_exp2(float x) {  // one MUFU.EX2, flush-to
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
+// exp2 of x <= 0 on the FMA / integer pipes, for the share of the softmax exponentials that MUFU does not take.
+// Cody-Waite split x = n + f with n = round(x) (the 1.5 * 2^23 shifter), f in [-1/2, 1/2]; 2^f by the cubic
+// 1 + f (c1 + f (c2 + f c3)), minimax in relative error on [-1/2, 1/2]: |p / 2^f - 1| < 1.02e-4 < 2^-13, below the
+// 2^-11 rounding of P to fp16. 2^n is added to the exponent field. x is clamped to -127: -inf (masked) and anything
+// below gives n = -127, f = 0, p = 1 exactly, i.e. the bit pattern 0 = +0.0, as MUFU's flush-to-zero does.
+__device__ __forceinline__ float poly_exp2(float x) {
+  x = fmaxf(x, -127.f);
+  const float t = x + 12582912.f;
+  const float f = x - (t - 12582912.f);
+  const float p = fmaf(fmaf(fmaf(0.05500893f, f, 0.24221095f), f, 0.6932829f), f, 1.0f);
+  return __int_as_float(__float_as_int(p) + (__float_as_int(t) << 23));
+}
 __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
   const __half2 h = __floats2half2_rn(a, b);
   return *reinterpret_cast<const uint32_t*>(&h);
+}
+// named barriers 1 / 2: warpgroup w waits on 1 + w for its turn at the tensor cores and hands the turn on to the other
+__device__ __forceinline__ void wg_turn_wait(int wg) { asm volatile("bar.sync %0, 256;" ::"r"(1 + wg) : "memory"); }
+__device__ __forceinline__ void wg_turn_pass(int wg) { asm volatile("bar.arrive %0, 256;" ::"r"(2 - wg) : "memory"); }
+
+// S fragment of one 64-key tile -> masked online softmax, exponentials left in s (fp32), l updated; returns the O
+// rescale factors through al0 / al1. s[4c + e]: row qi0 (e < 2) or qi1, key kv0 + 8c + 2 t4 + (e & 1).
+template <bool POLY>
+__device__ __forceinline__ void softmax_tile(float (&s)[AKV / 2], const AttnArgs& p, int kv0, int q0, int qi0, int qi1,
+                                             int t4, float& m0, float& m1, float& l0, float& l1, float& al0,
+                                             float& al1) {
+  if ((kv0 + AKV > p.nkv) || (p.causal && kv0 + AKV - 1 > q0)) {
+#pragma unroll
+    for (int i = 0; i < AKV / 2; ++i) {
+      const int kv = kv0 + 8 * (i >> 2) + 2 * t4 + (i & 1);
+      const int qi = (i & 2) ? qi1 : qi0;
+      if ((kv >= p.nkv) || (p.causal && kv > qi)) s[i] = -INFINITY;
+    }
+  }
+  float mx0 = s[0], mx1 = s[2];
+#pragma unroll
+  for (int c = 0; c < AKV / 8; ++c) {
+    mx0 = fmaxf(mx0, fmaxf(s[4 * c], s[4 * c + 1]));
+    mx1 = fmaxf(mx1, fmaxf(s[4 * c + 2], s[4 * c + 3]));
+  }
+  mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
+  mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
+  mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+  mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+  const float mn0 = fmaxf(m0, mx0 * p.scale_log2);   // scale > 0
+  const float mn1 = fmaxf(m1, mx1 * p.scale_log2);
+  al0 = (m0 == -INFINITY) ? 0.f : exp2f(m0 - mn0);   // nothing accumulated yet: O = 0, l = 0
+  al1 = (m1 == -INFINITY) ? 0.f : exp2f(m1 - mn1);
+  m0 = mn0;
+  m1 = mn1;
+  l0 *= al0;
+  l1 *= al1;
+  const float nm0 = (mn0 == -INFINITY) ? 0.f : -mn0;   // a fully masked row so far: exp2(-inf) = 0
+  const float nm1 = (mn1 == -INFINITY) ? 0.f : -mn1;
+#pragma unroll
+  for (int c = 0; c < AKV / 8; ++c) {
+    // POLY: the n8 blocks c = 3, 7 (one column pair in four) go to the FMA pipe, the rest to MUFU
+    const bool poly = POLY && (c & 3) == 3;
+    const float x0 = fmaf(s[4 * c], p.scale_log2, nm0), x1 = fmaf(s[4 * c + 1], p.scale_log2, nm0);
+    const float x2 = fmaf(s[4 * c + 2], p.scale_log2, nm1), x3 = fmaf(s[4 * c + 3], p.scale_log2, nm1);
+    s[4 * c] = poly ? poly_exp2(x0) : fast_exp2(x0);
+    s[4 * c + 1] = poly ? poly_exp2(x1) : fast_exp2(x1);
+    s[4 * c + 2] = poly ? poly_exp2(x2) : fast_exp2(x2);
+    s[4 * c + 3] = poly ? poly_exp2(x3) : fast_exp2(x3);
+    l0 += s[4 * c] + s[4 * c + 1];
+    l1 += s[4 * c + 2] + s[4 * c + 3];
+  }
+}
+
+// P (fp16) in the A-operand layout of wgmma: for key step kk, {row qi0 keys 2 t4 .. +1, row qi1 same, row qi0
+// keys 8 + 2 t4 .. +1, row qi1 same} = the S fragments of n8 blocks 2 kk and 2 kk + 1
+__device__ __forceinline__ void pack_p(uint32_t (&pa)[AKV / 16][4], const float (&s)[AKV / 2]) {
+#pragma unroll
+  for (int c = 0; c < AKV / 8; ++c) {
+    pa[c >> 1][(c & 1) * 2] = pack_half2(s[4 * c], s[4 * c + 1]);
+    pa[c >> 1][(c & 1) * 2 + 1] = pack_half2(s[4 * c + 2], s[4 * c + 3]);
+  }
+}
+
+template <int DV>
+__device__ __forceinline__ void rescale_o(float (&o)[DV / 2], float al0, float al1) {
+#pragma unroll
+  for (int c = 0; c < DV / 8; ++c) {
+    o[4 * c] *= al0;
+    o[4 * c + 1] *= al0;
+    o[4 * c + 2] *= al1;
+    o[4 * c + 3] *= al1;
+  }
 }
 
 template <int DPAD, int DV>
@@ -62,7 +161,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
     attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                         const __grid_constant__ CUtensorMap tmV, const AttnArgs p) {
   using Cfg = AttnCfg<DPAD, DV>;
-  constexpr bool WIDE = DV < DPAD;
+  constexpr bool WIDE = DPAD == WIDE_D;
   constexpr int PANELS = Cfg::PANELS;
   constexpr int KST = Cfg::KST;
   constexpr int VST = Cfg::VST;
@@ -107,15 +206,16 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
   pdl_wait();   // q / k / v come from the previous kernels; everything above overlapped their tail
   if (warp == ATT_PRODUCER_WARP) {
     if (elect_one()) {
+      // tensor maps: Q / K {d, heads, rows, batch}, V^T {nkv, d, heads, batch}
       mbar_arrive_expect_tx(&q_full, Cfg::Q_BYTES);
-      for (int pn = 0; pn < PANELS; ++pn) tma_load_3d(q_s + pn * (AQ * 128), &tmQ, &q_full, head * DPAD + pn * 64, q0, b);
+      for (int pn = 0; pn < PANELS; ++pn) tma_load_4d(q_s + pn * (AQ * 128), &tmQ, &q_full, pn * 64, head, q0, b);
       int ks = 0;
       uint32_t kph = 0;
       for (int j = 0; j < n_iter; ++j) {
         for (int pn = 0; pn < PANELS; ++pn) {
           mbar_wait_mma(&k_empty[ks], kph ^ 1);
           mbar_arrive_expect_tx(&k_full[ks], Cfg::KP_BYTES);
-          tma_load_3d(k_s + ks * Cfg::KP_BYTES, &tmK, &k_full[ks], head * DPAD + pn * 64, j * AKV, b);
+          tma_load_4d(k_s + ks * Cfg::KP_BYTES, &tmK, &k_full[ks], pn * 64, head, j * AKV, b);
           if (++ks == KST) {
             ks = 0;
             kph ^= 1;
@@ -123,8 +223,8 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
         }
         const int vs = j % VST;
         mbar_wait_mma(&v_empty[vs], ((j / VST) & 1) ^ 1);
-        mbar_arrive_expect_tx(&v_full[vs], Cfg::V_BYTES);
-        tma_load_3d(v_s + vs * Cfg::V_BYTES, &tmV, &v_full[vs], j * AKV, head * DPAD + dv0, b);
+        mbar_arrive_expect_tx(&v_full[vs], Cfg::V_TX);
+        tma_load_4d(v_s + vs * Cfg::V_BYTES, &tmV, &v_full[vs], j * AKV, dv0, head, b);
       }
     }
     __syncwarp();
@@ -133,111 +233,140 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
     const int t4 = lane & 3;
     const int qi0 = q0 + 64 * wg + 16 * (warp & 3) + (lane >> 2);   // fragment rows of this thread: qi0, qi0 + 8
     const int qi1 = qi0 + 8;
-    // head dimension d < DPAD: columns d .. DPAD-1 of Q / K are zero padding; only the 16-wide K steps that hold real
-    // columns are issued for S
+    // head dimension d < DPAD: columns d .. DPAD-1 of the Q / K panels are zero fill; only the 16-wide K steps that
+    // hold real columns are issued for S
     const int ksteps = (p.d + 15) >> 4;
     const uint32_t q_addr = smem_u32(q_s) + static_cast<uint32_t>(wg * 64 * 128);
     float o[DV / 2];
 #pragma unroll
     for (int i = 0; i < DV / 2; ++i) o[i] = 0.f;
+    float s[AKV / 2];
+#pragma unroll
+    for (int i = 0; i < AKV / 2; ++i) s[i] = 0.f;
+    uint32_t pa[AKV / 16][4];
     float m0 = -INFINITY, m1 = -INFINITY;   // running maxima (log2 domain) of rows qi0 / qi1
     float l0 = 0.f, l1 = 0.f;               // this thread's share of the row sums
+    float al0, al1;
     int ks = 0;
     uint32_t kph = 0;
     mbar_wait_mma(&q_full, 0);
-    for (int j = 0; j < n_iter; ++j) {
-      // ---- S = Q K^T over the K panels of this tile; each panel is handed back once its MMAs have completed
-      float s[AKV / 2];
-#pragma unroll
-      for (int i = 0; i < AKV / 2; ++i) s[i] = 0.f;
-      wgmma_hold(s);
-      int prev = -1;
+    if constexpr (WIDE) {
+      for (int j = 0; j < n_iter; ++j) {
+        // ---- S = Q K^T over the K panels of this tile; each panel is handed back once its MMAs have completed
+        wgmma_hold(s);
+        int prev = -1;
 #pragma unroll 1
-      for (int pn = 0; pn < PANELS; ++pn) {
-        mbar_wait_mma(&k_full[ks], kph);
-        const uint32_t k_addr = smem_u32(k_s + ks * Cfg::KP_BYTES);
+        for (int pn = 0; pn < PANELS; ++pn) {
+          mbar_wait_mma(&k_full[ks], kph);
+          const uint32_t k_addr = smem_u32(k_s + ks * Cfg::KP_BYTES);
+          wgmma_fence();
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk)
+            WgmmaSS<AKV>::mma(s, wg_desc(q_addr + pn * (AQ * 128) + kk * 32), wg_desc(k_addr + kk * 32),
+                              (pn | kk) != 0);
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (prev >= 0 && lane == 0) mbar_arrive(&k_empty[prev]);
+          prev = ks;
+          if (++ks == KST) {
+            ks = 0;
+            kph ^= 1;
+          }
+        }
+        wgmma_wait<0>();
+        wgmma_hold(s);
+        if (lane == 0) mbar_arrive(&k_empty[prev]);
+        softmax_tile<false>(s, p, j * AKV, q0, qi0, qi1, t4, m0, m1, l0, l1, al0, al1);
+        rescale_o<DV>(o, al0, al1);
+        pack_p(pa, s);
+
+        // ---- O += P V^T-tile
+        const int vs = j % VST;
+        mbar_wait_mma(&v_full[vs], (j / VST) & 1);
+        const uint32_t v_addr = smem_u32(v_s + vs * Cfg::V_BYTES);
+        wgmma_hold(o);
         wgmma_fence();
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk)
-          if (pn * 4 + kk < ksteps)
-            WgmmaSS<AKV>::mma(s, wg_desc(q_addr + pn * (AQ * 128) + kk * 32), wg_desc(k_addr + kk * 32), 1u);
+        for (int kk = 0; kk < AKV / 16; ++kk) WgmmaRS<DV>::mma(o, pa[kk], wg_desc(v_addr + kk * 32), 1u);
         wgmma_commit();
-        wgmma_wait<1>();
-        if (prev >= 0 && lane == 0) mbar_arrive(&k_empty[prev]);
-        prev = ks;
-        if (++ks == KST) {
+        wgmma_wait<0>();
+        wgmma_hold(o);
+        if (lane == 0) mbar_arrive(&v_empty[vs]);
+      }
+    } else {
+      // Every wgmma below is issued unconditionally (a data-dependent branch around one makes ptxas serialise them
+      // all), hence the peeled first and last windows. S issues ceil16(DV) K steps: for DV = ceil8(d) that is
+      // ceil16(d); where DV = DPAD the steps past d multiply the zero-filled panel columns.
+      constexpr int KSTEPS = (DV + 15) / 16;
+      auto issue_s = [&]() {   // S_j = Q K_j^T over the tile's panels (ring slots ks .. ks + PANELS - 1), one group
+#pragma unroll
+        for (int pn = 0; pn < PANELS; ++pn) {
+          mbar_wait_mma(&k_full[ks + pn], kph);
+          const uint32_t k_addr = smem_u32(k_s + (ks + pn) * Cfg::KP_BYTES);
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk)
+            if (pn * 4 + kk < KSTEPS)
+              WgmmaSS<AKV>::mma(s, wg_desc(q_addr + pn * (AQ * 128) + kk * 32), wg_desc(k_addr + kk * 32),
+                                (pn | kk) != 0);
+        }
+        wgmma_commit();
+      };
+      auto release_k = [&]() {   // KST is a multiple of PANELS: a tile's panels never straddle the ring's end
+        if (lane == 0)
+#pragma unroll
+          for (int pn = 0; pn < PANELS; ++pn) mbar_arrive(&k_empty[ks + pn]);
+        ks += PANELS;
+        if (ks == KST) {
           ks = 0;
           kph ^= 1;
         }
-      }
+      };
+      auto issue_pv = [&](int jv) {   // O += P_jv V_jv
+        const int vs = jv % VST;
+        mbar_wait_mma(&v_full[vs], (jv / VST) & 1);
+        const uint32_t v_addr = smem_u32(v_s + vs * Cfg::V_BYTES);
+#pragma unroll
+        for (int kk = 0; kk < AKV / 16; ++kk) WgmmaRS<DV>::mma(o, pa[kk], wg_desc(v_addr + kk * 32), 1u);
+        wgmma_commit();
+      };
+      // Turn order: warpgroup 1 hands warpgroup 0 the first turn; each warpgroup then takes n_iter + 1 turns and
+      // passes on every one except warpgroup 1's last, so both named barriers end with no pending arrivals.
+      if (wg == 1) wg_turn_pass(wg);
+      wg_turn_wait(wg);
+      wgmma_fence();
+      issue_s();
+      wg_turn_pass(wg);
       wgmma_wait<0>();
       wgmma_hold(s);
-      if (lane == 0) mbar_arrive(&k_empty[prev]);
-
-      // ---- mask, online softmax. s[4c + e]: row qi0 (e < 2) or qi1, key kv0 + 8c + 2 t4 + (e & 1)
-      const int kv0 = j * AKV;
-      if ((kv0 + AKV > p.nkv) || (p.causal && kv0 + AKV - 1 > q0)) {
-#pragma unroll
-        for (int i = 0; i < AKV / 2; ++i) {
-          const int kv = kv0 + 8 * (i >> 2) + 2 * t4 + (i & 1);
-          const int qi = (i & 2) ? qi1 : qi0;
-          if ((kv >= p.nkv) || (p.causal && kv > qi)) s[i] = -INFINITY;
-        }
+      release_k();
+      softmax_tile<true>(s, p, 0, q0, qi0, qi1, t4, m0, m1, l0, l1, al0, al1);
+      pack_p(pa, s);
+      for (int j = 1; j < n_iter; ++j) {
+        wg_turn_wait(wg);
+        wgmma_hold(s);
+        wgmma_hold(o);
+        wgmma_fence();
+        issue_s();
+        issue_pv(j - 1);
+        wg_turn_pass(wg);
+        wgmma_wait<1>();   // S_j is done; PV_{j-1}, committed after it, may still run under the softmax
+        wgmma_hold(s);
+        release_k();
+        softmax_tile<true>(s, p, j * AKV, q0, qi0, qi1, t4, m0, m1, l0, l1, al0, al1);
+        wgmma_wait<0>();
+        wgmma_hold(o);
+        if (lane == 0) mbar_arrive(&v_empty[(j - 1) % VST]);
+        rescale_o<DV>(o, al0, al1);
+        pack_p(pa, s);
       }
-      float mx0 = s[0], mx1 = s[2];
-#pragma unroll
-      for (int c = 0; c < AKV / 8; ++c) {
-        mx0 = fmaxf(mx0, fmaxf(s[4 * c], s[4 * c + 1]));
-        mx1 = fmaxf(mx1, fmaxf(s[4 * c + 2], s[4 * c + 3]));
-      }
-      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
-      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
-      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
-      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
-      const float mn0 = fmaxf(m0, mx0 * p.scale_log2);   // scale > 0
-      const float mn1 = fmaxf(m1, mx1 * p.scale_log2);
-      const float al0 = (m0 == -INFINITY) ? 0.f : exp2f(m0 - mn0);   // nothing accumulated yet: O = 0, l = 0
-      const float al1 = (m1 == -INFINITY) ? 0.f : exp2f(m1 - mn1);
-      m0 = mn0;
-      m1 = mn1;
-      l0 *= al0;
-      l1 *= al1;
-#pragma unroll
-      for (int c = 0; c < DV / 8; ++c) {
-        o[4 * c] *= al0;
-        o[4 * c + 1] *= al0;
-        o[4 * c + 2] *= al1;
-        o[4 * c + 3] *= al1;
-      }
-      const float nm0 = (mn0 == -INFINITY) ? 0.f : -mn0;   // a fully masked row so far: exp2(-inf) = 0
-      const float nm1 = (mn1 == -INFINITY) ? 0.f : -mn1;
-      // P (fp16) in the A-operand layout of wgmma: for key step kk, {row qi0 keys 2 t4 .. +1, row qi1 same, row qi0
-      // keys 8 + 2 t4 .. +1, row qi1 same} = the S fragments of n8 blocks 2 kk and 2 kk + 1
-      uint32_t pa[AKV / 16][4];
-#pragma unroll
-      for (int c = 0; c < AKV / 8; ++c) {
-        const float e0 = fast_exp2(fmaf(s[4 * c], p.scale_log2, nm0));
-        const float e1 = fast_exp2(fmaf(s[4 * c + 1], p.scale_log2, nm0));
-        const float e2 = fast_exp2(fmaf(s[4 * c + 2], p.scale_log2, nm1));
-        const float e3 = fast_exp2(fmaf(s[4 * c + 3], p.scale_log2, nm1));
-        l0 += e0 + e1;
-        l1 += e2 + e3;
-        pa[c >> 1][(c & 1) * 2] = pack_half2(e0, e1);
-        pa[c >> 1][(c & 1) * 2 + 1] = pack_half2(e2, e3);
-      }
-
-      // ---- O += P V^T-tile
-      const int vs = j % VST;
-      mbar_wait_mma(&v_full[vs], (j / VST) & 1);
-      const uint32_t v_addr = smem_u32(v_s + vs * Cfg::V_BYTES);
+      wg_turn_wait(wg);
       wgmma_hold(o);
       wgmma_fence();
-#pragma unroll
-      for (int kk = 0; kk < AKV / 16; ++kk) WgmmaRS<DV>::mma(o, pa[kk], wg_desc(v_addr + kk * 32), 1u);
-      wgmma_commit();
+      issue_pv(n_iter - 1);
+      if (wg == 0) wg_turn_pass(wg);
       wgmma_wait<0>();
       wgmma_hold(o);
-      if (lane == 0) mbar_arrive(&v_empty[vs]);
+      if (lane == 0) mbar_arrive(&v_empty[(n_iter - 1) % VST]);
     }
 
     // ---- epilogue: O / l
@@ -277,8 +406,44 @@ static int launch_attn(const CUtensorMap& q, const CUtensorMap& k, const CUtenso
   return 0;
 }
 
-constexpr int WIDE_D = 512;
-constexpr int WIDE_DV = 128;
+// Q / K as {d, heads, rows, batch} (head h of row r at element r * ld + h * hs), V^T as {nkv, d, heads, batch}
+// (channel c of head h at row h * hs + c). The innermost extent is d, so a 64-wide panel box reads columns d .. 63 and
+// a DV-row V^T box reads rows d .. DV-1 as zeros.
+static int make_attn_maps(const sdb_attn_desc* d, int heads, int hd, int hs, uint32_t dv_box, CUtensorMap* tq,
+                          CUtensorMap* tk, CUtensorMap* tv) {
+  const uint64_t h = static_cast<uint64_t>(heads), dd = static_cast<uint64_t>(hd), e = 2;
+  {
+    uint64_t dims[4] = {dd, h, static_cast<uint64_t>(d->nq), static_cast<uint64_t>(d->batch)};
+    uint64_t str[3] = {hs * e, static_cast<uint64_t>(d->ldq) * e, static_cast<uint64_t>(d->q_batch_stride) * e};
+    uint32_t box[4] = {64, 1, AQ, 1};
+    if (make_tmap_f16(tq, d->q, 4, dims, str, box)) return 1;
+  }
+  {
+    uint64_t dims[4] = {dd, h, static_cast<uint64_t>(d->nkv), static_cast<uint64_t>(d->batch)};
+    uint64_t str[3] = {hs * e, static_cast<uint64_t>(d->ldk) * e, static_cast<uint64_t>(d->k_batch_stride) * e};
+    uint32_t box[4] = {64, 1, AKV, 1};
+    if (make_tmap_f16(tk, d->k, 4, dims, str, box)) return 1;
+  }
+  {
+    uint64_t dims[4] = {static_cast<uint64_t>(d->nkv), dd, h, static_cast<uint64_t>(d->batch)};
+    uint64_t str[3] = {static_cast<uint64_t>(d->ldvt) * e, static_cast<uint64_t>(hs) * d->ldvt * e,
+                       static_cast<uint64_t>(d->vt_batch_stride) * e};
+    uint32_t box[4] = {AKV, dv_box, 1, 1};
+    if (make_tmap_f16(tv, d->vt, 4, dims, str, box)) return 1;
+  }
+  return 0;
+}
+
+// PV width for head dim d in a dpad-column slot: ceil8(d) for the head dims of the engine's models, else the slot
+// width; 0 where no instantiation exists (d > 160 in a 192 slot: PV at N = 192 next to S spills registers)
+static uint32_t attn_dv(int dpad, int d) {
+  const int dv = (d + 7) / 8 * 8;
+  switch (dpad) {
+    case 64: return dv <= 48 ? dv : 64;
+    case 128: return (dv == 80 || dv == 96) ? dv : 128;
+    default: return dv <= 160 ? 160 : 0;
+  }
+}
 
 }  // namespace sdb
 
@@ -291,40 +456,24 @@ extern "C" int sdb_attention(const sdb_attn_desc* d, sdb_stream_t stream) {
   }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   SDB_CHECK(d && d->q && d->k && d->vt && d->out, "sdb_attention: null pointer");
+  CUtensorMap tq, tk, tv;
+  AttnArgs p{};
+  p.nq = d->nq;
+  p.nkv = d->nkv;
+  p.d = d->d;
+  p.ldo = d->ldo;
+  p.o_batch_stride = d->o_batch_stride;
+  p.out = static_cast<__half*>(d->out);
+  p.scale_log2 = d->scale * 1.4426950408889634f;
   if (d->dpad == WIDE_D) {
     // single-head d = 512 (AutoencoderKL AttnBlock): q, k [B, n, 512], vt [B, 512, ldvt]
     SDB_CHECK(d->d == WIDE_D && d->heads == 1 && !d->causal, "sdb_attention: dpad 512 is the single-head d = 512 kernel");
+    SDB_CHECK(d->head_stride == 0 || d->head_stride == WIDE_D, "sdb_attention: dpad 512 takes head_stride 0 or 512");
     SDB_CHECK(d->batch > 0 && d->nq > 0 && d->nkv > 0, "sdb_attention: bad sizes");
     SDB_CHECK(d->ldq % 8 == 0 && d->ldk % 8 == 0 && d->ldvt % 8 == 0 && d->ldo % 8 == 0 && d->o_batch_stride % 8 == 0,
               "sdb_attention: leading dims must be multiples of 8");
-    CUtensorMap tq, tk, tv;
-    {
-      uint64_t dims[3] = {WIDE_D, static_cast<uint64_t>(d->nq), static_cast<uint64_t>(d->batch)};
-      uint64_t str[2] = {static_cast<uint64_t>(d->ldq) * 2, static_cast<uint64_t>(d->q_batch_stride) * 2};
-      uint32_t box[3] = {64, AQ, 1};
-      if (make_tmap_f16(&tq, d->q, 3, dims, str, box)) return 1;
-    }
-    {
-      uint64_t dims[3] = {WIDE_D, static_cast<uint64_t>(d->nkv), static_cast<uint64_t>(d->batch)};
-      uint64_t str[2] = {static_cast<uint64_t>(d->ldk) * 2, static_cast<uint64_t>(d->k_batch_stride) * 2};
-      uint32_t box[3] = {64, AKV, 1};
-      if (make_tmap_f16(&tk, d->k, 3, dims, str, box)) return 1;
-    }
-    {
-      uint64_t dims[3] = {static_cast<uint64_t>(d->nkv), WIDE_D, static_cast<uint64_t>(d->batch)};
-      uint64_t str[2] = {static_cast<uint64_t>(d->ldvt) * 2, static_cast<uint64_t>(d->vt_batch_stride) * 2};
-      uint32_t box[3] = {AKV, WIDE_DV, 1};
-      if (make_tmap_f16(&tv, d->vt, 3, dims, str, box)) return 1;
-    }
-    AttnArgs p{};
-    p.nq = d->nq;
-    p.nkv = d->nkv;
-    p.d = d->d;
+    if (make_attn_maps(d, 1, WIDE_D, WIDE_D, WIDE_DV, &tq, &tk, &tv)) return 1;
     p.heads = 1;
-    p.ldo = d->ldo;
-    p.o_batch_stride = d->o_batch_stride;
-    p.out = static_cast<__half*>(d->out);
-    p.scale_log2 = d->scale * 1.4426950408889634f;
     p.causal = 0;
     dim3 grid((d->nq + AQ - 1) / AQ, WIDE_D / WIDE_DV, d->batch);
     return launch_attn<WIDE_D, WIDE_DV>(tq, tk, tv, p, grid, st);
@@ -332,44 +481,23 @@ extern "C" int sdb_attention(const sdb_attn_desc* d, sdb_stream_t stream) {
   SDB_CHECK(d->dpad == 64 || d->dpad == 128 || d->dpad == 192, "sdb_attention: dpad must be 64/128/192/512 (got %d)",
             d->dpad);
   SDB_CHECK(d->d > 0 && d->d <= d->dpad && d->d % 2 == 0, "sdb_attention: bad head dim %d", d->d);
+  const int hs = d->head_stride ? d->head_stride : d->dpad;
+  SDB_CHECK(hs >= d->d && hs % 8 == 0, "sdb_attention: head_stride %d must be >= d and a multiple of 8", hs);
   SDB_CHECK(d->batch > 0 && d->heads > 0 && d->nq > 0 && d->nkv > 0, "sdb_attention: bad sizes");
   SDB_CHECK(d->ldq % 8 == 0 && d->ldk % 8 == 0 && d->ldvt % 8 == 0, "sdb_attention: leading dims must be multiples of 8");
   SDB_CHECK(d->ldo % 2 == 0 && d->o_batch_stride % 2 == 0, "sdb_attention: output stride must be even");
-
-  CUtensorMap tq, tk, tv;
-  const uint64_t hd = static_cast<uint64_t>(d->heads) * d->dpad;
-  {
-    uint64_t dims[3] = {hd, static_cast<uint64_t>(d->nq), static_cast<uint64_t>(d->batch)};
-    uint64_t str[2] = {static_cast<uint64_t>(d->ldq) * 2, static_cast<uint64_t>(d->q_batch_stride) * 2};
-    uint32_t box[3] = {64, AQ, 1};
-    if (make_tmap_f16(&tq, d->q, 3, dims, str, box)) return 1;
-  }
-  {
-    uint64_t dims[3] = {hd, static_cast<uint64_t>(d->nkv), static_cast<uint64_t>(d->batch)};
-    uint64_t str[2] = {static_cast<uint64_t>(d->ldk) * 2, static_cast<uint64_t>(d->k_batch_stride) * 2};
-    uint32_t box[3] = {64, AKV, 1};
-    if (make_tmap_f16(&tk, d->k, 3, dims, str, box)) return 1;
-  }
-  {
-    uint64_t dims[3] = {static_cast<uint64_t>(d->nkv), hd, static_cast<uint64_t>(d->batch)};
-    uint64_t str[2] = {static_cast<uint64_t>(d->ldvt) * 2, static_cast<uint64_t>(d->vt_batch_stride) * 2};
-    uint32_t box[3] = {AKV, static_cast<uint32_t>(d->dpad), 1};
-    if (make_tmap_f16(&tv, d->vt, 3, dims, str, box)) return 1;
-  }
-  AttnArgs p{};
-  p.nq = d->nq;
-  p.nkv = d->nkv;
-  p.d = d->d;
+  const uint32_t dv = attn_dv(d->dpad, d->d);
+  SDB_CHECK(dv != 0, "sdb_attention: no kernel for head dim %d in dpad %d", d->d, d->dpad);
+  if (make_attn_maps(d, d->heads, d->d, hs, dv, &tq, &tk, &tv)) return 1;
   p.heads = d->heads;
-  p.ldo = d->ldo;
-  p.o_batch_stride = d->o_batch_stride;
-  p.out = static_cast<__half*>(d->out);
-  p.scale_log2 = d->scale * 1.4426950408889634f;
   p.causal = d->causal;
   dim3 grid((d->nq + AQ - 1) / AQ, d->heads, d->batch);
-  switch (d->dpad) {
-    case 64: return launch_attn<64, 64>(tq, tk, tv, p, grid, st);
-    case 128: return launch_attn<128, 128>(tq, tk, tv, p, grid, st);
-    default: return launch_attn<192, 192>(tq, tk, tv, p, grid, st);
-  }
+#define SDB_ATTN(DP, W) \
+  if (d->dpad == (DP) && dv == (W)) return launch_attn<DP, W>(tq, tk, tv, p, grid, st);
+  SDB_ATTN(64, 8) SDB_ATTN(64, 16) SDB_ATTN(64, 24) SDB_ATTN(64, 32) SDB_ATTN(64, 40) SDB_ATTN(64, 48) SDB_ATTN(64, 64)
+  SDB_ATTN(128, 80) SDB_ATTN(128, 96) SDB_ATTN(128, 128)
+  SDB_ATTN(192, 160)
+#undef SDB_ATTN
+  SDB_CHECK(false, "sdb_attention: no kernel for head dim %d in dpad %d", d->d, d->dpad);
+  return 1;
 }

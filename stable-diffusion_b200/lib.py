@@ -58,7 +58,7 @@ class AttnDesc(C.Structure):
         ("ldq", C.c_int32), ("ldk", C.c_int32), ("ldvt", C.c_int32), ("ldo", C.c_int32),
         ("q_batch_stride", C.c_int64), ("k_batch_stride", C.c_int64),
         ("vt_batch_stride", C.c_int64), ("o_batch_stride", C.c_int64),
-        ("scale", C.c_float), ("causal", C.c_int32),
+        ("scale", C.c_float), ("causal", C.c_int32), ("head_stride", C.c_int32),
     ]
 
 

@@ -286,8 +286,9 @@ def splitk_workspace(device):
     return _WS[key]
 
 
-def attention(q, k, vt, *, heads, d, dpad, nq, nkv, scale, causal=False, out=None):
-    """q [B, nq, heads*dpad], k [B, nkv, heads*dpad], vt [B, heads*dpad, ldvt] fp16 -> out [B, nq, heads*d] fp16."""
+def attention(q, k, vt, *, heads, d, dpad, nq, nkv, scale, causal=False, out=None, head_stride=0):
+    """q [B, nq, heads*hs], k [B, nkv, heads*hs], vt [B, heads*hs, ldvt] fp16 -> out [B, nq, heads*d] fp16, where
+    hs = head_stride (0: dpad) is the distance between heads; head_stride=d is the packed layout."""
     for name, t_ in (("q", q), ("k", k), ("vt", vt)):
         assert t_.dtype == torch.float16 and t_.is_cuda and t_.dim() == 3 and t_.stride(2) == 1, f"{name}: bad layout"
     B = q.shape[0]
@@ -299,7 +300,7 @@ def attention(q, k, vt, *, heads, d, dpad, nq, nkv, scale, causal=False, out=Non
     a.ldq, a.ldk, a.ldvt, a.ldo = q.stride(1), k.stride(1), vt.stride(1), out.stride(1)
     a.q_batch_stride, a.k_batch_stride = q.stride(0), k.stride(0)
     a.vt_batch_stride, a.o_batch_stride = vt.stride(0), out.stride(0)
-    a.scale, a.causal = scale, 1 if causal else 0
+    a.scale, a.causal, a.head_stride = scale, 1 if causal else 0, head_stride
     if PROFILE is not None:
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()

@@ -49,6 +49,8 @@ def _pack_conv3_padk(w, kpad):  # small-Cin convs through im2col: k = (ky*3+kx)*
 
 
 def _pack_heads(w, heads, d, dpad):  # [heads*d, K] -> [heads*dpad, K], zero rows between heads
+    """The head-padded layout (head_stride = dpad) that sdb_attention still accepts; the engine packs heads at stride
+    d."""
     K = w.shape[1]
     p = torch.zeros((heads, dpad, K), dtype=torch.float16, device=w.device)
     p[:, :d] = w.reshape(heads, d, K).half()
@@ -251,7 +253,7 @@ class UNetModel(nn.Module):
 
         def pack_attn(pre, a):
             """AttentionBlock (openaimodel.py:278-324) with QKVAttentionLegacy: qkv rows are [head][q | k | v][ch]. They
-            are repacked into head-padded Q|K and V weights for the flash kernel. The V bias is folded into proj_out:
+            are repacked into head-major Q|K and V weights for the flash kernel. The V bias is folded into proj_out:
             softmax rows sum to one, so P (V + 1 b_v^T) = P V + 1 b_v^T, and proj_out(o + b_v) = W_p o + (W_p b_v + b_p)."""
             ch, d = a["ch"], a["dhead"]
             hh = a["heads"]
@@ -260,12 +262,9 @@ class UNetModel(nn.Module):
             b = sd[pre + ".qkv.bias"].reshape(hh, 3, d)
             s = {"ch": ch, "d": d, "dpad": dp, "heads": hh}
             s["gn"] = (f32(pre + ".norm.weight"), f32(pre + ".norm.bias"))
-            s["w_qk"] = torch.cat([_pack_heads(w[:, 0].reshape(hh * d, ch), hh, d, dp),
-                                   _pack_heads(w[:, 1].reshape(hh * d, ch), hh, d, dp)], 0).contiguous()
-            bq = torch.zeros((2, hh, dp), dtype=torch.float32, device=device)
-            bq[0, :, :d], bq[1, :, :d] = b[:, 0], b[:, 1]
-            s["b_qk"] = bq.reshape(-1).contiguous()
-            s["w_v"] = _pack_heads(w[:, 2].reshape(hh * d, ch), hh, d, dp)
+            s["w_qk"] = w[:, :2].transpose(0, 1).reshape(2 * hh * d, ch).half().contiguous()
+            s["b_qk"] = b[:, :2].transpose(0, 1).reshape(-1).float().contiguous()
+            s["w_v"] = w[:, 2].reshape(hh * d, ch).half().contiguous()
             wp = sd[pre + ".proj_out.weight"].reshape(ch, ch)
             s["w_proj"] = wp.half().contiguous()
             s["b_proj"] = (sd[pre + ".proj_out.bias"].double() + wp.double() @ b[:, 2].reshape(-1).double()).float().contiguous()
@@ -281,13 +280,12 @@ class UNetModel(nn.Module):
             s["w_out"], s["b_out"] = one(sd[pre + ".proj_out.weight"].reshape(ch, ch)), f32(pre + ".proj_out.bias")
             for i in (1, 2, 3):
                 s[f"ln{i}"] = (f32(f"{tb}.norm{i}.weight"), f32(f"{tb}.norm{i}.bias"))
-            s["w_qk1"] = torch.cat([_pack_heads(sd[tb + ".attn1.to_q.weight"], heads, d, dp),
-                                    _pack_heads(sd[tb + ".attn1.to_k.weight"], heads, d, dp)], 0).contiguous()
-            s["w_v1"] = _pack_heads(sd[tb + ".attn1.to_v.weight"], heads, d, dp)
+            s["w_qk1"] = torch.cat([sd[tb + ".attn1.to_q.weight"], sd[tb + ".attn1.to_k.weight"]], 0).half().contiguous()
+            s["w_v1"] = f16(tb + ".attn1.to_v.weight")
             s["w_o1"], s["b_o1"] = f16(tb + ".attn1.to_out.0.weight"), f32(tb + ".attn1.to_out.0.bias")
-            s["w_q2"] = _pack_heads(sd[tb + ".attn2.to_q.weight"], heads, d, dp)
-            s["w_k2"] = _pack_heads(sd[tb + ".attn2.to_k.weight"], heads, d, dp)
-            s["w_v2"] = _pack_heads(sd[tb + ".attn2.to_v.weight"], heads, d, dp)
+            s["w_q2"] = f16(tb + ".attn2.to_q.weight")
+            s["w_k2"] = f16(tb + ".attn2.to_k.weight")
+            s["w_v2"] = f16(tb + ".attn2.to_v.weight")
             s["w_o2"], s["b_o2"] = f16(tb + ".attn2.to_out.0.weight"), f32(tb + ".attn2.to_out.0.bias")
             s["w_ff1"], s["b_ff1"] = _pack_geglu(sd[tb + ".ff.net.0.proj.weight"], sd[tb + ".ff.net.0.proj.bias"])
             s["w_ff2"], s["b_ff2"] = f16(tb + ".ff.net.2.weight"), f32(tb + ".ff.net.2.bias")
@@ -380,7 +378,7 @@ class UNetModel(nn.Module):
         nb, H, Wd, ch = x.shape
         ntok = H * Wd
         heads, d, dp = s["heads"], s["d"], s["dpad"]
-        hd = heads * dp
+        hd = heads * d                                                                     # heads packed at stride d
         scale = d ** -0.5
         x3 = self.W["x3"]
         if x3:
@@ -400,13 +398,15 @@ class UNetModel(nn.Module):
         else:  # TMA needs 16-byte aligned strides: tiny token counts go through an explicit transpose
             v, _ = ops.gemm(y, s["w_v1"], want_f16=True)
             vt3 = ops.transpose_f16(v.view(nb, ntok, hd))
-        o = ops.attention(qk3[:, :, :hd], qk3[:, :, hd:], vt3, heads=heads, d=d, dpad=dp, nq=ntok, nkv=ntok, scale=scale)
+        o = ops.attention(qk3[:, :, :hd], qk3[:, :, hd:], vt3, heads=heads, d=d, dpad=dp, nq=ntok, nkv=ntok, scale=scale,
+                          head_stride=d)
         _, t1 = ops.gemm(o.view(-1, ch), s["w_o1"], bias=s["b_o1"], residual=t0, want_f32=True, splits=-1)
         # --- cross attention (K / V^T of the context are precomputed per prompt)
         y = ops.layernorm(t1, *s["ln2"])
         q, _ = ops.gemm(y, s["w_q2"], want_f16=True)
         k2, vt2, nkv = kv
-        o = ops.attention(q.view(nb, ntok, hd), k2, vt2, heads=heads, d=d, dpad=dp, nq=ntok, nkv=nkv, scale=scale)
+        o = ops.attention(q.view(nb, ntok, hd), k2, vt2, heads=heads, d=d, dpad=dp, nq=ntok, nkv=nkv, scale=scale,
+                          head_stride=d)
         _, t2 = ops.gemm(o.view(-1, ch), s["w_o2"], bias=s["b_o2"], residual=t1, want_f32=True, splits=-1)
         # --- GEGLU feed-forward
         y = ops.layernorm(t2, *s["ln3"])
@@ -431,7 +431,7 @@ class UNetModel(nn.Module):
         nb, H, Wd, ch = x.shape
         ntok = H * Wd
         heads, d, dp = s["heads"], s["d"], s["dpad"]
-        hd = heads * dp
+        hd = heads * d                                                                     # heads packed at stride d
         xn, _ = ops.groupnorm(x, *s["gn"], eps=1e-5, silu=False)
         xm = xn.view(-1, ch)
         qk, _ = ops.gemm(xm, s["w_qk"], bias=s["b_qk"], want_f16=True)                     # [M, 2*hd]
@@ -443,7 +443,7 @@ class UNetModel(nn.Module):
             v, _ = ops.gemm(xm, s["w_v"], want_f16=True)
             vt3 = ops.transpose_f16(v.view(nb, ntok, hd))
         o = ops.attention(qk3[:, :, :hd], qk3[:, :, hd:], vt3, heads=heads, d=d, dpad=dp, nq=ntok, nkv=ntok,
-                          scale=d ** -0.5)
+                          scale=d ** -0.5, head_stride=d)
         o16, out = ops.gemm(o.view(-1, ch), s["w_proj"], bias=s["b_proj"], residual=x.view(-1, ch), want_f32=True,
                             want_f16=emit_f16, splits=-1, rows_per_sample=ntok, want_stats=True, stats_group=self._sg)
         out = out.view(nb, H, Wd, ch)
@@ -460,7 +460,7 @@ class UNetModel(nn.Module):
         ld = (nkv + 7) // 8 * 8
         out = []
         for i, s in enumerate(self.W["st_list"]):
-            hd = s["heads"] * s["dpad"]
+            hd = s["heads"] * s["d"]
             if i not in bufs:
                 bufs[i] = (torch.empty((nb * nkv, hd), dtype=torch.float16, device=context.device),
                            torch.empty((nb * nkv, hd), dtype=torch.float16, device=context.device),
