@@ -116,7 +116,11 @@ int sdb_gemm_plan(const sdb_gemm_desc* d, int32_t* out);
  *   out: fp16 [batch, nq, heads*d]       (row stride ldo; unpadded head dim d)
  * hs = head_stride, the elements between consecutive heads (a multiple of 8, >= d; 0 means dpad). head_stride = d is
  * the packed layout the projections produce; elements d .. hs-1 of a head, if any, are never read.
- * dpad in {64,128,192}: d rounded up to the kernel's 64-column K panels (512: the single-head d = 512 kernel).
+ * dpad in {64,128,192}: d rounded up to the kernel's 64-column K panels.
+ * dpad in {384,512,576,960}: the single-head kernels (the AutoencoderKL AttnBlock at 512, the num_heads-1
+ * SpatialTransformers of the class-conditional ImageNet LDM at 384 / 576 / 960); they require heads == 1, d == dpad,
+ * causal == 0, head_stride 0 or d, and ldq, ldk, ldvt, ldo, o_batch_stride multiples of 8.
+ * Any other descriptor returns nonzero with a message in sdb_last_error() and launches nothing.
  * scale multiplies q.k before softmax (applied after the dot product, attention.py:180).
  * causal != 0 masks kv index > q index (CLIP text encoder).
  */

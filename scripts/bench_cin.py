@@ -1,0 +1,104 @@
+#!/usr/bin/env python
+"""Class-conditional ImageNet LDM (cin256-v2) sampling speed on the H100 engine: the notebook workload of
+scripts/sample_imagenet.py (classes 25, 187, 448, 992, 6 samples per class, DDIM-20, eta 0, guidance scale 3.0, so every
+UNet evaluation runs a batch of 12 at 64x64x3; decode_first_stage included) on seeded random weights.
+Also reports one graph-replayed UNet evaluation at (12, 3, 64, 64) (CUDA events) and every attention launch of one eager
+evaluation from ops.PROFILE: time, algorithmic FLOPs (4 B nq nkv d) and tensor floor (FLOPs / 989 TFLOP/s, the H100 SXM
+dense fp16 data-sheet rate), with the attention share of the evaluation. Prints one JSON line with the card name and
+power limit read in the same run.
+
+  python scripts/bench_cin.py --repeats 3 --out outputs/cin.json
+"""
+import argparse
+import json
+import os
+import statistics
+import sys
+import time
+
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from sdb200 import ops  # noqa: E402
+from bench_lsun import gpu_info  # noqa: E402
+
+
+def attention_launches(u, x, t, c, reps=5):
+    """[(B, heads, nq, nkv, d, us, flops)] of one eager evaluation (median over reps) and the eager evaluation's ms."""
+    runs, totals = [], []
+    for _ in range(reps):
+        ops.PROFILE = []
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        u(x, t, context=c)
+        e1.record()
+        torch.cuda.synchronize()
+        runs.append(ops.PROFILE)
+        totals.append(e0.elapsed_time(e1))
+    ops.PROFILE = None
+    out = []
+    for i, (kind, fl, _, _, shp) in enumerate(runs[0]):
+        if kind == "attention":
+            out.append((*shp, statistics.median(r[i][2].elapsed_time(r[i][3]) for r in runs) * 1e3, fl))
+    return out, statistics.median(totals)
+
+
+def main():
+    p = argparse.ArgumentParser()
+    p.add_argument("--repeats", type=int, default=3)
+    p.add_argument("--steps", type=int, default=20)
+    p.add_argument("--out", type=str, default=None)
+    a = p.parse_args()
+    import sample_imagenet as S
+    dev = torch.device("cuda")
+    m = S.load_model(random_init=True)
+    u = m.model.diffusion_model
+    u.use_cuda_graph = True
+    classes, n = [25, 187, 448, 992], 6
+    torch.manual_seed(0)
+    S.sample_classes(m, classes, n, ddim_steps=a.steps)        # warm-up: autotune, graph capture, first stage
+    torch.cuda.synchronize()
+    times = []
+    for _ in range(a.repeats):
+        t0 = time.perf_counter()
+        img = S.sample_classes(m, classes, n, ddim_steps=a.steps)
+        torch.cuda.synchronize()
+        times.append(time.perf_counter() - t0)
+    assert img.shape == (len(classes) * n, 3, 256, 256) and bool(torch.isfinite(img).all())
+    x = torch.randn(2 * n, 3, 64, 64, device=dev)
+    t = torch.full((2 * n,), 501.0, device=dev)
+    c = m.get_learned_conditioning({"class_label": torch.tensor(n * [1000] + n * [25], device=dev)})
+    for _ in range(5):
+        u(x, t, context=c)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    reps = 50
+    e0.record()
+    for _ in range(reps):
+        u(x, t, context=c)
+    e1.record()
+    e1.synchronize()
+    unet_ms = e0.elapsed_time(e1) / reps
+    u.use_cuda_graph = False
+    launches, eager_ms = attention_launches(u, x, t, c)
+    attn_us = sum(r[5] for r in launches)
+    rows = [dict(B=B, heads=H, nq=nq, nkv=nkv, d=d, us=round(us, 1), gflop=round(fl / 1e9, 3),
+                 tensor_floor_us=round(fl / 989e12 * 1e6, 1)) for B, H, nq, nkv, d, us, fl in launches]
+    for r in rows:
+        print(f"attention B={r['B']} nq={r['nq']} nkv={r['nkv']} d={r['d']}: {r['us']:7.1f} us, {r['gflop']:.2f} GFLOP, "
+              f"tensor floor {r['tensor_floor_us']:.1f} us", file=sys.stderr)
+    res = dict(workload=f"cin256-v2 LDM, classes {classes} x {n}, DDIM-{a.steps} eta 0, scale 3.0 (UNet batch {2 * n} at "
+                        "64x64x3), decode_first_stage, random weights",
+               images_per_s=len(classes) * n / min(times), run_s=times, unet_eval_ms_graph=unet_ms,
+               unet_eval_ms_eager_profiled=eager_ms, attention_us_eager=attn_us,
+               attention_share_of_eager_eval=attn_us / 1e3 / eager_ms, attention_launches=rows, **gpu_info())
+    line = json.dumps(res)
+    print(line)
+    if a.out:
+        os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
+        with open(a.out, "w") as f:
+            f.write(line + "\n")
+
+
+if __name__ == "__main__":
+    main()

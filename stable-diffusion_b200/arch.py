@@ -59,6 +59,18 @@ CELEBAHQ_UNET = dict(image_size=64, in_channels=3, out_channels=3, model_channel
 # a small member for tests: widths 96 / 192 / 288, concats 288 and 480; 3 and 9 channels per GroupNorm group
 TINY_VQ_UNET = dict(image_size=16, in_channels=3, out_channels=3, model_channels=96, attention_resolutions=[2, 4],
                     num_res_blocks=1, channel_mult=[1, 2, 3], num_head_channels=32)
+# the class-conditional ImageNet LDM (configs/latent-diffusion/cin256-v2.yaml): the spatial-transformer UNet with
+# num_heads 1 and legacy dim_head = ch, i.e. single-head attention at d = 384 / 576 / 960, cross-attention on the
+# ClassEmbedder's one-token context; VQ-f4 first stage. Widths 192 .. 960 and every skip concat are multiples of 64.
+CIN256_V2_UNET = dict(image_size=64, in_channels=3, out_channels=3, model_channels=192, attention_resolutions=[8, 4, 2],
+                      num_res_blocks=2, channel_mult=[1, 2, 3, 5], num_heads=1, use_spatial_transformer=True,
+                      transformer_depth=1, context_dim=512)
+CIN256_V2_COND = dict(embed_dim=512, n_classes=1001, key="class_label")   # class 1000: the unconditional label
+# a small member for tests: widths 64 / 384 / 960, single-head attention at d = 384 and 960
+TINY_CIN_UNET = dict(image_size=16, in_channels=3, out_channels=3, model_channels=64, attention_resolutions=[2, 4],
+                     num_res_blocks=1, channel_mult=[1, 6, 15], num_heads=1, use_spatial_transformer=True,
+                     transformer_depth=1, context_dim=64)
+TINY_CIN_COND = dict(embed_dim=64, n_classes=1001, key="class_label")
 # VQModelInterface first stages (models/first_stage_models/vq-f4/config.yaml) and a small member
 VQ_F4 = dict(embed_dim=3, n_embed=8192, ddconfig=dict(double_z=False, z_channels=3, resolution=256, in_channels=3, out_ch=3,
                                                        ch=128, ch_mult=[1, 2, 4], num_res_blocks=2, attn_resolutions=[],
@@ -337,6 +349,12 @@ def vq_param_shapes(cfg):
     return p
 
 
+def class_embedder_param_shapes(cfg):
+    """Keys as ClassEmbedder.state_dict() (ldm/modules/encoders/modules.py:19-32), under `cond_stage_model.` in an
+    LDM checkpoint."""
+    return OrderedDict([("embedding.weight", (cfg["n_classes"], cfg["embed_dim"]))])
+
+
 # ------------------------------------------------------------------------------------------------ CLIP
 def clip_param_shapes(cfg):
     """Keys as transformers CLIPTextModel.state_dict() (`text_model.*`); in an SD checkpoint they sit under
@@ -427,7 +445,8 @@ def random_state_dict(shapes, seed, prefix="", device="cpu"):
             t = 0.15 + 0.05 * rn()
         elif _is_norm_key(k):
             t = 1.0 + 0.1 * rn()
-        elif k.endswith("quantize.embedding.weight"):   # VQ codebook: unit scale, or every z_q collapses towards 0
+        elif k.endswith("quantize.embedding.weight") or k.split(".")[-2:] == ["embedding", "weight"]:
+            # VQ codebook (unit scale, or every z_q collapses towards 0) and ClassEmbedder table (nn.Embedding's N(0, 1))
             t = rn()
         elif "embedding" in k:
             t = 0.02 * rn()

@@ -1,7 +1,8 @@
 // Flash-style fused attention on wgmma (sm_90a): S = Q K^T and O += P V on the tensor cores with S, O in registers,
 // online softmax on the accumulator fragments, P kept in registers as the A operand of the second MMA.
 //
-//   warp 8      : TMA producer (Q once; K in 64-column panels and V^T tiles, each through an mbarrier ring)
+//   warp 8      : TMA producer (Q once, or with each K panel at d = 960; K in 64-column panels and V^T tiles, each
+//                 through an mbarrier ring)
 //   warps 0..7  : two consumer warpgroups of 64 query rows each: wgmma S (M = 64, N = 64 keys), masking, online
 //                 softmax (a row lives in the four threads of a quad), wgmma PV (M = 64, N = DV), epilogue O / l
 //
@@ -16,11 +17,20 @@
 //     so one warpgroup's exp work overlaps its own PV and the other warpgroup's MMAs. A quarter of the exponentials
 //     run as a polynomial on the FMA pipe (poly_exp2) next to the MUFU ones.
 //     The 288 threads x 224 registers of one CTA per SM fit the register file, so there is no setmaxnreg rebalancing.
-//   attention_tc_kernel<512, 128>  : single-head d = 512 (the AutoencoderKL mid-block AttnBlock,
-//     ldm/modules/diffusionmodules/model.py:178-202): one CTA = 128 query rows x ONE 128-column slice of the output
-//     (grid.y = 4 slices; S is recomputed per slice: a wider O does not fit the registers next to S), Q resident as
-//     eight 64-column panels, K streamed panel by panel through a 4-deep ring (S and PV are not overlapped here).
+//   attention_tc_kernel<D, DV>, D in {384, 512, 576, 960}: single-head attention at d = D, not causal (the
+//     AutoencoderKL mid-block AttnBlock at 512, ldm/modules/diffusionmodules/model.py:178-202; the SpatialTransformers of
+//     the class-conditional ImageNet LDM at 384 / 576 / 960, num_heads 1 with legacy dim_head = ch). One CTA = 128 query
+//     rows x ONE DV-column slice of the output (grid.y = D / DV slices; S is recomputed per slice: a wider O does not fit
+//     the registers next to S), K streamed panel by panel through a 4-deep ring (S and PV are not overlapped here).
 //     The N x N logits never leave the SM.
+//     DV is the widest PV slice that ptxas fits with no spills (at DV = 192 it spills and serialises the wgmmas):
+//       D = 384: DV = 128, 3 slices (S computed 3x), Q resident as 6 panels: 164,864 B of shared memory, 140 registers.
+//       D = 512: DV = 128, 4 slices (4x), Q resident as 8 panels: 197,632 B, 140 registers.
+//       D = 576: DV =  96, 6 slices (6x), Q resident as 9 panels: 205,824 B, 122 registers.
+//       D = 960: DV = 160, 6 slices (6x), 154 registers. A resident Q tile (240 KiB) does not fit the 227 KiB a CTA
+//         may have, so Q is streamed: each K-ring stage also carries the matching 64-column Q panel (16 KiB) on the
+//         same mbarrier and is freed with it (140,288 B). Q is then re-read from L2 once per 64-key tile; the engine's
+//         d = 960 layers have 16 or 64 tokens (a single tile) at the 32x32 / 64x64 latents.
 //
 // Replaces the materialised einsum('b i d, b j d -> b i j') * scale -> softmax -> einsum('b i j, b j d -> b i d')
 // of ldm/modules/attention.py:178-192 (and CLIP self-attention with a causal mask).
@@ -36,20 +46,26 @@ constexpr int AQ = 128;   // query rows per CTA
 constexpr int AKV = 64;   // kv rows per iteration
 constexpr int ATT_THREADS = 288;
 constexpr int ATT_PRODUCER_WARP = 8;
-constexpr int WIDE_D = 512;
-constexpr int WIDE_DV = 128;
+constexpr int MAX_SMEM = 232448;   // dynamic shared memory a CTA may opt into on sm_90
+
+// the single-head family (dpad = d > 192); the multi-head kernels use the 64 / 128 / 192 head slots
+__host__ __device__ constexpr bool attn_wide(int dpad) { return dpad > 192; }
 
 template <int DPAD, int DV>
 struct AttnCfg {
   static constexpr int PANELS = DPAD / 64;
-  static constexpr int Q_BYTES = AQ * DPAD * 2;
+  static constexpr int QP_BYTES = AQ * 128;                 // one 64-column Q panel
   static constexpr int KP_BYTES = AKV * 64 * 2;            // one 64-column K panel
   static constexpr int V_TX = DV * AKV * 2;                 // one V^T tile [DV x 64 keys]
   static constexpr int V_BYTES = (V_TX + 1023) / 1024 * 1024;   // ring stage: swizzle atoms stay 1024-byte aligned
   // multi-head: two tiles of K panels, so S_{j+1}'s panels load while S_j's are still held
-  static constexpr int KST = DPAD == WIDE_D ? 4 : (2 * PANELS < 4 ? 4 : 2 * PANELS);   // K panel ring depth
-  static constexpr int VST = DPAD == WIDE_D ? 2 : 4;   // V^T ring depth: the producer loads K_{j+1} after V_j's slot frees
+  static constexpr int KST = attn_wide(DPAD) ? 4 : (2 * PANELS < 4 ? 4 : 2 * PANELS);   // K panel ring depth
+  static constexpr int VST = attn_wide(DPAD) ? 2 : 4;   // V^T ring depth: the producer loads K_{j+1} after V_j's slot frees
+  // Q resident when it fits next to the rings, else streamed with the K panels (one Q panel per K-ring stage)
+  static constexpr bool STREAM_Q = PANELS * QP_BYTES + KST * KP_BYTES + VST * V_BYTES + 1024 > MAX_SMEM - 256;
+  static constexpr int Q_BYTES = STREAM_Q ? KST * QP_BYTES : PANELS * QP_BYTES;
   static constexpr int SMEM = Q_BYTES + KST * KP_BYTES + VST * V_BYTES + 1024;
+  static_assert(SMEM <= MAX_SMEM - 256, "attention tile does not fit shared memory");   // 256: static mbarriers
 };
 
 struct AttnArgs {
@@ -161,7 +177,8 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
     attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                         const __grid_constant__ CUtensorMap tmV, const AttnArgs p) {
   using Cfg = AttnCfg<DPAD, DV>;
-  constexpr bool WIDE = DPAD == WIDE_D;
+  constexpr bool WIDE = attn_wide(DPAD);
+  constexpr bool STREAM_Q = Cfg::STREAM_Q;
   constexpr int PANELS = Cfg::PANELS;
   constexpr int KST = Cfg::KST;
   constexpr int VST = Cfg::VST;
@@ -207,14 +224,21 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
   if (warp == ATT_PRODUCER_WARP) {
     if (elect_one()) {
       // tensor maps: Q / K {d, heads, rows, batch}, V^T {nkv, d, heads, batch}
-      mbar_arrive_expect_tx(&q_full, Cfg::Q_BYTES);
-      for (int pn = 0; pn < PANELS; ++pn) tma_load_4d(q_s + pn * (AQ * 128), &tmQ, &q_full, pn * 64, head, q0, b);
+      if constexpr (!STREAM_Q) {
+        mbar_arrive_expect_tx(&q_full, Cfg::Q_BYTES);
+        for (int pn = 0; pn < PANELS; ++pn) tma_load_4d(q_s + pn * (AQ * 128), &tmQ, &q_full, pn * 64, head, q0, b);
+      }
       int ks = 0;
       uint32_t kph = 0;
       for (int j = 0; j < n_iter; ++j) {
         for (int pn = 0; pn < PANELS; ++pn) {
           mbar_wait_mma(&k_empty[ks], kph ^ 1);
-          mbar_arrive_expect_tx(&k_full[ks], Cfg::KP_BYTES);
+          if constexpr (STREAM_Q) {   // the stage's Q panel rides on the K panel's barrier
+            mbar_arrive_expect_tx(&k_full[ks], Cfg::KP_BYTES + Cfg::QP_BYTES);
+            tma_load_4d(q_s + ks * Cfg::QP_BYTES, &tmQ, &k_full[ks], pn * 64, head, q0, b);
+          } else {
+            mbar_arrive_expect_tx(&k_full[ks], Cfg::KP_BYTES);
+          }
           tma_load_4d(k_s + ks * Cfg::KP_BYTES, &tmK, &k_full[ks], pn * 64, head, j * AKV, b);
           if (++ks == KST) {
             ks = 0;
@@ -249,7 +273,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
     float al0, al1;
     int ks = 0;
     uint32_t kph = 0;
-    mbar_wait_mma(&q_full, 0);
+    if constexpr (!STREAM_Q) mbar_wait_mma(&q_full, 0);
     if constexpr (WIDE) {
       for (int j = 0; j < n_iter; ++j) {
         // ---- S = Q K^T over the K panels of this tile; each panel is handed back once its MMAs have completed
@@ -259,11 +283,11 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
         for (int pn = 0; pn < PANELS; ++pn) {
           mbar_wait_mma(&k_full[ks], kph);
           const uint32_t k_addr = smem_u32(k_s + ks * Cfg::KP_BYTES);
+          const uint32_t qp_addr = STREAM_Q ? q_addr + ks * Cfg::QP_BYTES : q_addr + pn * Cfg::QP_BYTES;
           wgmma_fence();
 #pragma unroll
           for (int kk = 0; kk < 4; ++kk)
-            WgmmaSS<AKV>::mma(s, wg_desc(q_addr + pn * (AQ * 128) + kk * 32), wg_desc(k_addr + kk * 32),
-                              (pn | kk) != 0);
+            WgmmaSS<AKV>::mma(s, wg_desc(qp_addr + kk * 32), wg_desc(k_addr + kk * 32), (pn | kk) != 0);
           wgmma_commit();
           wgmma_wait<1>();
           if (prev >= 0 && lane == 0) mbar_arrive(&k_empty[prev]);
@@ -465,21 +489,31 @@ extern "C" int sdb_attention(const sdb_attn_desc* d, sdb_stream_t stream) {
   p.o_batch_stride = d->o_batch_stride;
   p.out = static_cast<__half*>(d->out);
   p.scale_log2 = d->scale * 1.4426950408889634f;
-  if (d->dpad == WIDE_D) {
-    // single-head d = 512 (AutoencoderKL AttnBlock): q, k [B, n, 512], vt [B, 512, ldvt]
-    SDB_CHECK(d->d == WIDE_D && d->heads == 1 && !d->causal, "sdb_attention: dpad 512 is the single-head d = 512 kernel");
-    SDB_CHECK(d->head_stride == 0 || d->head_stride == WIDE_D, "sdb_attention: dpad 512 takes head_stride 0 or 512");
+  if (d->dpad == 384 || d->dpad == 512 || d->dpad == 576 || d->dpad == 960) {
+    // single-head d = dpad (AutoencoderKL AttnBlock at 512, num_heads-1 SpatialTransformers at 384 / 576 / 960):
+    // q, k [B, n, d], vt [B, d, ldvt]
+    const int dp = d->dpad;
+    SDB_CHECK(d->d == dp && d->heads == 1 && !d->causal,
+              "sdb_attention: dpad %d is the single-head d = %d kernel (got d %d, heads %d, causal %d)", dp, dp, d->d,
+              d->heads, d->causal);
+    SDB_CHECK(d->head_stride == 0 || d->head_stride == dp, "sdb_attention: dpad %d takes head_stride 0 or %d", dp, dp);
     SDB_CHECK(d->batch > 0 && d->nq > 0 && d->nkv > 0, "sdb_attention: bad sizes");
     SDB_CHECK(d->ldq % 8 == 0 && d->ldk % 8 == 0 && d->ldvt % 8 == 0 && d->ldo % 8 == 0 && d->o_batch_stride % 8 == 0,
               "sdb_attention: leading dims must be multiples of 8");
-    if (make_attn_maps(d, 1, WIDE_D, WIDE_D, WIDE_DV, &tq, &tk, &tv)) return 1;
+    const int dv = dp == 576 ? 96 : (dp == 960 ? 160 : 128);   // PV slice width: dp / dv slices, S recomputed per slice
+    if (make_attn_maps(d, 1, dp, dp, dv, &tq, &tk, &tv)) return 1;
     p.heads = 1;
     p.causal = 0;
-    dim3 grid((d->nq + AQ - 1) / AQ, WIDE_D / WIDE_DV, d->batch);
-    return launch_attn<WIDE_D, WIDE_DV>(tq, tk, tv, p, grid, st);
+    dim3 grid((d->nq + AQ - 1) / AQ, dp / dv, d->batch);
+    switch (dp) {
+      case 384: return launch_attn<384, 128>(tq, tk, tv, p, grid, st);
+      case 512: return launch_attn<512, 128>(tq, tk, tv, p, grid, st);
+      case 576: return launch_attn<576, 96>(tq, tk, tv, p, grid, st);
+      default: return launch_attn<960, 160>(tq, tk, tv, p, grid, st);
+    }
   }
-  SDB_CHECK(d->dpad == 64 || d->dpad == 128 || d->dpad == 192, "sdb_attention: dpad must be 64/128/192/512 (got %d)",
-            d->dpad);
+  SDB_CHECK(d->dpad == 64 || d->dpad == 128 || d->dpad == 192,
+            "sdb_attention: dpad must be 64/128/192/384/512/576/960 (got %d)", d->dpad);
   SDB_CHECK(d->d > 0 && d->d <= d->dpad && d->d % 2 == 0, "sdb_attention: bad head dim %d", d->d);
   const int hs = d->head_stride ? d->head_stride : d->dpad;
   SDB_CHECK(hs >= d->d && hs % 8 == 0, "sdb_attention: head_stride %d must be >= d and a multiple of 8", hs);

@@ -527,13 +527,16 @@ def timestep_embedding_f32(t, dim, max_period=10000.0):
     return out
 
 
-def linear_small(x, w, bias=None, act=ACT_NONE, want_f16=False):
-    """x fp32 [m, k] (m small), w fp16 [n, k] -> fp32 [m, n] (fp32 activations end to end)."""
+def linear_small(x, w, bias=None, act=ACT_NONE, want_f16=False, out=None):
+    """x fp32 [m, k] (m small), w fp16 [n, k] -> fp32 [m, n] (fp32 activations end to end), into `out` if given."""
     _chk32(x, "x")
     _chk16(w, "w")
     m, k = x.shape
     n = w.shape[0]
-    out = torch.empty((m, n), dtype=torch.float32, device=x.device)
+    if out is None:
+        out = torch.empty((m, n), dtype=torch.float32, device=x.device)
+    _chk32(out, "out")
+    assert out.shape == (m, n)
     out16 = torch.empty((m, n), dtype=torch.float16, device=x.device) if want_f16 else None
     _l.check(_l.load().sdb_linear_small(_ptr(x), m, k, _ptr(w), n, _ptr(bias), act, _ptr(out), _ptr(out16),
                                         _stream()), "sdb_linear_small")

@@ -143,8 +143,9 @@ class UNetModel(nn.Module):
         # channels per fused GroupNorm-statistics entry: every channel count of the UNet (and of its skip concats) is a
         # multiple of model_channels, so the 32 groups always tile into entries of model_channels / 32 channels
         self._sg = model_channels // 32 if model_channels % 32 == 0 else 1
-        if not self.conditional:
-            # entries must also divide every GEMM tile width (multiples of 32): 192 channels -> 6 per group -> entries of 2
+        if not self.conditional or all(bn % self._sg for bn in (64, 128, 160, 256)):
+            # entries must also divide the GEMM tile widths (the GEMM drops the fused statistics otherwise): 192
+            # channels -> 6 per group -> entries of 2; SD-v1's 10 divides the 160-wide tiles
             self._sg = math.gcd(self._sg, 16)
         self.W = None           # packed weights (device)
         self._ctx_ref = None    # the context tensor whose cross-attention K/V are cached (strong reference)
@@ -274,7 +275,7 @@ class UNetModel(nn.Module):
             ch, d = a["ch"], a["dhead"]
             dp = _dpad(d)
             tb = pre + ".transformer_blocks.0"
-            s = {"ch": ch, "d": d, "dpad": dp, "heads": heads}
+            s = {"ch": ch, "d": d, "dpad": dp, "heads": heads, "tb": tb}
             s["gn"] = (f32(pre + ".norm.weight"), f32(pre + ".norm.bias"))
             s["w_in"], s["b_in"] = one(sd[pre + ".proj_in.weight"].reshape(ch, ch)), f32(pre + ".proj_in.bias")
             s["w_out"], s["b_out"] = one(sd[pre + ".proj_out.weight"].reshape(ch, ch)), f32(pre + ".proj_out.bias")
@@ -400,14 +401,20 @@ class UNetModel(nn.Module):
             vt3 = ops.transpose_f16(v.view(nb, ntok, hd))
         o = ops.attention(qk3[:, :, :hd], qk3[:, :, hd:], vt3, heads=heads, d=d, dpad=dp, nq=ntok, nkv=ntok, scale=scale,
                           head_stride=d)
-        _, t1 = ops.gemm(o.view(-1, ch), s["w_o1"], bias=s["b_o1"], residual=t0, want_f32=True, splits=-1)
-        # --- cross attention (K / V^T of the context are precomputed per prompt)
-        y = ops.layernorm(t1, *s["ln2"])
-        q, _ = ops.gemm(y, s["w_q2"], want_f16=True)
         k2, vt2, nkv = kv
-        o = ops.attention(q.view(nb, ntok, hd), k2, vt2, heads=heads, d=d, dpad=dp, nq=ntok, nkv=nkv, scale=scale,
-                          head_stride=d)
-        _, t2 = ops.gemm(o.view(-1, ch), s["w_o2"], bias=s["b_o2"], residual=t1, want_f32=True, splits=-1)
+        if k2 is None:
+            # one-token context (context_kv): attn2(LN2(t1), c) = u per sample, added as the FiLM operand of the attn1
+            # out-projection, which then yields t2 = t0 + attn1 + u directly
+            _, t2 = ops.gemm(o.view(-1, ch), s["w_o1"], bias=s["b_o1"], film=vt2, rows_per_sample=ntok, residual=t0,
+                             want_f32=True, splits=-1)
+        else:
+            _, t1 = ops.gemm(o.view(-1, ch), s["w_o1"], bias=s["b_o1"], residual=t0, want_f32=True, splits=-1)
+            # --- cross attention (K / V^T of the context are precomputed per prompt)
+            y = ops.layernorm(t1, *s["ln2"])
+            q, _ = ops.gemm(y, s["w_q2"], want_f16=True)
+            o = ops.attention(q.view(nb, ntok, hd), k2, vt2, heads=heads, d=d, dpad=dp, nq=ntok, nkv=nkv, scale=scale,
+                              head_stride=d)
+            _, t2 = ops.gemm(o.view(-1, ch), s["w_o2"], bias=s["b_o2"], residual=t1, want_f32=True, splits=-1)
         # --- GEGLU feed-forward
         y = ops.layernorm(t2, *s["ln3"])
         g, _ = ops.gemm(y, s["w_ff1"], bias=s["b_ff1"], act=ACT_GEGLU, want_f16=True,
@@ -451,12 +458,36 @@ class UNetModel(nn.Module):
             out._sdb_f16 = o16.view(nb, H, Wd, ch)
         return out
 
+    def _one_token_weights(self):
+        """[sum ch, context_dim] fp16 / [sum ch] fp32: W_o2 W_v2 of every SpatialTransformer (folded in fp64) and b_o2,
+        stacked so that u = W c + b for all of them is one weight-streaming launch."""
+        W = self.W
+        if "u_w" not in W:      # from the fp32 weights of the set in use: one fp16 rounding of the product
+            src = self._host_sd if self._active == "raw" else self._alt_sd[self._active]
+            f64 = lambda k: src[k].to(device=W["device"], dtype=torch.float64)
+            W["u_w"] = torch.cat([(f64(s["tb"] + ".attn2.to_out.0.weight") @ f64(s["tb"] + ".attn2.to_v.weight")).half()
+                                  for s in W["st_list"]], 0).contiguous()
+            W["u_b"] = torch.cat([s["b_o2"] for s in W["st_list"]], 0).contiguous()
+        return W["u_w"], W["u_b"]
+
     def context_kv(self, context, static=False):
         """Cross-attention K and V^T for all SpatialTransformers (x/t independent: once per prompt).
-        static=True writes into persistent per-shape buffers so captured CUDA graphs stay valid across prompts."""
+        static=True writes into persistent per-shape buffers so captured CUDA graphs stay valid across prompts.
+        A one-token context (the ClassEmbedder's) makes the softmax over one key exactly 1, so attn2(x, c) =
+        to_out(to_v(c)) does not depend on x: each SpatialTransformer gets (None, u [nb, ch], 1) with
+        u = W_o2 W_v2 c + b_o2 instead of K / V^T."""
         nb, nkv, cd = context.shape
-        ctx16 = ops.cast_f16(context.contiguous().float().view(nb * nkv, cd))
         bufs = self._kv_static.setdefault((nb, nkv), {}) if static else {}
+        if nkv == 1:
+            w, b = self._one_token_weights()
+            u = ops.linear_small(context.contiguous().float().view(nb, cd), w, b, out=bufs.get("u"))
+            bufs["u"] = u
+            out, off = [], 0
+            for s in self.W["st_list"]:
+                out.append((None, u[:, off: off + s["ch"]], 1))
+                off += s["ch"]
+            return out
+        ctx16 = ops.cast_f16(context.contiguous().float().view(nb * nkv, cd))
         ld = (nkv + 7) // 8 * 8
         out = []
         for i, s in enumerate(self.W["st_list"]):
@@ -661,7 +692,7 @@ class UNetModel(nn.Module):
             if not cached:
                 self.set_context(context)
             g = self._graph_for(tuple(x.shape), self._ctx_kv)
-            assert g["kvs"] is self._ctx_kv or all(a[0].data_ptr() == b[0].data_ptr() for a, b in zip(g["kvs"], self._ctx_kv))
+            assert g["kvs"] is self._ctx_kv or all(a[1].data_ptr() == b[1].data_ptr() for a, b in zip(g["kvs"], self._ctx_kv))
             if x.data_ptr() != g["x"].data_ptr():
                 g["x"].copy_(x)
             g["t"].copy_(timesteps)

@@ -26,6 +26,7 @@ TARGET_MAP = {
     "ldm.models.autoencoder.AutoencoderKL": "sdb200.vae.AutoencoderKL",
     "ldm.models.autoencoder.VQModelInterface": "sdb200.vq.VQModelInterface",
     "ldm.modules.encoders.modules.FrozenCLIPEmbedder": "sdb200.clip.FrozenCLIPEmbedder",
+    "ldm.modules.encoders.modules.ClassEmbedder": "sdb200.encoders.ClassEmbedder",
 }
 
 
