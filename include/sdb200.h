@@ -189,6 +189,13 @@ int sdb_nhwc_to_nchw(const float* x, int32_t nb, int32_t c, int32_t hw, float* o
  * pad_lo applies top/left, bottom/right pad is implied by ho/wo (openaimodel.py:149-153; model.py:72-76). */
 int sdb_im2col3x3(const float* x, int32_t nb, int32_t h, int32_t w, int32_t c, int32_t stride, int32_t pad_lo,
                   int32_t ho, int32_t wo, int32_t kpad, void* out_f16, sdb_stream_t stream);
+/* im2col of a concat-conditioned UNet's conv_in (DiffusionWrapper "concat", ddpm.py:1405-1407) straight from the two
+ * NCHW fp32 sources x [nb, cx, h, w] and cond [cond_nb, cc, cond_h, cond_w] (their dims must agree): 3x3, stride 1,
+ * pad 1, out fp16 [nb*h*w, kpad], k = (ky*3+kx)*(cx+cc) + ch, channels cx.. read from cond; 9*(cx+cc) <= kpad.
+ * Values equal im2col3x3 of the NHWC concat bit for bit. */
+int sdb_im2col3x3_concat(const float* x, int32_t nb, int32_t cx, int32_t h, int32_t w, const float* cond,
+                         int32_t cond_nb, int32_t cc, int32_t cond_h, int32_t cond_w, int32_t kpad, void* out_f16,
+                         sdb_stream_t stream);
 /* nearest 2x upsample NHWC fp32 -> fp16 (openaimodel.py:116; model.py:54) */
 int sdb_upsample2x(const float* x, int32_t nb, int32_t h, int32_t w, int32_t c, void* out_f16, sdb_stream_t stream);
 /* fp32 -> fp16 cast, optional transpose of [rows, cols] per batch into [cols, ldo] */
@@ -270,6 +277,19 @@ int sdb_ddpm_step(const float* x, const float* eps, const float* noise, float sq
  * may be NULL. e_dim 1 .. 8, any n_e (the codebook streams through shared memory). */
 int sdb_vq_quantize(const float* z, int64_t m, int32_t e_dim, float scale, const float* codebook, const float* code_sq,
                     int32_t n_e, float* z_q, int64_t* indices, sdb_stream_t stream);
+/* Inpainting pre-processing (scripts/inpaint.py make_batch + the interpolated mask channel), fp32 in the reference's
+ * operation order: image uint8 RGB [nb, h, w, 3], mask uint8 L [nb, h, w], m = (mask / 255 >= 0.5).
+ * masked_nchw fp32 [nb, 3, h, w] = ((1 - m) * (image / 255)) * 2 - 1 (the VQ encoder's input); channel mask_channel of
+ * cond fp32 [nb, cond_c, cond_h, cond_w] = nearest-resized m * 2 - 1 (F.interpolate's src = floor(dst * (float)in / out)).
+ * The other channels of cond are not written. */
+int sdb_inpaint_prepare(const uint8_t* image_u8, const uint8_t* mask_u8, int32_t nb, int32_t h, int32_t w,
+                        float* masked_nchw, float* cond, int32_t cond_c, int32_t cond_h, int32_t cond_w,
+                        int32_t mask_channel, sdb_stream_t stream);
+/* Inpainting composite (scripts/inpaint.py): x_nhwc fp32 [npix, 3] the decoded image, image uint8 [npix, 3], mask
+ * uint8 [npix]; out uint8 [npix, 3] = trunc(255 * ((1 - m) * clamp(((image / 255) * 2 - 1 + 1) / 2) + m * clamp((x + 1) / 2)))
+ * with m = (mask / 255 >= 0.5), fp32 in the reference's order. */
+int sdb_inpaint_composite(const float* x_nhwc, const uint8_t* image_u8, const uint8_t* mask_u8, int64_t npix,
+                          uint8_t* out_u8, sdb_stream_t stream);
 /* out = a*x + b (latent scaling z/0.18215, ddpm.py:713) */
 int sdb_axpby(const float* x, float a, float b, int64_t n, float* out, sdb_stream_t stream);
 /* out = a*x + b*y (DDIMSampler.stochastic_encode, ddim.py:206-220; q_sample, ddpm.py:274-277) */

@@ -78,6 +78,17 @@ VQ_F4 = dict(embed_dim=3, n_embed=8192, ddconfig=dict(double_z=False, z_channels
 TINY_VQ = dict(embed_dim=3, n_embed=512, ddconfig=dict(double_z=False, z_channels=3, resolution=32, in_channels=3, out_ch=3,
                                                         ch=64, ch_mult=[1, 2], num_res_blocks=1, attn_resolutions=[],
                                                         dropout=0.0))
+# the LDM inpainting model (models/ldm/inpainting_big/config.yaml, scripts/inpaint.py): x_t (3 channels) concatenated
+# with the VQ encoding of the masked image (3) and the resized mask (1); AttentionBlocks of 8 heads at d = 64 / 96 / 128,
+# up / down ResBlocks without scale-shift norm. The first stage is VQ-f4 without mid-block attention.
+INPAINTING_BIG_UNET = dict(image_size=64, in_channels=7, out_channels=3, model_channels=256,
+                           attention_resolutions=[8, 4, 2], num_res_blocks=2, channel_mult=[1, 2, 3, 4], num_heads=8,
+                           resblock_updown=True)
+VQ_F4_NOATTN = dict(embed_dim=3, n_embed=8192, ddconfig={**VQ_F4["ddconfig"], "attn_type": "none"})
+# small members for tests: heads of d = 16 and 24 at two attention levels; a VQ-f2 without mid-block attention
+TINY_INPAINT_UNET = dict(image_size=16, in_channels=7, out_channels=3, model_channels=64, attention_resolutions=[2, 4],
+                         num_res_blocks=1, channel_mult=[1, 2, 3], num_heads=8, resblock_updown=True)
+TINY_VQ_NOATTN = dict(embed_dim=3, n_embed=512, ddconfig={**TINY_VQ["ddconfig"], "attn_type": "none"})
 TINY_VAE = dict(embed_dim=4, ddconfig=dict(double_z=True, z_channels=4, resolution=32, in_channels=3, out_ch=3,
                                            ch=64, ch_mult=[1, 2], num_res_blocks=1, attn_resolutions=[],
                                            dropout=0.0))
@@ -273,11 +284,17 @@ def _attn_shapes(p, pre, c):
 
 
 def vae_param_shapes(cfg):
-    """Keys as AutoencoderKL.state_dict() (encoder.*, decoder.*, quant_conv.*, post_quant_conv.*) — 248 tensors."""
+    """Keys as AutoencoderKL.state_dict() (encoder.*, decoder.*, quant_conv.*, post_quant_conv.*) — 248 tensors.
+    ddconfig.attn_type "none" (make_attn, model.py:205-211: nn.Identity) drops the mid-block attention keys."""
     dd = cfg["ddconfig"]
     ch, mult, nrb = dd["ch"], dd["ch_mult"], dd["num_res_blocks"]
     zc = dd["z_channels"]
     assert not dd["attn_resolutions"], "SD v1 VAE has attention only in the mid block"
+    attn_type = dd.get("attn_type", "vanilla")
+    if attn_type == "linear":
+        raise NotImplementedError("ddconfig attn_type 'linear' (LinAttnBlock) is not supported")
+    assert attn_type in ("vanilla", "none"), f"attn_type {attn_type} unknown"
+    mid_attn = attn_type == "vanilla"
     p = OrderedDict()
     # encoder (model.py:368-432)
     p["encoder.conv_in.weight"] = (ch, dd["in_channels"], 3, 3)
@@ -294,7 +311,8 @@ def vae_param_shapes(cfg):
             p[f"encoder.down.{lvl}.downsample.conv.weight"] = (bi, bi, 3, 3)
             p[f"encoder.down.{lvl}.downsample.conv.bias"] = (bi,)
     _resnet_shapes(p, "encoder.mid.block_1", bi, bi)
-    _attn_shapes(p, "encoder.mid.attn_1", bi)
+    if mid_attn:
+        _attn_shapes(p, "encoder.mid.attn_1", bi)
     _resnet_shapes(p, "encoder.mid.block_2", bi, bi)
     p["encoder.norm_out.weight"] = (bi,)
     p["encoder.norm_out.bias"] = (bi,)
@@ -306,7 +324,8 @@ def vae_param_shapes(cfg):
     p["decoder.conv_in.weight"] = (bi, zc, 3, 3)
     p["decoder.conv_in.bias"] = (bi,)
     _resnet_shapes(p, "decoder.mid.block_1", bi, bi)
-    _attn_shapes(p, "decoder.mid.attn_1", bi)
+    if mid_attn:
+        _attn_shapes(p, "decoder.mid.attn_1", bi)
     _resnet_shapes(p, "decoder.mid.block_2", bi, bi)
     ups = OrderedDict()
     for lvl in reversed(range(len(mult))):

@@ -27,11 +27,18 @@ class DiffusionWrapper(nn.Module):
         super().__init__()
         self.diffusion_model = instantiate_from_config(remap_config(diff_model_config))
         self.conditioning_key = conditioning_key
-        assert self.conditioning_key in [None, "crossattn"], "supported: crossattn (SD v1) or None (unconditional)"
+        assert self.conditioning_key in [None, "concat", "crossattn", "hybrid", "adm"]
+        if self.conditioning_key in ("hybrid", "adm"):
+            raise NotImplementedError(f"conditioning_key {self.conditioning_key!r}: supported are crossattn (SD v1), "
+                                      "concat (inpainting) and None (unconditional)")
 
     def forward(self, x, t, c_concat=None, c_crossattn=None):
         if self.conditioning_key is None:
             return self.diffusion_model(x, t)
+        if self.conditioning_key == "concat":
+            # the UNet reads x and the conditioning as two sources (no cat([x] + c_concat) per step)
+            c = c_concat[0] if len(c_concat) == 1 else torch.cat(c_concat, 1)
+            return self.diffusion_model(x, t, concat=c)
         cc = c_crossattn[0] if len(c_crossattn) == 1 else torch.cat(c_crossattn, 1)
         return self.diffusion_model(x, t, context=cc)
 
@@ -90,9 +97,10 @@ class LatentDiffusion(nn.Module):
         if use_ema:
             self.model_ema = _EmaWeights(self.model.diffusion_model)
         self.first_stage_model = instantiate_from_config(remap_config(first_stage_config))
-        if cond_stage_config == "__is_first_stage__":
-            raise NotImplementedError(cond_stage_config)
-        self.cond_stage_model = instantiate_from_config(remap_config(cond_stage_config))
+        if cond_stage_config == "__is_first_stage__":      # ddpm.py:511-513: one module under both prefixes
+            self.cond_stage_model = self.first_stage_model
+        else:
+            self.cond_stage_model = instantiate_from_config(remap_config(cond_stage_config))
         self.register_schedule(timesteps, linear_start, linear_end)
 
     # -- schedule: fp64 numpy -> fp32 buffers (ddpm.py:117-169, util.py:21-25)
@@ -151,15 +159,16 @@ class LatentDiffusion(nn.Module):
         else:
             if not isinstance(cond, list):
                 cond = [cond]
-            cond = {"c_crossattn": cond}
+            cond = {"c_concat" if self.model.conditioning_key == "concat" else "c_crossattn": cond}
         x_recon = self.model(x_noisy, t, **cond)
         if isinstance(x_recon, tuple) and not return_ids:
             return x_recon[0]
         return x_recon
 
     def set_context(self, c):
-        """Fast path used by sdb200 samplers: cross-attention K/V of the (guidance-doubled) context, once per batch."""
-        if c is not None:
+        """Fast path used by sdb200 samplers: cross-attention K/V of the (guidance-doubled) context, once per batch. A
+        concat model has no cross-attention: its conditioning reaches the UNet through apply_model on every step."""
+        if c is not None and self.model.conditioning_key == "crossattn":
             self.model.diffusion_model.set_context(c)
 
     def get_learned_conditioning(self, c):

@@ -93,6 +93,7 @@ SIGNATURES = {
     "sdb_nchw_to_nhwc": ([_P, _I, _I, _I, _P, _P, _P], C.c_int),
     "sdb_nhwc_to_nchw": ([_P, _I, _I, _I, _P, _P], C.c_int),
     "sdb_im2col3x3": ([_P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P], C.c_int),
+    "sdb_im2col3x3_concat": ([_P, _I, _I, _I, _I, _P, _I, _I, _I, _I, _I, _P, _P], C.c_int),
     "sdb_upsample2x": ([_P, _I, _I, _I, _I, _P, _P], C.c_int),
     "sdb_cast_f16": ([_P, _L, _P, _P], C.c_int),
     "sdb_transpose_f16": ([_P, _I, _I, _I, _I, _P, _I, _P], C.c_int),
@@ -109,6 +110,8 @@ SIGNATURES = {
     "sdb_dpm_solver_step": ([_P, _P, _P, _I, _F, _F, _F, _I, _P, _F, _F, _F, _L, _P, _P, _P, _P], C.c_int),
     "sdb_mask_blend": ([_P, _P, _I, _I, _I, _L, _P, _P, _P], C.c_int),
     "sdb_axpby2": ([_P, _P, _F, _F, _L, _P, _P], C.c_int),
+    "sdb_inpaint_prepare": ([_P, _P, _I, _I, _I, _P, _P, _I, _I, _I, _I, _P], C.c_int),
+    "sdb_inpaint_composite": ([_P, _P, _P, _L, _P, _P], C.c_int),
     # post-processing (safety.cu)
     "sdb_resample_u8": ([_P, _P, _I, _I, _I, _I, _I, _P, _P, _I, _I, _P, _P], C.c_int),
     "sdb_clip_normalize": ([_P, _I, _I, _I, _I, _F, _F, _F, _F, _F, _F, _P, _P], C.c_int),

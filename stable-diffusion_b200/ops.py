@@ -469,6 +469,50 @@ def im2col3x3(x, stride, pad_lo, ho, wo, kpad):
     return out
 
 
+def im2col3x3_concat(x, cond, kpad):
+    """3x3 / pad 1 im2col of cat([x, cond], 1) from the two NCHW fp32 tensors -> fp16 [nb*h*w, kpad]."""
+    _chk32(x, "x")
+    _chk32(cond, "cond")
+    nb, cx, h, w = x.shape
+    out = torch.empty((nb * h * w, kpad), dtype=torch.float16, device=x.device)
+    _l.check(_l.load().sdb_im2col3x3_concat(_ptr(x), nb, cx, h, w, _ptr(cond), cond.shape[0], cond.shape[1],
+                                            cond.shape[2], cond.shape[3], kpad, _ptr(out), _stream()),
+             "sdb_im2col3x3_concat")
+    _count()
+    return out
+
+
+def inpaint_prepare(image_u8, mask_u8, cond, mask_channel):
+    """image uint8 [nb, h, w, 3], mask uint8 [nb, h, w] -> the masked image fp32 NCHW [nb, 3, h, w]; writes the resized
+    ±1 mask into channel `mask_channel` of cond fp32 [nb, c, hc, wc] (sdb_inpaint_prepare)."""
+    _chk32(cond, "cond")
+    nb, h, w, _ = image_u8.shape
+    assert image_u8.dtype == torch.uint8 and mask_u8.dtype == torch.uint8 and image_u8.shape[3] == 3
+    assert image_u8.is_contiguous() and mask_u8.is_contiguous() and tuple(mask_u8.shape) == (nb, h, w)
+    assert cond.shape[0] == nb
+    masked = torch.empty((nb, 3, h, w), dtype=torch.float32, device=image_u8.device)
+    _l.check(_l.load().sdb_inpaint_prepare(_ptr(image_u8), _ptr(mask_u8), nb, h, w, _ptr(masked), _ptr(cond),
+                                           cond.shape[1], cond.shape[2], cond.shape[3], mask_channel, _stream()),
+             "sdb_inpaint_prepare")
+    _count(2)
+    return masked
+
+
+def inpaint_composite(x_nhwc, image_u8, mask_u8):
+    """Decoded image fp32 NHWC [nb, h, w, 3], original image uint8 [nb, h, w, 3], mask uint8 [nb, h, w] -> the inpainted
+    uint8 image [nb, h, w, 3] (sdb_inpaint_composite)."""
+    _chk32(x_nhwc, "x_nhwc")
+    assert image_u8.dtype == torch.uint8 and mask_u8.dtype == torch.uint8
+    assert image_u8.is_contiguous() and mask_u8.is_contiguous()
+    assert tuple(image_u8.shape) == tuple(x_nhwc.shape) and x_nhwc.shape[-1] == 3
+    assert tuple(mask_u8.shape) == tuple(x_nhwc.shape[:-1])
+    out = torch.empty(image_u8.shape, dtype=torch.uint8, device=image_u8.device)
+    _l.check(_l.load().sdb_inpaint_composite(_ptr(x_nhwc), _ptr(image_u8), _ptr(mask_u8), mask_u8.numel(), _ptr(out),
+                                             _stream()), "sdb_inpaint_composite")
+    _count()
+    return out
+
+
 def upsample2x(x):
     _chk32(x, "x")
     nb, h, w, c = x.shape

@@ -549,26 +549,31 @@ class UNetModel(nn.Module):
                 _, o = ops.gemm(up, p["w"], taps=9, bias=p["b"], want_f32=True, splits=-1, want_stats=True, stats_group=self._sg)
                 h = o.view(nb, 2 * H, 2 * Wd, c)
             elif kind == "conv_in":
-                nb, H, Wd, c = h.shape
-                col = ops.im2col3x3(h, 1, 1, H, Wd, 64)
+                if isinstance(h, tuple):    # concat route: (x, conditioning), both NCHW, one im2col for the pair
+                    nb, _, H, Wd = h[0].shape
+                    col = ops.im2col3x3_concat(h[0], h[1], 64)
+                else:
+                    nb, H, Wd, c = h.shape
+                    col = ops.im2col3x3(h, 1, 1, H, Wd, 64)
                 _, o = ops.gemm(col, p["w"], bias=p["b"], want_f32=True, rows_per_sample=H * Wd, want_stats=True, stats_group=self._sg)
                 h = o.view(nb, H, Wd, p["cout"])
         return h
 
     # ------------------------------------------------------------------ forward
-    def _forward_impl(self, x, t, kvs):
-        """x NCHW fp32, t fp32 [nb], kvs from context_kv -> eps NCHW fp32. Pure kernel sequence (graph-capturable)."""
+    def _forward_impl(self, x, t, kvs, concat=None):
+        """x NCHW fp32, t fp32 [nb], kvs from context_kv, concat: NCHW fp32 channels that follow x's (or None) -> eps
+        NCHW fp32. Pure kernel sequence (graph-capturable)."""
         nb, _, H, Wd = x.shape
         if self._arena is None:
             self._arena = ops.StatsArena(x.device)
         self._arena.reset()          # one memset for all fused GroupNorm statistics of this evaluation
         ops.ARENA = self._arena
         try:
-            return self._forward_body(x, t, kvs)
+            return self._forward_body(x, t, kvs, concat)
         finally:
             ops.ARENA = None
 
-    def _forward_body(self, x, t, kvs):
+    def _forward_body(self, x, t, kvs, concat=None):
         nb, _, H, Wd = x.shape
         # The FiLM chain (timestep embedding -> time_embed MLP -> all emb_layers, three weight-streaming launches, ~37 us)
         # depends on t only: it runs on a side stream next to nchw->nhwc / conv_in and joins before the first ResBlock.
@@ -580,7 +585,7 @@ class UNetModel(nn.Module):
         with torch.cuda.stream(side):
             film = self._film(t)
         film.record_stream(cur)
-        h, _ = ops.nchw_to_nhwc(x)
+        h = (x, concat) if concat is not None else ops.nchw_to_nhwc(x)[0]
         W = self.W
         hs = []
         st_idx = [0]
@@ -605,29 +610,32 @@ class UNetModel(nn.Module):
             _, o = ops.gemm(hn, W["w_out"], taps=9, bias=W["b_out"], want_f32=True)
         return ops.nhwc_to_nchw(o.view(nb, H, Wd, self.out_channels))
 
-    def _graph_for(self, shape, kvs):
-        """Capture one UNet evaluation (~400 kernels) as a CUDA graph with static x / t / eps / K,V buffers."""
-        g = self._graphs.get(shape)
+    def _graph_for(self, shape, kvs, concat_shape=None):
+        """Capture one UNet evaluation (~400 kernels) as a CUDA graph with static x / t / eps / K,V buffers, and a static
+        conditioning buffer on the concat route."""
+        key = shape if concat_shape is None else (shape, concat_shape)
+        g = self._graphs.get(key)
         if g is None:
             dev = self.W["device"]
             sx = torch.zeros(shape, dtype=torch.float32, device=dev)
             st = torch.zeros((shape[0],), dtype=torch.float32, device=dev)
+            sc = None if concat_shape is None else torch.zeros(concat_shape, dtype=torch.float32, device=dev)
             side = torch.cuda.Stream()
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):      # warm-up outside capture: cudaFuncSetAttribute, allocator pools,
                 ops.AUTOTUNE = self.autotune   # and one-time (block_n, split-K) selection per GEMM problem
                 try:
-                    self._forward_impl(sx, st, kvs)
+                    self._forward_impl(sx, st, kvs, sc)
                 finally:
                     ops.AUTOTUNE = False
-                self._forward_impl(sx, st, kvs)
+                self._forward_impl(sx, st, kvs, sc)
             torch.cuda.current_stream().wait_stream(side)
             graph = torch.cuda.CUDAGraph()
             n0 = ops.launch_count()
             with torch.cuda.graph(graph):
-                out = self._forward_impl(sx, st, kvs)
-            g = {"graph": graph, "x": sx, "t": st, "out": out, "launches": ops.launch_count() - n0, "kvs": kvs}
-            self._graphs[shape] = g
+                out = self._forward_impl(sx, st, kvs, sc)
+            g = {"graph": graph, "x": sx, "t": st, "c": sc, "out": out, "launches": ops.launch_count() - n0, "kvs": kvs}
+            self._graphs[key] = g
         return g
 
     # ------------------------------------------------------------------ handle-level C entry (include/sdb200.h)
@@ -675,18 +683,25 @@ class UNetModel(nn.Module):
         assert context is not None and context.shape[0] == nb and context.shape[2] == self.context_dim
 
     @torch.no_grad()
-    def forward(self, x, timesteps=None, context=None, y=None, **kwargs):
+    def forward(self, x, timesteps=None, context=None, y=None, concat=None, **kwargs):
+        """eps = UNet(x, t[, context]). concat: NCHW channels that follow x's in the UNet input (DiffusionWrapper's
+        "concat" conditioning): forward(x, t, concat=c) equals forward(cat([x, c], 1), t) without building the concat."""
         assert y is None, "must specify y if and only if the model is class-conditional"
         assert self.W is not None, "weights not loaded (load_state_dict / load_weights, then .cuda())"
         if not x.is_cuda:
             raise RuntimeError("sdb200.UNetModel runs on CUDA (sm_90a) only; there is no CPU fallback")
-        assert x.dim() == 4 and x.shape[1] == self.in_channels
+        cin = x.shape[1] + (0 if concat is None else concat.shape[1])
+        assert x.dim() == 4 and cin == self.in_channels, (tuple(x.shape), self.in_channels)
+        if concat is not None:
+            assert not self.conditional, "concat conditioning with a spatial-transformer UNet is not supported"
+            assert concat.dim() == 4 and concat.shape[0] == x.shape[0] and concat.shape[2:] == x.shape[2:], \
+                (tuple(concat.shape), tuple(x.shape))
         self._check_context(context, x.shape[0])
         nb, _, H, Wd = x.shape
         lv = len(self.cfg["channel_mult"]) - 1
         assert H % (1 << lv) == 0 and Wd % (1 << lv) == 0, "latent size must be divisible by 2^(levels-1)"
         if not self.conditional:
-            return self._forward_uncond(x, timesteps)
+            return self._forward_uncond(x, timesteps, concat)
         cached = self._context_cached(context)
         if self.use_cuda_graph:
             if not cached:
@@ -706,17 +721,20 @@ class UNetModel(nn.Module):
         eps = self._forward_impl(x.contiguous().float(), t, kvs)
         return eps.to(x.dtype)
 
-    def _forward_uncond(self, x, timesteps):
+    def _forward_uncond(self, x, timesteps, concat=None):
         if self.use_cuda_graph:
-            g = self._graph_for(tuple(x.shape), None)
+            g = self._graph_for(tuple(x.shape), None, None if concat is None else tuple(concat.shape))
             if x.data_ptr() != g["x"].data_ptr():
                 g["x"].copy_(x)
+            if concat is not None and concat.data_ptr() != g["c"].data_ptr():
+                g["c"].copy_(concat)
             g["t"].copy_(timesteps)
             g["graph"].replay()
             ops.add_graph_launches(g["launches"])
             return g["out"].clone() if x.dtype == torch.float32 else g["out"].to(x.dtype)
         t = timesteps.to(torch.float32).contiguous()
-        return self._forward_impl(x.contiguous().float(), t, None).to(x.dtype)
+        c = None if concat is None else concat.contiguous().float()
+        return self._forward_impl(x.contiguous().float(), t, None, c).to(x.dtype)
 
 
 class CUNet:

@@ -133,8 +133,10 @@ class ConvAutoencoder(nn.Module):
             return out
 
         for side in ("encoder", "decoder"):
+            # attn_type "none": the mid attention is nn.Identity and has no keys
+            mid_attn = attn(side + ".mid.attn_1") if side + ".mid.attn_1.q.weight" in sd else None
             W[side] = {"conv_in": conv3(side + ".conv_in"), "mid1": resnet(side + ".mid.block_1"),
-                       "attn": attn(side + ".mid.attn_1"), "mid2": resnet(side + ".mid.block_2"),
+                       "attn": mid_attn, "mid2": resnet(side + ".mid.block_2"),
                        "gn_out": (f32(side + ".norm_out.weight"), f32(side + ".norm_out.bias")),
                        "conv_out": conv3(side + ".conv_out")}
         W["encoder"]["levels"] = levels("encoder.down", "downsample")
@@ -221,7 +223,8 @@ class ConvAutoencoder(nn.Module):
         D = self.W["decoder"]
         h = self._conv3(D["conv_in"], x32=h)
         h = self._resnet(D["mid1"], h)
-        h = self._attn(D["attn"], h)
+        if D["attn"] is not None:
+            h = self._attn(D["attn"], h)
         h = self._resnet(D["mid2"], h)
         for lvl in reversed(D["levels"]):
             for r in lvl["blocks"]:
@@ -247,7 +250,8 @@ class ConvAutoencoder(nn.Module):
                                 splits=-1, want_stats=True, stats_group=_sg(c))
                 h = o.view(nb, H // 2, Wd // 2, c)
         h = self._resnet(E["mid1"], h)
-        h = self._attn(E["attn"], h)
+        if E["attn"] is not None:
+            h = self._attn(E["attn"], h)
         h = self._resnet(E["mid2"], h)
         hn, _ = ops.groupnorm(h, *E["gn_out"], eps=1e-6, silu=True)
         return self._conv3(E["conv_out"], x16=hn)
