@@ -96,6 +96,25 @@ def gemm(a0, b, *, a1=None, a2=None, a3=None, nb=None, h=None, w=None, taps=1, b
     assert b.shape[1] == kb, (b.shape, taps, chans)
     M = nb * h * w
     n_out = n // 2 if act == ACT_GEGLU else n
+    # the descriptor carries one row stride per operand and assumes unit column stride: check the layouts it implies
+    if bias is not None:
+        _chk32(bias, "bias")
+        assert tuple(bias.shape) == (n,), f"bias: need fp32 [{n}], got {tuple(bias.shape)}"
+    if film is not None:
+        assert film.dtype == torch.float32 and film.is_cuda and film.dim() == 2, "film: need a 2-D cuda fp32 matrix"
+        assert film.shape[1] == n and film.stride(1) == 1, f"film: need [samples, {n}] with unit column stride"
+        rps_ = rows_per_sample if rows_per_sample else h * w
+        assert film.shape[0] >= (M + rps_ - 1) // rps_, "film: fewer rows than samples"
+    if residual is not None:
+        assert residual.dtype == torch.float32 and residual.is_cuda, "residual: need cuda fp32"
+        residual = residual.view(-1, residual.shape[-1])     # raises when the rows are not one stride apart
+        assert tuple(residual.shape) == (M, n_out) and residual.stride(1) == 1, \
+            f"residual: need [{M}, {n_out}] rows with unit column stride, got {tuple(residual.shape)} {residual.stride()}"
+    for t_, dt, name in ((out_f16, torch.float16, "out_f16"), (out_f32, torch.float32, "out_f32"),
+                         (out_f16_lo, torch.float16, "out_f16_lo")):
+        if t_ is not None:
+            assert t_.dtype == dt and t_.is_cuda and t_.is_contiguous(), f"{name}: need contiguous cuda {dt}"
+            assert t_.numel() == M * n_out and t_.shape[-1] == n_out, f"{name}: need [{M}, {n_out}], got {tuple(t_.shape)}"
     if out_f16 is None and (want_f16 or want_lo):
         out_f16 = torch.empty((M, n_out), dtype=torch.float16, device=a0.device)
     if out_f16_lo is None and want_lo:
@@ -116,7 +135,7 @@ def gemm(a0, b, *, a1=None, a2=None, a3=None, nb=None, h=None, w=None, taps=1, b
     d.ldf = film.stride(0) if film is not None else 0
     d.rows_per_sample = rows_per_sample
     d.residual = _ptr(residual)
-    d.ldr = residual.shape[-1] if residual is not None else 0
+    d.ldr = residual.stride(0) if residual is not None else 0
     d.act = act
     d.out_f16, d.out_f32, d.out_f16_lo = _ptr(out_f16), _ptr(out_f32), _ptr(out_f16_lo)
     d.ldo = 0
@@ -138,8 +157,7 @@ def gemm(a0, b, *, a1=None, a2=None, a3=None, nb=None, h=None, w=None, taps=1, b
     plan = (C.c_int32 * 5)()
     tunable = block_n == 0 and pair == 0 and splitk_mode == 0 and splits in (0, -1) and act != ACT_GEGLU
     if tunable:
-        key = (M, n, b.shape[1], taps, len(srcs), bias is not None, film is not None, residual is not None, act,
-               out_f16 is not None, out_f32 is not None, out_f16_lo is not None, stats_ok, stats_group, conv_stride)
+        key = tune_key(d, b.shape[1], stats_ok)
         choice = TUNED.get(key)
         if choice is None and AUTOTUNE:
             choice = TUNED[key] = _tune_gemm(d, M, n, rps, stats_ok, stats_group)
@@ -212,16 +230,18 @@ def channel_stats(x):
     return st
 
 
-def _tune_gemm(d, M, n, rps, stats_ok, stats_group):
-    """Time the (tile width, CTA pair, split-K) candidates of one GEMM problem on its real operands (CUDA events, GPU
-    kept busy by a leading spin so host launch gaps do not enter) and return the fastest
-    (block_n, pair, splits, splitk_mode)."""
+def tune_key(d, kb, stats_ok):
+    """Key of the autotuner's cache (TUNED) for the descriptor gemm() built; kb = columns of B."""
+    nsrc = sum(1 for p in (d.a0, d.a1, d.a2, d.a3) if p)
+    return (d.nb * d.h * d.w, d.n, kb, d.taps, nsrc, bool(d.bias), bool(d.film), bool(d.residual), d.act,
+            bool(d.out_f16), bool(d.out_f32), bool(d.out_f16_lo), stats_ok, d.stats_group, d.conv_stride)
+
+
+def tune_candidates(d, M, n):
+    """The (block_n, pair, splits, splitk_mode) candidates the autotuner times for descriptor `d`, in timing order, and
+    the largest statistics slot count T among them. d.stats_out must already be set (a placeholder will do) when
+    statistics are wanted; d's tile fields are left at the last candidate tried."""
     lib = _l.load()
-    st = _stream()
-    keep = (d.block_n, d.pair, d.splits, d.splitk_mode, d.stats_out)
-    scratch = None
-    if stats_ok:
-        d.stats_out = C.c_void_p(16)     # placeholder while the candidates are planned (sized below)
     plan = (C.c_int32 * 5)()
     cands = []
     max_slots = 1
@@ -246,6 +266,20 @@ def _tune_gemm(d, M, n, rps, stats_ok, stats_group):
                     continue
                 cands.append((bn, cg, sp, mode))
                 max_slots = max(max_slots, int(plan[4]))
+    return cands, max_slots
+
+
+def _tune_gemm(d, M, n, rps, stats_ok, stats_group):
+    """Time the (tile width, CTA pair, split-K) candidates of one GEMM problem on its real operands (CUDA events, GPU
+    kept busy by a leading spin so host launch gaps do not enter) and return the fastest
+    (block_n, pair, splits, splitk_mode)."""
+    lib = _l.load()
+    st = _stream()
+    keep = (d.block_n, d.pair, d.splits, d.splitk_mode, d.stats_out)
+    scratch = None
+    if stats_ok:
+        d.stats_out = C.c_void_p(16)     # placeholder while the candidates are planned (sized below)
+    cands, max_slots = tune_candidates(d, M, n)
     if stats_ok:
         # the statistics slots per sample depend on the candidate (tiles x cluster splits, or one per 32 rows with the
         # workspace epilogue): size the scratch for the largest one - a smaller buffer is overrun by the epilogues
