@@ -290,6 +290,22 @@ int sdb_inpaint_prepare(const uint8_t* image_u8, const uint8_t* mask_u8, int32_t
  * with m = (mask / 255 >= 0.5), fp32 in the reference's order. */
 int sdb_inpaint_composite(const float* x_nhwc, const uint8_t* image_u8, const uint8_t* mask_u8, int64_t npix,
                           uint8_t* out_u8, sdb_stream_t stream);
+/* Super-resolution conditioning (notebook_helpers.py get_cond): image uint8 RGB [nb, h, w, 3] -> out fp32
+ * [nb, 3, h, w] = 2 * (image / 255) - 1, fp32 in the reference's order (ToTensor, then 2c - 1). */
+int sdb_lr_prepare(const uint8_t* image_u8, int32_t nb, int32_t h, int32_t w, float* out_nchw, sdb_stream_t stream);
+/* Patch tiling of LatentDiffusion's split_input_params path (ddpm.py:611-651): nn.Unfold(kernel (kh, kw), stride
+ * (sy, sx)) of x fp32 [nb, c, h, w] viewed as tiles fp32 [L*nb, c, kh, kw], tile index l*nb + n, l = ty*lx + tx,
+ * ly = (h - kh) / sy + 1, lx = (w - kw) / sx + 1 (rows / columns the tiles miss are dropped, as by Unfold). A copy. */
+int sdb_patch_unfold(const float* x, int32_t nb, int32_t c, int32_t h, int32_t w, int32_t kh, int32_t kw, int32_t sy,
+                     int32_t sx, float* tiles, sdb_stream_t stream);
+/* The stitch of the split path: out fp32 [nb, c, h, w] = fold(tiles * weight) / norm with nn.Fold(kernel (kh, kw),
+ * stride (sy, sx)); tiles fp32 [ly*lx*nb, c, kh, kw] (tiles_nhwc 0) or [ly*lx*nb, kh, kw, c] (1) in sdb_patch_unfold's
+ * order, weight fp32 [ly*lx, kh, kw] (get_weighting, per tile), norm fp32 [h, w] (fold of the weights). The tiles must
+ * cover the output exactly: h = (ly - 1) * sy + kh, w = (lx - 1) * sx + kw. Each output element sums its covering tiles
+ * in a fixed order (no atomics): deterministic. */
+int sdb_patch_fold(const float* tiles, int32_t tiles_nhwc, int32_t nb, int32_t c, int32_t kh, int32_t kw, int32_t ly,
+                   int32_t lx, int32_t sy, int32_t sx, const float* weight, const float* norm, int32_t h, int32_t w,
+                   float* out_nchw, sdb_stream_t stream);
 /* out = a*x + b (latent scaling z/0.18215, ddpm.py:713) */
 int sdb_axpby(const float* x, float a, float b, int64_t n, float* out, sdb_stream_t stream);
 /* out = a*x + b*y (DDIMSampler.stochastic_encode, ddim.py:206-220; q_sample, ddpm.py:274-277) */

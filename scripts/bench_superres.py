@@ -1,0 +1,112 @@
+#!/usr/bin/env python
+"""LDM super-resolution (models/ldm/bsr_sr) speed on the H100 engine: the reference notebook's workload, a 256x256 input
+to a 1024x1024 image (latent 256x256 in 3x3 tiles of 128x128 at stride 64, DDIM-100, eta 1, batch 1, LR conversion +
+tiled sampling + tiled VQ-f4 decode), on seeded random weights and a seeded random input.
+Also reports, with CUDA events: one tiled UNet evaluation (the 9 tiles of (3 + 3) x 128x128 as one graph-replayed batch)
+and its TFLOP/s from the layer shapes; the same 9 tiles as 9 graph-replayed calls of one tile; the tiled decode; the
+stitch kernels (sdb_patch_fold for eps at 256x256 and for the decode at 1024x1024, and the per-step sdb_patch_unfold).
+Prints one JSON line with the card name and power limit read in the same run.
+
+  python scripts/bench_superres.py --repeats 2 --out outputs/superres.json
+"""
+import argparse
+import json
+import os
+import sys
+import time
+
+import numpy as np
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from sdb200 import arch, ops  # noqa: E402
+from sdb200.samplers import DDIMSampler  # noqa: E402
+from bench_inpaint import unet_flops  # noqa: E402
+from bench_lsun import gpu_info  # noqa: E402
+
+
+def timed(fn, reps):
+    """Mean milliseconds per call of fn over reps calls, after two warm-up calls (CUDA events)."""
+    for _ in range(2):
+        fn()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(reps):
+        fn()
+    e1.record()
+    e1.synchronize()
+    return e0.elapsed_time(e1) / reps
+
+
+def main():
+    p = argparse.ArgumentParser()
+    p.add_argument("--repeats", type=int, default=2)
+    p.add_argument("--steps", type=int, default=100)
+    p.add_argument("--size", type=int, default=256)
+    p.add_argument("--out", type=str, default=None)
+    a = p.parse_args()
+    import superres as S
+    dev = torch.device("cuda")
+    m = S.load_model(random_init=True)
+    u = m.model.diffusion_model
+    u.use_cuda_graph = True
+    sampler = DDIMSampler(m)
+    g = np.random.default_rng(0)
+    lrs = [torch.from_numpy(g.integers(0, 256, (1, a.size, a.size, 3), dtype=np.uint8)).to(dev)
+           for _ in range(a.repeats + 1)]
+    torch.manual_seed(0)
+    with m.ema_scope():
+        S.superresolve(m, sampler, lrs[0], steps=2)          # warm-up: autotune, graph capture, tables, decoder
+        torch.cuda.synchronize()
+        times, split = [], []
+        for lr in lrs[1:]:
+            ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
+            t0 = time.perf_counter()
+            ev[0].record()
+            x, c, s, path = S.superresolve(m, sampler, lr, steps=a.steps, eta=1.0, return_latents=True)
+            ev[1].record()
+            torch.cuda.synchronize()
+            times.append(time.perf_counter() - t0)
+            ev[1].synchronize()
+            split.append(ev[0].elapsed_time(ev[1]))
+    assert path == "split" and tuple(x.shape) == (1, 3, 4 * a.size, 4 * a.size) and bool(torch.isfinite(x).all())
+
+    plan = m._split_plan((1, 3, a.size, a.size), 1, dev)
+    dplan = m._split_plan((1, 3, a.size, a.size), 4, dev)
+    n, ks = plan["n"], plan["ks"]
+    gt = torch.Generator(device=dev).manual_seed(1)
+    xt = torch.randn(n, 3, *ks, generator=gt, device=dev)
+    ct = torch.randn(n, 3, *ks, generator=gt, device=dev)
+    t = torch.full((n,), 501.0, device=dev)
+    tiled = timed(lambda: u(xt, t, concat=ct), 20)
+    one = [(xt[i:i + 1].contiguous(), t[i:i + 1].contiguous(), ct[i:i + 1].contiguous()) for i in range(n)]
+    nine_calls = timed(lambda: [u(x1, t1, concat=c1) for x1, t1, c1 in one], 10)
+    fl = unet_flops(arch.BSR_SR_UNET, *ks, nb=n)
+    decode = timed(lambda: m.decode_first_stage(s), 3)
+    eps_tiles = u(xt, t, concat=ct)
+    fold_eps = timed(lambda: ops.patch_fold(eps_tiles, plan["weight"], plan["norm"], plan["grid"], plan["stride"]), 50)
+    xl = torch.randn(1, 3, a.size, a.size, generator=gt, device=dev)
+    unfold = timed(lambda: ops.patch_unfold(xl, ks, plan["stride"]), 50)
+    kd = dplan["ks"][0] * 4
+    dec_tiles = torch.randn(dplan["n"], kd, kd, 3, generator=gt, device=dev)
+    sd = (dplan["stride"][0] * 4, dplan["stride"][1] * 4)
+    fold_dec = timed(lambda: ops.patch_fold(dec_tiles, dplan["weight"], dplan["norm"], dplan["grid"], sd, nhwc=True), 20)
+    res = dict(workload=f"bsr_sr LDM, {a.size}x{a.size} -> {4 * a.size}x{4 * a.size}, {plan['grid'][0]}x{plan['grid'][1]} "
+                        f"tiles of {ks[0]}x{ks[1]} at stride {plan['stride'][0]}, DDIM-{a.steps} eta 1, batch 1, LR "
+                        "conversion + tiled sampling + tiled VQ-f4 decode, random weights",
+               images_per_s=1.0 / min(times), run_s=times, run_ms_events=split,
+               unet_tiled_eval_ms_graph=tiled, unet_tiled_tflop=fl / 1e12, unet_tiled_tflops=fl / (tiled * 1e-3) / 1e12,
+               unet_nine_single_tile_calls_ms_graph=nine_calls, tiled_decode_ms=decode,
+               stitch_eps_fold_ms=fold_eps, stitch_decode_fold_ms=fold_dec, unfold_xt_ms=unfold,
+               unet_chunk=plan["chunk"], decode_chunk=dplan["chunk"], **gpu_info())
+    line = json.dumps(res)
+    print(line)
+    if a.out:
+        os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
+        with open(a.out, "w") as f:
+            f.write(line + "\n")
+
+
+if __name__ == "__main__":
+    main()

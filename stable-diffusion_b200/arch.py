@@ -89,6 +89,16 @@ VQ_F4_NOATTN = dict(embed_dim=3, n_embed=8192, ddconfig={**VQ_F4["ddconfig"], "a
 TINY_INPAINT_UNET = dict(image_size=16, in_channels=7, out_channels=3, model_channels=64, attention_resolutions=[2, 4],
                          num_res_blocks=1, channel_mult=[1, 2, 3], num_heads=8, resblock_updown=True)
 TINY_VQ_NOATTN = dict(embed_dim=3, n_embed=512, ddconfig={**TINY_VQ["ddconfig"], "attn_type": "none"})
+# the LDM super-resolution model (models/ldm/bsr_sr/config.yaml, notebook_helpers.py): x_t (3 channels) concatenated
+# with the low-resolution image (3, the Identity cond stage's output at the latent size); plain ResBlocks, AttentionBlocks
+# of num_head_channels 32 at ds 8 and in the middle block (20 heads at 640 channels; ds 16 is never reached). Widths
+# 160 / 320 / 640 and skip concats 480 / 960 / 1280: 5, 15 and 30 channels per GroupNorm group. VQ-f4 first stage.
+BSR_SR_UNET = dict(image_size=64, in_channels=6, out_channels=3, model_channels=160, attention_resolutions=[16, 8],
+                   num_res_blocks=2, channel_mult=[1, 2, 2, 4], num_head_channels=32)
+# small members for tests: width 160 (5 channels per group) with d = 32 heads at ds 2; a VQ-f4 (vqf 4) first stage
+TINY_BSR_UNET = dict(image_size=16, in_channels=6, out_channels=3, model_channels=160, attention_resolutions=[2],
+                     num_res_blocks=1, channel_mult=[1, 2], num_head_channels=32)
+TINY_VQ_F4 = dict(embed_dim=3, n_embed=512, ddconfig={**TINY_VQ["ddconfig"], "ch_mult": [1, 1, 2]})
 TINY_VAE = dict(embed_dim=4, ddconfig=dict(double_z=True, z_channels=4, resolution=32, in_channels=3, out_ch=3,
                                            ch=64, ch_mult=[1, 2], num_res_blocks=1, attn_resolutions=[],
                                            dropout=0.0))

@@ -22,6 +22,66 @@ from .util import instantiate_from_config, remap_config
 from .vq import VQModelInterface
 
 
+# ------------------------------------------------------------------ patch tiling (split_input_params, ddpm.py:564-651)
+# cond_stage_keys whose conditioning is an image at the latent size, tiled together with x (ddpm.py:916-927)
+SPLIT_COND_KEYS = ("image", "LR_image", "segmentation", "bbox_img")
+# Upper bounds on the device memory one tile needs, in bytes per pixel of the tile per channel of the widest full-resolution
+# level: the UNet keeps its skips, fp16 hi / lo operands and fp32 outputs at that level alive together; the decoder holds
+# a few fp32 / fp16 copies of its last level. Tiles are batched up to half the free memory.
+_UNET_TILE_BYTES, _DECODER_TILE_BYTES = 256, 48
+
+
+def border_distance(h, w):
+    """delta_border (ddpm.py:571-582): each pixel's normalized distance to the nearest tile border, fp32 [h, w], 0 at
+    the border and 0.5 at the centre. The same fp32 operations as the reference, so the tables match it bit for bit."""
+    ay = (torch.arange(h, dtype=torch.float32) / float(h - 1)).view(h, 1)
+    ax = (torch.arange(w, dtype=torch.float32) / float(w - 1)).view(1, w)
+    return torch.minimum(torch.minimum(ay, ax), torch.minimum(1 - ay, 1 - ax))
+
+
+def split_geometry(h, w, params, uf=1):
+    """Tile geometry of the split path for a latent of h x w: (ks, stride, (ly, lx)). uf == 1 is apply_model's, uf > 1
+    decode_first_stage's, which first shrinks ks and stride to the latent as the reference does. Raises ValueError where
+    the reference has no finite result: a kernel larger than the latent (apply_model), tiles that leave rows or columns
+    uncovered (the reference divides by a zero normalization there), a non-square kernel at uf > 1 (the reference's
+    fold kernel is ks[0] on both sides), and tie_braker with a single row or column of tiles (delta_border of a 1-wide
+    grid divides 0 by 0)."""
+    ks, stride = tuple(int(v) for v in params["ks"]), tuple(int(v) for v in params["stride"])
+    if uf > 1:
+        ks = (min(ks[0], h), min(ks[1], w))
+        if stride[0] > h or stride[1] > w:
+            stride = (min(stride[0], h), min(stride[1], w))
+        if ks[0] != ks[1]:
+            raise ValueError(f"split decode: kernel {ks} is not square, and the reference folds {uf}x-upsampled tiles "
+                             "with a square kernel of ks[0]")
+    elif ks[0] > h or ks[1] > w:
+        raise ValueError(f"split apply_model: kernel {ks} is larger than the {h}x{w} latent")
+    if (h - ks[0]) % stride[0] or (w - ks[1]) % stride[1]:
+        raise ValueError(f"split path: tiles of {ks} at stride {stride} do not cover the {h}x{w} latent "
+                         "((side - ks) % stride must be 0)")
+    grid = ((h - ks[0]) // stride[0] + 1, (w - ks[1]) // stride[1] + 1)
+    if params.get("tie_braker") and min(grid) == 1:
+        raise ValueError(f"split path: tie_braker needs at least two rows and columns of tiles, got {grid}")
+    return ks, stride, grid
+
+
+def split_tables(ks, stride, grid, params, uf=1):
+    """get_weighting / fold(weighting) (ddpm.py:584-624) on the CPU in fp32: the per-tile weights [ly*lx, kh, kw] and
+    the normalization [(ly - 1)*sy + kh, (lx - 1)*sx + kw], at tile size (kh, kw) = ks*uf and stride (sy, sx) =
+    stride*uf."""
+    kh, kw = ks[0] * uf, ks[1] * uf
+    L = grid[0] * grid[1]
+    wt = torch.clip(border_distance(kh, kw), params["clip_min_weight"], params["clip_max_weight"])
+    weight = wt.view(1, kh * kw, 1).repeat(1, 1, L)
+    if params.get("tie_braker"):
+        lw = torch.clip(border_distance(*grid), params["clip_min_tie_weight"], params["clip_max_tie_weight"])
+        weight = weight * lw.view(1, 1, L)
+    sy, sx = stride[0] * uf, stride[1] * uf
+    size = ((grid[0] - 1) * sy + kh, (grid[1] - 1) * sx + kw)
+    norm = torch.nn.functional.fold(weight, size, kernel_size=(kh, kw), stride=(sy, sx)).view(*size)
+    return weight[0].t().contiguous().view(L, kh, kw), norm
+
+
 class DiffusionWrapper(nn.Module):
     def __init__(self, diff_model_config, conditioning_key):
         super().__init__()
@@ -160,10 +220,103 @@ class LatentDiffusion(nn.Module):
             if not isinstance(cond, list):
                 cond = [cond]
             cond = {"c_concat" if self.model.conditioning_key == "concat" else "c_crossattn": cond}
+        if getattr(self, "split_input_params", None) is not None:
+            assert not return_ids
+            return self._apply_split(x_noisy, t, cond)
         x_recon = self.model(x_noisy, t, **cond)
         if isinstance(x_recon, tuple) and not return_ids:
             return x_recon[0]
         return x_recon
+
+    def _split_plan(self, shape, uf, device):
+        """Geometry, weight / normalization tables (on the device) and tile-batch size of the split path for a latent of
+        `shape`, computed once per geometry. The batch of tiles is cut into equal chunks when it would not fit in half
+        the free device memory (a bound from memory, fixed per geometry so every step replays one captured graph)."""
+        p = self.split_input_params
+        key = (tuple(shape), uf, str(device), tuple(sorted((k, str(v)) for k, v in p.items())))
+        cache = self.__dict__.setdefault("_split_cache", {})
+        if key not in cache:
+            nb, _, h, w = shape
+            ks, stride, grid = split_geometry(h, w, p, uf)
+            weight, norm = split_tables(ks, stride, grid, p, uf)
+            n = grid[0] * grid[1] * nb
+            if uf == 1:
+                per_tile = ks[0] * ks[1] * self.model.diffusion_model.model_channels * _UNET_TILE_BYTES
+            else:
+                dd = self.first_stage_model.cfg["ddconfig"]
+                per_tile = ks[0] * ks[1] * uf * uf * dd["ch"] * dd["ch_mult"][0] * _DECODER_TILE_BYTES
+            cap = max(1, int(torch.cuda.mem_get_info(device)[0] // 2 // per_tile))
+            chunks = -(-n // cap)
+            cache[key] = dict(ks=ks, stride=stride, grid=grid, n=n, chunk=-(-n // chunks), chunks=chunks,
+                              weight=weight.to(device), norm=norm.to(device))
+        return cache[key]
+
+    def _apply_split(self, x, t, cond):
+        """The split apply_model (ddpm.py:891-992, concat conditioning or none): every tile of every sample in one UNet
+        batch (tile l*nb + n; GroupNorm and attention are per sample, so this is the reference's per-tile loop), stitched
+        by sdb_patch_fold. The conditioning tiles are gathered once per conditioning tensor, not per step."""
+        if len(cond) != 1:
+            raise NotImplementedError("split apply_model takes one conditioning")
+        key = self.model.conditioning_key
+        c = None
+        if key is not None:
+            if key != "concat" or self.cond_stage_key not in SPLIT_COND_KEYS:
+                raise NotImplementedError(f"split apply_model with {key!r} conditioning and cond_stage_key "
+                                          f"{self.cond_stage_key!r}: supported are concat conditioning on {SPLIT_COND_KEYS}")
+            cl = cond["c_concat"]
+            c = cl[0] if len(cl) == 1 else torch.cat(cl, 1)
+        x = x.contiguous().float()
+        plan = self._split_plan(x.shape, 1, x.device)
+        ks, stride, n, chunk, chunks = plan["ks"], plan["stride"], plan["n"], plan["chunk"], plan["chunks"]
+        unet = self.model.diffusion_model
+        ct = None if c is None else self._cond_tiles(c, plan, chunk * chunks)
+        ts = t.reshape(-1).repeat(n // x.shape[0])
+        if chunks == 1:
+            # graph mode: x_t's tiles go straight into the captured graph's static input
+            bufs = unet.graph_inputs((n, x.shape[1], *ks), None if ct is None else tuple(ct.shape))
+            xt = ops.patch_unfold(x, ks, stride, out=None if bufs is None else bufs[0])
+        else:
+            xt = torch.zeros((chunk * chunks, x.shape[1], *ks), dtype=torch.float32, device=x.device)
+            ops.patch_unfold(x, ks, stride, out=xt[:n])
+            ts = torch.cat([ts, ts[:1].expand(chunk * chunks - n)])
+        eps = []
+        for i in range(chunks):
+            s = slice(i * chunk, (i + 1) * chunk)
+            eps.append(self.model(xt[s], ts[s]) if ct is None else self.model(xt[s], ts[s], c_concat=[ct[s]]))
+        eps = eps[0] if chunks == 1 else torch.cat(eps)[:n]
+        return ops.patch_fold(eps.contiguous().float(), plan["weight"], plan["norm"], plan["grid"], stride)
+
+    def _cond_tiles(self, c, plan, rows):
+        """The conditioning's tiles ([rows, c, kh, kw], zero rows after the last tile), cached for the tensor they came
+        from: the conditioning is constant over a sampling run."""
+        key = (c.data_ptr(), c._version, tuple(c.shape), plan["ks"], plan["stride"], rows)
+        hit = self.__dict__.get("_split_cond")
+        if hit is None or hit[0] != key:
+            ct = torch.zeros((rows, c.shape[1], *plan["ks"]), dtype=torch.float32, device=c.device)
+            ops.patch_unfold(c.contiguous().float(), plan["ks"], plan["stride"], out=ct[:plan["n"]])
+            hit = (key, ct, c)        # c is kept alive, so its address is not reused by another tensor
+            self._split_cond = hit
+        return hit[1]
+
+    def _decode_split(self, z, force_not_quantize):
+        """The split decode_first_stage (ddpm.py:705-763): quantize and post_quant_conv once on the whole latent (both
+        act per pixel, so this equals the reference's per-tile quantize), cut tiles, decode them in memory-bounded equal
+        chunks, and stitch the vqf-times larger tiles with sdb_patch_fold straight from the decoder's NHWC output."""
+        fs = self.first_stage_model
+        uf = int(self.split_input_params["vqf"])
+        z = z.contiguous().float()
+        plan = self._split_plan(z.shape, uf, z.device)
+        scale = 1. / float(self.scale_factor)
+        if isinstance(fs, VQModelInterface):
+            q = fs.post_quant(z, force_not_quantize=force_not_quantize, scale=scale)
+        else:
+            q = fs.post_quant(z, scale=scale)
+        qt, _ = ops.nchw_to_nhwc(ops.patch_unfold(ops.nhwc_to_nchw(q), plan["ks"], plan["stride"]))
+        chunk = plan["chunk"]
+        outs = [fs._decoder(qt[i:i + chunk]) for i in range(0, plan["n"], chunk)]
+        o = outs[0] if len(outs) == 1 else torch.cat(outs)
+        stride = (plan["stride"][0] * uf, plan["stride"][1] * uf)
+        return ops.patch_fold(o, plan["weight"], plan["norm"], plan["grid"], stride, nhwc=True)
 
     def set_context(self, c):
         """Fast path used by sdb200 samplers: cross-attention K/V of the (guidance-doubled) context, once per batch. A
@@ -195,6 +348,9 @@ class LatentDiffusion(nn.Module):
     def decode_first_stage(self, z, predict_cids=False, force_not_quantize=False):
         if predict_cids:
             raise NotImplementedError("decode_first_stage(predict_cids=True): codebook-index latents are not supported")
+        sp = getattr(self, "split_input_params", None)
+        if sp is not None and sp["patch_distributed_vq"]:
+            return self._decode_split(z, force_not_quantize)
         if isinstance(self.first_stage_model, VQModelInterface):     # ddpm.py:753-761: quantize, then decode
             return self.first_stage_model.decode(z, force_not_quantize=force_not_quantize,
                                                  scale=1. / float(self.scale_factor))

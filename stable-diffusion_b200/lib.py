@@ -112,6 +112,9 @@ SIGNATURES = {
     "sdb_axpby2": ([_P, _P, _F, _F, _L, _P, _P], C.c_int),
     "sdb_inpaint_prepare": ([_P, _P, _I, _I, _I, _P, _P, _I, _I, _I, _I, _P], C.c_int),
     "sdb_inpaint_composite": ([_P, _P, _P, _L, _P, _P], C.c_int),
+    "sdb_lr_prepare": ([_P, _I, _I, _I, _P, _P], C.c_int),
+    "sdb_patch_unfold": ([_P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P], C.c_int),
+    "sdb_patch_fold": ([_P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _I, _I, _P, _P], C.c_int),
     # post-processing (safety.cu)
     "sdb_resample_u8": ([_P, _P, _I, _I, _I, _I, _I, _P, _P, _I, _I, _P, _P], C.c_int),
     "sdb_clip_normalize": ([_P, _I, _I, _I, _I, _F, _F, _F, _F, _F, _F, _P, _P], C.c_int),

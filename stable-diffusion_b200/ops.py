@@ -547,6 +547,53 @@ def inpaint_composite(x_nhwc, image_u8, mask_u8):
     return out
 
 
+def lr_prepare(image_u8):
+    """Low-resolution image uint8 RGB [nb, h, w, 3] -> the super-resolution conditioning 2 * (u / 255) - 1, fp32 NCHW
+    [nb, 3, h, w] (sdb_lr_prepare)."""
+    assert image_u8.dtype == torch.uint8 and image_u8.is_cuda and image_u8.is_contiguous()
+    assert image_u8.dim() == 4 and image_u8.shape[3] == 3, tuple(image_u8.shape)
+    nb, h, w, _ = image_u8.shape
+    out = torch.empty((nb, 3, h, w), dtype=torch.float32, device=image_u8.device)
+    _l.check(_l.load().sdb_lr_prepare(_ptr(image_u8), nb, h, w, _ptr(out), _stream()), "sdb_lr_prepare")
+    _count()
+    return out
+
+
+def patch_unfold(x, ks, stride, out=None):
+    """nn.Unfold(ks, stride=stride) of x fp32 NCHW [nb, c, h, w] as tiles [L*nb, c, ks[0], ks[1]], tile l*nb + n
+    (sdb_patch_unfold). `out` may be a preallocated contiguous buffer of that shape (a captured graph's input)."""
+    _chk32(x, "x")
+    nb, c, h, w = x.shape
+    L = ((h - ks[0]) // stride[0] + 1) * ((w - ks[1]) // stride[1] + 1)
+    shape = (L * nb, c, ks[0], ks[1])
+    if out is None:
+        out = torch.empty(shape, dtype=torch.float32, device=x.device)
+    _chk32(out, "out")
+    assert tuple(out.shape) == shape, (tuple(out.shape), shape)
+    _l.check(_l.load().sdb_patch_unfold(_ptr(x), nb, c, h, w, ks[0], ks[1], stride[0], stride[1], _ptr(out), _stream()),
+             "sdb_patch_unfold")
+    _count()
+    return out
+
+
+def patch_fold(tiles, weight, norm, grid, stride, nhwc=False):
+    """fold(tiles * weight) / norm -> fp32 NCHW [nb, c, h, w] (sdb_patch_fold). tiles fp32 [ly*lx*nb, c, kh, kw] (or
+    [.., kh, kw, c] with nhwc), weight fp32 [ly*lx, kh, kw], norm fp32 [h, w]; grid = (ly, lx)."""
+    _chk32(tiles, "tiles")
+    _chk32(weight, "weight")
+    _chk32(norm, "norm")
+    ly, lx = grid
+    n, c, kh, kw = (tiles.shape[0], tiles.shape[3], tiles.shape[1], tiles.shape[2]) if nhwc else tiles.shape
+    assert n % (ly * lx) == 0 and tuple(weight.shape) == (ly * lx, kh, kw), (tuple(tiles.shape), tuple(weight.shape))
+    nb = n // (ly * lx)
+    h, w = norm.shape
+    out = torch.empty((nb, c, h, w), dtype=torch.float32, device=tiles.device)
+    _l.check(_l.load().sdb_patch_fold(_ptr(tiles), int(nhwc), nb, c, kh, kw, ly, lx, stride[0], stride[1], _ptr(weight),
+                                      _ptr(norm), h, w, _ptr(out), _stream()), "sdb_patch_fold")
+    _count()
+    return out
+
+
 def upsample2x(x):
     _chk32(x, "x")
     nb, h, w, c = x.shape

@@ -721,6 +721,15 @@ class UNetModel(nn.Module):
         eps = self._forward_impl(x.contiguous().float(), t, kvs)
         return eps.to(x.dtype)
 
+    def graph_inputs(self, shape, concat_shape=None):
+        """Graph mode, no spatial transformer: the static x and conditioning buffers (the latter None without concat) of
+        the graph captured for these shapes, capturing it first. A caller that writes its next input straight into them
+        skips forward()'s copy. None in eager mode."""
+        if not self.use_cuda_graph or self.conditional:
+            return None
+        g = self._graph_for(tuple(shape), None, None if concat_shape is None else tuple(concat_shape))
+        return g["x"], g["c"]
+
     def _forward_uncond(self, x, timesteps, concat=None):
         if self.use_cuda_graph:
             g = self._graph_for(tuple(x.shape), None, None if concat is None else tuple(concat.shape))

@@ -272,11 +272,16 @@ class AutoencoderKL(ConvAutoencoder):
     def decode(self, z, scale=1.0, nhwc=False):
         """AutoencoderKL.decode (autoencoder.py:330-333) on z*scale; NCHW fp32 in / out (nhwc=True keeps the
         kernels' native NHWC output, which is what the image writer wants: txt2img.py:322)."""
+        out = self._decoder(self.post_quant(z, scale=scale))
+        return out if nhwc else ops.nhwc_to_nchw(out)
+
+    @torch.no_grad()
+    def post_quant(self, z, scale=1.0):
+        """The per-pixel head of decode: post_quant_conv of z*scale; NCHW fp32 in, the decoder's NHWC fp32 input out."""
         assert self.W is not None and z.is_cuda, "sdb200.AutoencoderKL runs on CUDA only (no CPU fallback)"
         W = self.W
         zh, _ = ops.nchw_to_nhwc(z.contiguous().float())
-        out = self._decoder(ops.pointwise_small(zh, W["pq_w"], W["pq_b"], alpha=float(scale)))
-        return out if nhwc else ops.nhwc_to_nchw(out)
+        return ops.pointwise_small(zh, W["pq_w"], W["pq_b"], alpha=float(scale))
 
     @torch.no_grad()
     def encode(self, x):

@@ -64,12 +64,16 @@ class VQModelInterface(ConvAutoencoder):
     def decode(self, h, force_not_quantize=False, scale=1.0, nhwc=False):
         """VQModelInterface.decode on h*scale (scale: decode_first_stage's 1 / scale_factor): quantize unless
         force_not_quantize, post_quant_conv, decoder. NCHW fp32 in / out (nhwc=True keeps the NHWC output)."""
+        out = self._decoder(self.post_quant(h, force_not_quantize, scale))
+        return out if nhwc else ops.nhwc_to_nchw(out)
+
+    @torch.no_grad()
+    def post_quant(self, h, force_not_quantize=False, scale=1.0):
+        """The per-pixel head of decode: quantize h*scale (unless force_not_quantize), then post_quant_conv; NCHW fp32
+        in, the decoder's NHWC fp32 input out."""
         assert self.W is not None and h.is_cuda, "sdb200.VQModelInterface runs on CUDA only (no CPU fallback)"
         W = self.W
         zh, _ = ops.nchw_to_nhwc(h.contiguous().float())
         if force_not_quantize:
-            q = ops.pointwise_small(zh, W["pq_w"], W["pq_b"], alpha=float(scale))
-        else:
-            q = ops.pointwise_small(self._quantize_nhwc(zh, scale), W["pq_w"], W["pq_b"])
-        out = self._decoder(q)
-        return out if nhwc else ops.nhwc_to_nchw(out)
+            return ops.pointwise_small(zh, W["pq_w"], W["pq_b"], alpha=float(scale))
+        return ops.pointwise_small(self._quantize_nhwc(zh, scale), W["pq_w"], W["pq_b"])
