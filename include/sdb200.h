@@ -36,7 +36,9 @@ enum {
   SDB_ACT_GEGLU = 1,      /* out[:, j] = x_j * gelu_erf(gate_j); ldm/modules/attention.py:37-45 (weights packed
                              so each accumulator tile holds [x half | gate half]) */
   SDB_ACT_QUICK_GELU = 2, /* x * sigmoid(1.702 x): CLIP MLP (transformers CLIPMLP, quick_gelu) */
-  SDB_ACT_SILU = 3        /* x * sigmoid(x): time_embed MLP, openaimodel.py:506-511 */
+  SDB_ACT_SILU = 3,       /* x * sigmoid(x): time_embed MLP, openaimodel.py:506-511 */
+  SDB_ACT_GELU = 4        /* gelu_erf(x) = 0.5 x (1 + erf(x / sqrt 2)), exact nn.GELU: the BERTEmbedder feed-forward
+                             (x_transformer.py:199-202); any other value is rejected by sdb_gemm */
 };
 
 /*

@@ -8,6 +8,11 @@ files the prompt is replaced by seeded token ids (--token_seed). Post-processing
 (txt2img.py:317-327), on the GPU: the invisible watermark ("StableDiffusionV1", dwtDct) is always embedded unless
 --no_watermark; the safety checker runs when its weights are supplied (--safety_ckpt: a diffusers
 StableDiffusionSafetyChecker state dict, .safetensors or tensors-only pickle) - no weights ship offline.
+
+--laion400m switches to the LAION-400M model as the reference does (configs/latent-diffusion/txt2img-1p4B-eval.yaml,
+models/ldm/text2img-large/model.ckpt, outputs/txt2img-samples-laion400m): BERT-conditioned UNet, same KL-f8 first stage.
+Its prompts are tokenised with the uncased WordPiece vocabulary of --bert_vocab (or the locally cached bert-base-uncased
+files); without one, seeded stand-in ids [CLS] r... [SEP] [PAD]... are used and the empty prompt is [CLS] [SEP] [PAD]...
 """
 import argparse
 import os
@@ -23,24 +28,40 @@ from sdb200 import pipeline  # noqa: E402
 from sdb200.safety import StableDiffusionSafetyChecker, WatermarkEncoder, put_watermark  # noqa: E402
 
 DEFAULT_CONFIG = "configs/stable-diffusion/v1-inference.yaml"
+LAION_CONFIG = "configs/latent-diffusion/txt2img-1p4B-eval.yaml"
+LAION_CKPT = "models/ldm/text2img-large/model.ckpt"
+LAION_OUTDIR = "outputs/txt2img-samples-laion400m"
+BERT_CLS, BERT_SEP, BERT_PAD = 101, 102, 0          # bert-base-uncased [CLS] / [SEP] / [PAD]
+
+
+def apply_laion400m(opt):
+    """txt2img.py:237-241: --laion400m replaces config, checkpoint and output directory."""
+    if opt.laion400m:
+        print("Falling back to LAION 400M model...")
+        opt.config = LAION_CONFIG
+        opt.ckpt = LAION_CKPT
+        opt.outdir = LAION_OUTDIR
+    return opt
 
 
 def load_model_from_config(config, ckpt, device, verbose=False, random_init=False, unsafe_ckpt=False):
-    """scripts/txt2img.py:49-66 via sdb200.checkpoint (pickled .ckpt or .safetensors, reference YAML or built-in v1).
-    Seeded random weights are used only on request (--random_init): a missing checkpoint or config path is an error."""
+    """scripts/txt2img.py:49-66 via sdb200.checkpoint (pickled .ckpt or .safetensors, reference YAML or built-in values
+    of v1-inference.yaml / txt2img-1p4B-eval.yaml when the reference's default path of either is absent). Seeded random
+    weights are used only on request (--random_init): a missing checkpoint or config path is an error."""
+    laion = config == LAION_CONFIG
     if config and not os.path.exists(config):
-        if config != DEFAULT_CONFIG:
+        if config not in (DEFAULT_CONFIG, LAION_CONFIG):
             raise FileNotFoundError(f"--config {config} does not exist")
-        config = None                         # the reference's default path is absent here: built-in v1-inference values
+        config = None                         # the reference's default path is absent here: built-in values
     if random_init:
         print("--random_init: seeded random-init weights (images will be noise-like)")
-        model = pipeline.build_model()
+        model = pipeline.build_laion_model() if laion else pipeline.build_model()
         pipeline.load_random_weights(model, device, gen_device=device)
         return model.eval()
     if not ckpt or not os.path.exists(ckpt):
         raise FileNotFoundError(f"checkpoint {ckpt!r} does not exist (pass --ckpt, or --random_init for seeded random "
                                 "weights)")
-    cfg = config if config else {"model": pipeline.v1_model_config()}
+    cfg = config if config else {"model": pipeline.laion_model_config() if laion else pipeline.v1_model_config()}
     return sdb200.checkpoint.load_model_from_config(cfg, ckpt, device=device, verbose=verbose, allow_pickle=unsafe_ckpt)
 
 
@@ -49,6 +70,23 @@ def synthetic_ids(n, seed, device):
     ids = torch.randint(0, 49406, (n, 77), generator=g)
     ids[:, 0] = 49406
     ids[:, 20:] = 49407
+    return ids.to(device)
+
+
+def synthetic_bert_ids(n, seed, device):
+    """Stand-in bert-base-uncased ids: [CLS], 19 seeded word-piece ids (999 .. 30521), [SEP], [PAD]..."""
+    g = torch.Generator().manual_seed(seed)
+    ids = torch.full((n, 77), BERT_PAD, dtype=torch.long)
+    ids[:, 0] = BERT_CLS
+    ids[:, 1:20] = torch.randint(999, 30522, (n, 19), generator=g)
+    ids[:, 20] = BERT_SEP
+    return ids.to(device)
+
+
+def bert_uncond_ids(n, device):
+    """The empty prompt as bert-base-uncased tokenises it: [CLS] [SEP] [PAD]..."""
+    ids = torch.full((n, 77), BERT_PAD, dtype=torch.long)
+    ids[:, 0], ids[:, 1] = BERT_CLS, BERT_SEP
     return ids.to(device)
 
 
@@ -81,13 +119,13 @@ def main():
     p.add_argument("--precision", type=str, choices=["full", "autocast"], default="autocast")
     p.add_argument("--clip_vocab", type=str, default=None,
                    help="directory with the CLIP vocab.json + merges.txt (host-side BPE); default: transformers' local cache")
+    p.add_argument("--bert_vocab", type=str, default=None,
+                   help="directory with the bert-base-uncased vocab.txt (--laion400m); default: the local Hugging Face cache")
     p.add_argument("--token_seed", type=int, default=1234, help="seed of the stand-in token ids (no tokenizer offline)")
     p.add_argument("--safety_ckpt", type=str, default=None,
                    help="state dict of diffusers' StableDiffusionSafetyChecker: flagged images are blanked (txt2img.py:88-95)")
     p.add_argument("--no_watermark", action="store_true", help="do not embed the invisible watermark (txt2img.py:261-264)")
-    opt = p.parse_args()
-    if opt.laion400m:
-        raise NotImplementedError("--laion400m (a different checkpoint/config) is outside the SD-v1 path of this engine")
+    opt = apply_laion400m(p.parse_args())
     torch.manual_seed(opt.seed)           # seed_everything (txt2img.py:243)
     device = torch.device("cuda")
     model = load_model_from_config(opt.config, opt.ckpt, device, random_init=opt.random_init, unsafe_ckpt=opt.unsafe_ckpt)
@@ -115,8 +153,10 @@ def main():
     else:
         prompts = [opt.prompt]
     enc = model.cond_stage_model
-    if opt.clip_vocab:
+    if opt.clip_vocab and not opt.laion400m:
         enc.version, enc.tokenizer = opt.clip_vocab, None
+    if opt.bert_vocab and opt.laion400m:
+        enc.vocab_dir, enc.tokenizer = opt.bert_vocab, None
     start_code = torch.randn([B, opt.C, opt.H // opt.f, opt.W // opt.f], device=device) if opt.fixed_code else None
     base_count = len(os.listdir(sample_path))
     tic = time.time()
@@ -129,9 +169,12 @@ def main():
             except RuntimeError as e:
                 if n == 0 and pi == 0:
                     print(f"tokenizer unavailable ({e}); using seeded token ids")
-                ids = synthetic_ids(B, opt.token_seed + pi, device)
-                un = torch.full((B, 77), 49407, dtype=torch.long, device=device)
-                un[:, 0] = 49406
+                if opt.laion400m:
+                    ids, un = synthetic_bert_ids(B, opt.token_seed + pi, device), bert_uncond_ids(B, device)
+                else:
+                    ids = synthetic_ids(B, opt.token_seed + pi, device)
+                    un = torch.full((B, 77), 49407, dtype=torch.long, device=device)
+                    un[:, 0] = 49406
             x_T = start_code if start_code is not None else torch.randn(
                 [B, opt.C, opt.H // opt.f, opt.W // opt.f], device=device)      # plms.py:124
             if safety_checker is not None:       # check_safety on the fp32 image, then 255 * x -> uint8 (txt2img.py:317-322)

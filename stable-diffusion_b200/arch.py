@@ -104,6 +104,13 @@ TINY_VAE = dict(embed_dim=4, ddconfig=dict(double_z=True, z_channels=4, resoluti
                                            dropout=0.0))
 TINY_CLIP = dict(vocab_size=1000, hidden_size=128, intermediate_size=512, num_hidden_layers=2,
                  num_attention_heads=2, max_position_embeddings=77, layer_norm_eps=1e-5)
+# the LAION-400M text-to-image LDM (configs/latent-diffusion/txt2img-1p4B-eval.yaml): SD-v1's UNet with a 1280-wide
+# context, cond stage BERTEmbedder(n_embed=1280, n_layer=32) (x_transformer Encoder: 8 heads of 64 whatever the width)
+LAION_UNET = dict(SD_V1_UNET, context_dim=1280)
+LAION_BERT = dict(n_embed=1280, n_layer=32, vocab_size=30522, max_seq_len=77)
+# small members for tests: the attention's inner width stays 8 x 64 = 512
+TINY_BERT = dict(n_embed=128, n_layer=2, vocab_size=1000, max_seq_len=77)
+TINY_LAION_UNET = dict(TINY_UNET, context_dim=128)
 
 
 # ------------------------------------------------------------------------------------------------ UNet
@@ -410,6 +417,34 @@ def clip_param_shapes(cfg):
     return p
 
 
+def bert_param_shapes(cfg):
+    """Keys as the reference BERTEmbedder.state_dict() (`transformer.*`, x_transformer.TransformerWrapper around an
+    Encoder of `n_layer` ('a', 'f') pairs), to_logits included; under `cond_stage_model.` in an LDM checkpoint."""
+    d, v, inner = cfg["n_embed"], cfg["vocab_size"], 8 * 64
+    p = OrderedDict()
+    p["transformer.token_emb.weight"] = (v, d)
+    p["transformer.pos_emb.emb.weight"] = (cfg["max_seq_len"], d)
+    for j in range(2 * cfg["n_layer"]):
+        pre = f"transformer.attn_layers.layers.{j}"
+        p[f"{pre}.0.weight"] = (d,)
+        p[f"{pre}.0.bias"] = (d,)
+        if j % 2 == 0:
+            for n in ("to_q", "to_k", "to_v"):
+                p[f"{pre}.1.{n}.weight"] = (inner, d)
+            p[f"{pre}.1.to_out.weight"] = (d, inner)
+            p[f"{pre}.1.to_out.bias"] = (d,)
+        else:
+            p[f"{pre}.1.net.0.0.weight"] = (4 * d, d)
+            p[f"{pre}.1.net.0.0.bias"] = (4 * d,)
+            p[f"{pre}.1.net.2.weight"] = (d, 4 * d)
+            p[f"{pre}.1.net.2.bias"] = (d,)
+    p["transformer.norm.weight"] = (d,)
+    p["transformer.norm.bias"] = (d,)
+    p["transformer.to_logits.weight"] = (v, d)
+    p["transformer.to_logits.bias"] = (v,)
+    return p
+
+
 def safety_param_shapes(cfg):
     """Keys as diffusers StableDiffusionSafetyChecker.state_dict(): the CLIPVisionModel sits under `vision_model.`."""
     h, inter, pd = cfg["hidden_size"], cfg["intermediate_size"], cfg["projection_dim"]
@@ -452,6 +487,9 @@ def _is_norm_key(k):
     leaf = parts[-2]
     if leaf.startswith("norm") or leaf.startswith("layer_norm") or leaf in ("final_layer_norm", "norm_out", "pre_layrnorm",
                                                                              "post_layernorm"):
+        return True
+    # BERTEmbedder LayerNorms: transformer.attn_layers.layers.{j}.0
+    if len(parts) == 6 and parts[:3] == ["transformer", "attn_layers", "layers"] and parts[4] == "0":
         return True
     # UNet GroupNorms live at in_layers.0 / out_layers.0 / out.0
     return (len(parts) >= 3 and parts[-3] in ("in_layers", "out_layers") and leaf == "0") or k.startswith("out.0.")

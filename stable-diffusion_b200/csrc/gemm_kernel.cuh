@@ -117,6 +117,7 @@ __device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + __ex
 __device__ __forceinline__ float apply_act(float x, int act) {
   if (act == SDB_ACT_QUICK_GELU) return x * sigmoidf_(1.702f * x);
   if (act == SDB_ACT_SILU) return x * sigmoidf_(x);
+  if (act == SDB_ACT_GELU) return gelu_erf(x);
   return x;
 }
 

@@ -101,6 +101,7 @@ static double choice_cost(const sdb_gemm_desc* d, const Geometry& g, const Choic
 }
 
 static int make_geometry(const sdb_gemm_desc* d, Geometry* g) {
+  SDB_CHECK(d->act >= SDB_ACT_NONE && d->act <= SDB_ACT_GELU, "sdb_gemm: unknown activation %d", d->act);
   const void* srcs[MAX_SRC] = {d->a0, d->a1, d->a2, d->a3};
   const int chans[MAX_SRC] = {d->c0, d->c1, d->c2, d->c3};
   int nsrc = 0, chunks = 0;

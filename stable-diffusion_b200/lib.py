@@ -10,7 +10,7 @@ from pathlib import Path
 
 _LIB_PATH = Path(__file__).resolve().parent / "csrc" / "libsdb200.so"
 
-ACT_NONE, ACT_GEGLU, ACT_QUICK_GELU, ACT_SILU = 0, 1, 2, 3
+ACT_NONE, ACT_GEGLU, ACT_QUICK_GELU, ACT_SILU, ACT_GELU = 0, 1, 2, 3, 4
 
 
 class GemmDesc(C.Structure):

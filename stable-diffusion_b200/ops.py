@@ -11,7 +11,7 @@ import ctypes as C
 import torch
 
 from . import lib as _l
-from .lib import ACT_GEGLU, ACT_NONE, ACT_QUICK_GELU, ACT_SILU, AttnDesc, GemmDesc  # noqa: F401
+from .lib import ACT_GEGLU, ACT_GELU, ACT_NONE, ACT_QUICK_GELU, ACT_SILU, AttnDesc, GemmDesc  # noqa: F401
 
 LAUNCHES = 0        # op calls made through this module
 _GRAPH_LAUNCHES = 0  # kernels replayed from CUDA graphs (counted at capture time, added per replay)

@@ -36,6 +36,31 @@ def build_model(unet_cfg=None, vae_cfg=None, clip_cfg=None):
         unet_config={"target": "sdb200.unet.UNetModel", "params": dict(unet_cfg or arch.SD_V1_UNET)}, **V1_PARAMS)
 
 
+# configs/latent-diffusion/txt2img-1p4B-eval.yaml: the LAION-400M model (scripts/txt2img.py --laion400m)
+LAION_PARAMS = dict(V1_PARAMS, first_stage_key="image", cond_stage_key="caption", image_size=32,
+                    cond_stage_trainable=True)
+
+
+def laion_model_config(unet_cfg=None, vae_cfg=None, bert_cfg=None):
+    """The `model:` node of configs/latent-diffusion/txt2img-1p4B-eval.yaml as a dict, with the reference's target
+    names (used when that YAML is not at hand)."""
+    bert = dict(bert_cfg or arch.LAION_BERT)
+    return {"target": "ldm.models.diffusion.ddpm.LatentDiffusion", "params": dict(
+        LAION_PARAMS,
+        unet_config={"target": "ldm.modules.diffusionmodules.openaimodel.UNetModel",
+                     "params": dict(unet_cfg or arch.LAION_UNET)},
+        first_stage_config={"target": "ldm.models.autoencoder.AutoencoderKL", "params": dict(vae_cfg or arch.SD_V1_VAE)},
+        cond_stage_config={"target": "ldm.modules.encoders.modules.BERTEmbedder", "params": bert})}
+
+
+def build_laion_model(unet_cfg=None, vae_cfg=None, bert_cfg=None):
+    """LatentDiffusion with the txt2img-1p4B-eval.yaml parameters: UNet (context 1280), KL-f8, BERTEmbedder."""
+    return LatentDiffusion(
+        first_stage_config={"target": "sdb200.vae.AutoencoderKL", "params": dict(vae_cfg or arch.SD_V1_VAE)},
+        cond_stage_config={"target": "sdb200.bert.BERTEmbedder", "params": dict(bert_cfg or arch.LAION_BERT)},
+        unet_config={"target": "sdb200.unet.UNetModel", "params": dict(unet_cfg or arch.LAION_UNET)}, **LAION_PARAMS)
+
+
 def load_random_weights(model, device, seeds=(11, 12, 13), gen_device=None):
     """Seeded synthetic weights for all three stages (no checkpoint offline). gen_device='cuda' draws on the GPU."""
     gd = gen_device or "cpu"
@@ -49,7 +74,7 @@ def load_random_weights(model, device, seeds=(11, 12, 13), gen_device=None):
 
 
 class Txt2Img:
-    """scripts/txt2img.py main loop for one batch: uc/c = CLIP(ids) -> sampler.sample -> decode_first_stage ->
+    """scripts/txt2img.py main loop for one batch: uc/c = cond stage (CLIP or BERT) of ids -> sampler.sample -> decode_first_stage ->
     clamp((x+1)/2, 0, 1) -> 255*x uint8 (HWC)."""
 
     def __init__(self, model, sampler="plms", steps=50, scale=7.5, height=512, width=512, eta=0.0, f=8, channels=4,

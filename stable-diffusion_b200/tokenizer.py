@@ -182,3 +182,138 @@ class CLIPBPETokenizer:
             ids = [self.bos_id] + self.tokenize_ids(t)[: n - 2] + [self.eos_id]
             out.append(ids + [self.eos_id] * (n - len(ids)))
         return out
+
+
+# ------------------------------------------------------------------------------------------------ BERT WordPiece
+# `BERTTokenizer` of the LAION-400M model (ldm/modules/encoders/modules.py:53-67) is transformers' BertTokenizerFast
+# ("bert-base-uncased") with truncation to 77 and max_length padding. The restatement below follows the published
+# uncased BERT pipeline from a vocab.txt alone:
+#   raw text split on the literal special tokens -> drop NUL / U+FFFD / control characters, whitespace to " " -> spaces
+#   around CJK ideographs -> NFD and drop non-spacing marks -> lowercase -> split on whitespace, every punctuation
+#   character a token of its own -> greedy longest-match WordPiece ("##" continuation, [UNK] for a word that does not
+#   decompose or is longer than 100 characters) -> [CLS] + 75 tokens max + [SEP], padded with [PAD].
+# It is pinned against the installed transformers.BertTokenizerFast on a synthetic vocabulary (tests/test_laion_cpu.py).
+BERT_SPECIAL = ("[CLS]", "[SEP]", "[PAD]", "[UNK]", "[MASK]")
+
+
+def _bert_is_white(ch):
+    return ch in "\t\n\r" or ch in _WHITE
+
+
+def _bert_is_control(ch):
+    return ch not in "\t\n\r" and unicodedata.category(ch)[0] == "C"
+
+
+def _bert_is_punct(ch):
+    o = ord(ch)
+    return 33 <= o <= 47 or 58 <= o <= 64 or 91 <= o <= 96 or 123 <= o <= 126 or unicodedata.category(ch)[0] == "P"
+
+
+def _is_cjk(ch):
+    o = ord(ch)
+    return (0x4E00 <= o <= 0x9FFF or 0x3400 <= o <= 0x4DBF or 0x20000 <= o <= 0x2A6DF or 0x2A700 <= o <= 0x2B73F or
+            0x2B740 <= o <= 0x2B81F or 0x2B920 <= o <= 0x2CEAF or 0xF900 <= o <= 0xFAFF or 0x2F800 <= o <= 0x2FA1F)
+
+
+def bert_normalize(text):
+    """The uncased BERT normaliser: clean-up, CJK spacing, accent stripping, per-character lowercasing."""
+    out = []
+    for ch in text:
+        if ch == "\x00" or ch == "�" or _bert_is_control(ch):
+            continue
+        if _bert_is_white(ch):
+            out.append(" ")
+        elif _is_cjk(ch):
+            out.append(" " + ch + " ")
+        else:
+            out.append(ch)
+    text = unicodedata.normalize("NFD", "".join(out))
+    return "".join(ch.lower() for ch in text if unicodedata.category(ch) != "Mn")
+
+
+def bert_split(text):
+    """Whitespace splits (and is dropped); each punctuation character is a word of its own."""
+    words, cur = [], []
+    for ch in text:
+        if _bert_is_white(ch) or _bert_is_punct(ch):
+            if cur:
+                words.append("".join(cur))
+                cur = []
+            if not _bert_is_white(ch):
+                words.append(ch)
+        else:
+            cur.append(ch)
+    if cur:
+        words.append("".join(cur))
+    return words
+
+
+class BertWordPieceTokenizer:
+    def __init__(self, vocab, max_length=77, max_word_chars=100):
+        """vocab: {token: id} or a path to vocab.txt (one token per line, id = line number)."""
+        if isinstance(vocab, (str, os.PathLike)):
+            with open(vocab, encoding="utf-8") as f:
+                vocab = {ln.rstrip("\n"): i for i, ln in enumerate(f) if ln.rstrip("\n")}
+        self.vocab = dict(vocab)
+        missing = [t for t in ("[CLS]", "[SEP]", "[PAD]", "[UNK]") if t not in self.vocab]
+        if missing:
+            raise ValueError(f"BERT vocabulary lacks {missing}")
+        self.cls_id, self.sep_id = self.vocab["[CLS]"], self.vocab["[SEP]"]
+        self.pad_id, self.unk_id = self.vocab["[PAD]"], self.vocab["[UNK]"]
+        self.max_length, self.max_word_chars = max_length, max_word_chars
+        self._specials = [t for t in BERT_SPECIAL if t in self.vocab]
+
+    @classmethod
+    def from_dir(cls, path, max_length=77):
+        return cls(os.path.join(path, "vocab.txt"), max_length)
+
+    def __len__(self):
+        return len(self.vocab)
+
+    def _wordpiece(self, word):
+        if len(word) > self.max_word_chars:
+            return [self.unk_id]
+        ids, start = [], 0
+        while start < len(word):
+            end = len(word)
+            while end > start:
+                piece = word[start:end] if start == 0 else "##" + word[start:end]
+                if piece in self.vocab:
+                    ids.append(self.vocab[piece])
+                    break
+                end -= 1
+            if end == start:
+                return [self.unk_id]
+            start = end
+        return ids
+
+    def _encode_plain(self, text):
+        ids = []
+        for w in bert_split(bert_normalize(text)):
+            ids.extend(self._wordpiece(w))
+        return ids
+
+    def tokenize_ids(self, text):
+        """Token ids of `text` without [CLS] / [SEP] / padding; literal special tokens map to their ids."""
+        ids, rest = [], text
+        while rest:
+            hits = [(rest.find(s), s) for s in self._specials if s in rest]
+            if not hits:
+                ids.extend(self._encode_plain(rest))
+                break
+            cut, special = min(hits, key=lambda h: (h[0], -len(h[1])))
+            ids.extend(self._encode_plain(rest[:cut]))
+            ids.append(self.vocab[special])
+            rest = rest[cut + len(special):]
+        return ids
+
+    def __call__(self, texts, max_length=None):
+        """list[str] (or one str) -> list of max_length-long id lists: [CLS] + tokens (truncated) + [SEP], [PAD] after."""
+        if isinstance(texts, str):
+            texts = [texts]
+        n = max_length or self.max_length
+        out = []
+        for t in texts:
+            ids = [self.cls_id] + self.tokenize_ids(t)[: n - 2] + [self.sep_id]
+            out.append(ids + [self.pad_id] * (n - len(ids)))
+        return out

@@ -27,6 +27,7 @@ TARGET_MAP = {
     "ldm.models.autoencoder.VQModelInterface": "sdb200.vq.VQModelInterface",
     "ldm.modules.encoders.modules.FrozenCLIPEmbedder": "sdb200.clip.FrozenCLIPEmbedder",
     "ldm.modules.encoders.modules.ClassEmbedder": "sdb200.encoders.ClassEmbedder",
+    "ldm.modules.encoders.modules.BERTEmbedder": "sdb200.bert.BERTEmbedder",
 }
 
 
