@@ -308,6 +308,18 @@ int sdb_patch_unfold(const float* x, int32_t nb, int32_t c, int32_t h, int32_t w
 int sdb_patch_fold(const float* tiles, int32_t tiles_nhwc, int32_t nb, int32_t c, int32_t kh, int32_t kw, int32_t ly,
                    int32_t lx, int32_t sy, int32_t sx, const float* weight, const float* norm, int32_t h, int32_t w,
                    float* out_nchw, sdb_stream_t stream);
+/* SpatialRescaler (ldm/modules/encoders/modules.py:106-134) with method 'bilinear', multiplier 0.5: n_stages
+ * (0..3) x F.interpolate(scale_factor=0.5, mode='bilinear') of x fp32 [nb, cin, h, w] (each stage floor(side / 2),
+ * computed as torch's CUDA kernel orders it), then the optional channel_mapper 1x1 conv: weight fp32 [cout, cin],
+ * bias fp32 [cout] or NULL, accumulated by fma over cin ascending, bias last. weight NULL: no mapper, cout = cin.
+ * out fp32 [nb, cout, h >> n_stages, w >> n_stages]. */
+int sdb_spatial_rescale(const float* x_nchw, int32_t nb, int32_t cin, int32_t h, int32_t w, int32_t n_stages,
+                        const float* weight, const float* bias, int32_t cout, float* out_nchw, sdb_stream_t stream);
+/* The same SpatialRescaler applied to the one-hot of uint8 label ids [nb, h, w] (ids < cin <= 256; the caller checks
+ * them), without materialising it: each output pixel sums W[o, k] * count_k / 4^n_stages over the classes k present in
+ * its window, ascending. Bit-identical to sdb_spatial_rescale on the one-hot. The channel map (weight) is required. */
+int sdb_seg_labels_rescale(const uint8_t* labels, int32_t nb, int32_t cin, int32_t h, int32_t w, int32_t n_stages,
+                           const float* weight, const float* bias, int32_t cout, float* out_nchw, sdb_stream_t stream);
 /* out = a*x + b (latent scaling z/0.18215, ddpm.py:713) */
 int sdb_axpby(const float* x, float a, float b, int64_t n, float* out, sdb_stream_t stream);
 /* out = a*x + b*y (DDIMSampler.stochastic_encode, ddim.py:206-220; q_sample, ddpm.py:274-277) */

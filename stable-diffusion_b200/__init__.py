@@ -11,7 +11,7 @@ from . import arch, bert, checkpoint, clip, diffusion, dist, encoders, lib, ops,
 from .bert import BERTEmbedder  # noqa: E402,F401
 from .clip import FrozenCLIPEmbedder  # noqa: E402,F401
 from .diffusion import LatentDiffusion  # noqa: E402,F401
-from .encoders import ClassEmbedder  # noqa: E402,F401
+from .encoders import ClassEmbedder, SpatialRescaler  # noqa: E402,F401
 from .safety import StableDiffusionSafetyChecker  # noqa: E402,F401
 from .samplers import DDIMSampler, DPMSolverSampler, PLMSSampler  # noqa: E402,F401
 from .unet import UNetModel  # noqa: E402,F401

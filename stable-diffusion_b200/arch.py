@@ -99,6 +99,18 @@ BSR_SR_UNET = dict(image_size=64, in_channels=6, out_channels=3, model_channels=
 TINY_BSR_UNET = dict(image_size=16, in_channels=6, out_channels=3, model_channels=160, attention_resolutions=[2],
                      num_res_blocks=1, channel_mult=[1, 2], num_head_channels=32)
 TINY_VQ_F4 = dict(embed_dim=3, n_embed=512, ddconfig={**TINY_VQ["ddconfig"], "ch_mult": [1, 1, 2]})
+# the LDM semantic-synthesis models (models/ldm/semantic_synthesis256 and semantic_synthesis512: the same keys and
+# shapes, image_size 64 / 128): x_t (3 channels) concatenated with the SpatialRescaler's 182 -> 3 channel map of the
+# label map at the latent size. legacy defaults; attention_resolutions 32 / 16 / 8 are never reached (ds 1, 2, 4), so
+# the only attention is the middle block's AttentionBlock of 8 heads at d = 128. Widths 128 / 512 / 1024, skip concats
+# up to 2048: 4 .. 64 channels per GroupNorm group. VQ-f4 first stage.
+SEMANTIC_SYNTHESIS_UNET = dict(image_size=64, in_channels=6, out_channels=3, model_channels=128,
+                               attention_resolutions=[32, 16, 8], num_res_blocks=2, channel_mult=[1, 4, 8], num_heads=8)
+SEMANTIC_SYNTHESIS_COND = dict(n_stages=2, in_channels=182, out_channels=3)
+# small members for tests, same topology: widths 64 / 256 / 512, mid attention 8 x d 64; a 20-class rescaler
+TINY_SEMANTIC_UNET = dict(image_size=16, in_channels=6, out_channels=3, model_channels=64,
+                          attention_resolutions=[32, 16, 8], num_res_blocks=1, channel_mult=[1, 4, 8], num_heads=8)
+TINY_SEMANTIC_COND = dict(n_stages=2, in_channels=20, out_channels=3)
 TINY_VAE = dict(embed_dim=4, ddconfig=dict(double_z=True, z_channels=4, resolution=32, in_channels=3, out_ch=3,
                                            ch=64, ch_mult=[1, 2], num_res_blocks=1, attn_resolutions=[],
                                            dropout=0.0))
@@ -389,6 +401,17 @@ def class_embedder_param_shapes(cfg):
     """Keys as ClassEmbedder.state_dict() (ldm/modules/encoders/modules.py:19-32), under `cond_stage_model.` in an
     LDM checkpoint."""
     return OrderedDict([("embedding.weight", (cfg["n_classes"], cfg["embed_dim"]))])
+
+
+def spatial_rescaler_param_shapes(cfg):
+    """Keys as SpatialRescaler.state_dict() (modules.py:106-134): the channel_mapper 1x1 conv when out_channels is set
+    (bias only with bias=True); under `cond_stage_model.` in an LDM checkpoint."""
+    p = OrderedDict()
+    if cfg.get("out_channels") is not None:
+        p["channel_mapper.weight"] = (cfg["out_channels"], cfg.get("in_channels", 3), 1, 1)
+        if cfg.get("bias", False):
+            p["channel_mapper.bias"] = (cfg["out_channels"],)
+    return p
 
 
 # ------------------------------------------------------------------------------------------------ CLIP

@@ -115,6 +115,8 @@ SIGNATURES = {
     "sdb_lr_prepare": ([_P, _I, _I, _I, _P, _P], C.c_int),
     "sdb_patch_unfold": ([_P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P], C.c_int),
     "sdb_patch_fold": ([_P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _I, _I, _P, _P], C.c_int),
+    "sdb_spatial_rescale": ([_P, _I, _I, _I, _I, _I, _P, _P, _I, _P, _P], C.c_int),
+    "sdb_seg_labels_rescale": ([_P, _I, _I, _I, _I, _I, _P, _P, _I, _P, _P], C.c_int),
     # post-processing (safety.cu)
     "sdb_resample_u8": ([_P, _P, _I, _I, _I, _I, _I, _P, _P, _I, _I, _P, _P], C.c_int),
     "sdb_clip_normalize": ([_P, _I, _I, _I, _I, _F, _F, _F, _F, _F, _F, _P, _P], C.c_int),

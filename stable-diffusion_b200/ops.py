@@ -594,6 +594,47 @@ def patch_fold(tiles, weight, norm, grid, stride, nhwc=False):
     return out
 
 
+def spatial_rescale(x, n_stages, weight=None, bias=None):
+    """SpatialRescaler (bilinear, multiplier 0.5) of x fp32 NCHW [nb, cin, h, w]: n_stages x0.5 interpolations, then the
+    channel_mapper 1x1 conv when weight fp32 [cout, cin] is given (bias fp32 [cout] or None). Returns fp32 NCHW
+    [nb, cout, h >> n_stages, w >> n_stages] (sdb_spatial_rescale)."""
+    _chk32(x, "x")
+    nb, cin, h, w = x.shape
+    cout = cin
+    if weight is not None:
+        _chk32(weight, "weight")
+        assert weight.dim() == 2 and weight.shape[1] == cin, (tuple(weight.shape), cin)
+        cout = weight.shape[0]
+    if bias is not None:
+        assert weight is not None
+        _chk32(bias, "bias")
+        assert tuple(bias.shape) == (cout,)
+    out = torch.empty((nb, cout, h >> n_stages, w >> n_stages), dtype=torch.float32, device=x.device)
+    _l.check(_l.load().sdb_spatial_rescale(_ptr(x), nb, cin, h, w, n_stages, _ptr(weight), _ptr(bias), cout, _ptr(out),
+                                           _stream()), "sdb_spatial_rescale")
+    _count()
+    return out
+
+
+def seg_labels_rescale(labels_u8, cin, n_stages, weight, bias=None):
+    """The SpatialRescaler of the one-hot of labels uint8 [nb, h, w] (ids < cin, checked by the caller) with the channel
+    map weight fp32 [cout, cin] (+ bias), without materialising the one-hot: fp32 NCHW [nb, cout, h >> n_stages,
+    w >> n_stages], bit-identical to spatial_rescale of the one-hot (sdb_seg_labels_rescale)."""
+    assert labels_u8.dtype == torch.uint8 and labels_u8.is_cuda and labels_u8.is_contiguous() and labels_u8.dim() == 3
+    _chk32(weight, "weight")
+    assert weight.dim() == 2 and weight.shape[1] == cin, (tuple(weight.shape), cin)
+    cout = weight.shape[0]
+    if bias is not None:
+        _chk32(bias, "bias")
+        assert tuple(bias.shape) == (cout,)
+    nb, h, w = labels_u8.shape
+    out = torch.empty((nb, cout, h >> n_stages, w >> n_stages), dtype=torch.float32, device=labels_u8.device)
+    _l.check(_l.load().sdb_seg_labels_rescale(_ptr(labels_u8), nb, cin, h, w, n_stages, _ptr(weight), _ptr(bias), cout,
+                                              _ptr(out), _stream()), "sdb_seg_labels_rescale")
+    _count()
+    return out
+
+
 def upsample2x(x):
     _chk32(x, "x")
     nb, h, w, c = x.shape

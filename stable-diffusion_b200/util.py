@@ -28,6 +28,7 @@ TARGET_MAP = {
     "ldm.modules.encoders.modules.FrozenCLIPEmbedder": "sdb200.clip.FrozenCLIPEmbedder",
     "ldm.modules.encoders.modules.ClassEmbedder": "sdb200.encoders.ClassEmbedder",
     "ldm.modules.encoders.modules.BERTEmbedder": "sdb200.bert.BERTEmbedder",
+    "ldm.modules.encoders.modules.SpatialRescaler": "sdb200.encoders.SpatialRescaler",
 }
 
 
