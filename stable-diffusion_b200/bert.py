@@ -19,18 +19,21 @@ from __future__ import annotations
 import os
 
 import torch
-import torch.nn as nn
 
 from . import ops
 from .arch import bert_param_shapes
+from .clip import encoder_layers
 from .ops import ACT_GELU
-from .util import adopt_state_dict
+from .util import PackedStage
 
 HEADS, DIM_HEAD = 8, 64          # x_transformer.py DEFAULT_DIM_HEAD and AttentionLayers' heads: fixed by the config
 LN_EPS = 1e-5
 
 
-class BERTEmbedder(nn.Module):
+class BERTEmbedder(PackedStage):
+    # to_logits is part of the reference's state dict but not of the embedding: not required, dropped when present
+    drop_prefixes = ("transformer.to_logits.",)
+
     def __init__(self, n_embed, n_layer, vocab_size=30522, max_seq_len=77, device="cuda", use_tokenizer=True,
                  embedding_dropout=0.0, vocab_dir=None):
         super().__init__()
@@ -41,37 +44,10 @@ class BERTEmbedder(nn.Module):
         self.embedding_dropout = float(embedding_dropout)   # dropout is inactive at inference (eval mode)
         self.vocab_dir = vocab_dir
         self.tokenizer = None
-        # to_logits is part of the reference's state dict but not of the embedding: not required, dropped when present
-        self.shapes = {k: v for k, v in bert_param_shapes(self.cfg).items() if not k.startswith("transformer.to_logits.")}
-        self.W = None
-        self._host_sd = None
+        self.shapes = {k: v for k, v in bert_param_shapes(self.cfg).items() if not k.startswith(self.drop_prefixes)}
 
     def freeze(self):
         return self
-
-    def _load_from_state_dict(self, state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
-                              error_msgs):
-        sd = adopt_state_dict(self, state_dict, prefix, missing_keys, unexpected_keys, error_msgs,
-                              ignore=("transformer.to_logits.",))
-        if sd is None:
-            return
-        self._host_sd = sd
-        if self.W is not None:
-            self.pack_weights(self.W["device"])
-
-    def load_weights(self, sd, device):
-        for k, shape in self.shapes.items():
-            assert k in sd and tuple(sd[k].shape) == tuple(shape), k
-        self._host_sd = {k: sd[k] for k in self.shapes}
-        self.pack_weights(torch.device(device))
-        return self
-
-    def _apply(self, fn, *a, **k):
-        r = super()._apply(fn, *a, **k)
-        probe = fn(torch.empty(0))
-        if probe.is_cuda and self._host_sd is not None and (self.W is None or self.W["device"] != probe.device):
-            self.pack_weights(probe.device)
-        return r
 
     @torch.no_grad()
     def pack_weights(self, device):
@@ -118,22 +94,10 @@ class BERTEmbedder(nn.Module):
         W = self.W
         ids = self.check_ids(ids).to(W["device"]).contiguous()
         B, n = ids.shape
-        D, inner = self.cfg["n_embed"], HEADS * DIM_HEAD
-        x = ops.embed_tokens(ids, W["tok"], W["pos"])                                  # [B*n, D] fp32
-        for L in W["layers"]:
-            y = ops.layernorm(x, *L["ln1"], eps=LN_EPS)
-            qk, _ = ops.gemm(y, L["w_qk"], want_f16=True)                              # [B*n, 2*inner]
-            v, _ = ops.gemm(y, L["w_v"], want_f16=True)
-            qk3 = qk.view(B, n, 2 * inner)
-            vt = ops.transpose_f16(v.view(B, n, inner))                                # [B, inner, pad8(n)]
-            o = ops.attention(qk3[:, :, :inner], qk3[:, :, inner:], vt, heads=HEADS, d=DIM_HEAD, dpad=DIM_HEAD,
-                              nq=n, nkv=n, scale=DIM_HEAD ** -0.5, causal=False)
-            _, x = ops.gemm(o.view(-1, inner), L["w_o"], bias=L["b_o"], residual=x, want_f32=True)
-            y = ops.layernorm(x, *L["ln2"], eps=LN_EPS)
-            g, _ = ops.gemm(y, L["w_fc1"], bias=L["b_fc1"], act=ACT_GELU, want_f16=True)
-            _, x = ops.gemm(g, L["w_fc2"], bias=L["b_fc2"], residual=x, want_f32=True)
+        x = ops.embed_tokens(ids, W["tok"], W["pos"])                                  # [B*n, n_embed] fp32
+        x = encoder_layers(x, W["layers"], B, heads=HEADS, d=DIM_HEAD, eps=LN_EPS, act=ACT_GELU)
         _, z = ops.layernorm(x, *W["ln_f"], eps=LN_EPS, want_f32=True)
-        return z.view(B, n, D)
+        return z.view(B, n, self.cfg["n_embed"])
 
     def _tokenize(self, text):
         """list[str] -> int64 [B, max_seq_len] as BERTTokenizer (modules.py:63-67): truncation, max_length padding."""

@@ -21,7 +21,51 @@ import torch.nn as nn
 from . import ops
 from .arch import SD_V1_CLIP, clip_param_shapes
 from .ops import ACT_QUICK_GELU
-from .util import adopt_state_dict
+from .util import PackedStage
+
+
+def pack_clip_layers(sd, prefix, n_layers):
+    """The layer dicts of encoder_layers from HF CLIP encoder layers `{prefix}.{i}.*` (transformers' CLIPEncoderLayer
+    keys; sd: fp32 tensors on the target device)."""
+    f32 = lambda k: sd[k].contiguous()
+    f16 = lambda k: sd[k].half().contiguous()
+    layers = []
+    for i in range(n_layers):
+        p = f"{prefix}.{i}"
+        wo = sd[p + ".self_attn.out_proj.weight"]
+        layers.append({
+            "ln1": (f32(p + ".layer_norm1.weight"), f32(p + ".layer_norm1.bias")),
+            "ln2": (f32(p + ".layer_norm2.weight"), f32(p + ".layer_norm2.bias")),
+            "w_qk": torch.cat([sd[p + ".self_attn.q_proj.weight"], sd[p + ".self_attn.k_proj.weight"]], 0).half().contiguous(),
+            "b_qk": torch.cat([sd[p + ".self_attn.q_proj.bias"], sd[p + ".self_attn.k_proj.bias"]]).contiguous(),
+            "w_v": f16(p + ".self_attn.v_proj.weight"),
+            "w_o": wo.half().contiguous(),
+            # softmax rows sum to 1: the value bias passes through the attention unchanged -> fold it through out_proj
+            "b_o": (sd[p + ".self_attn.out_proj.bias"] + wo @ sd[p + ".self_attn.v_proj.bias"]).contiguous(),
+            "w_fc1": f16(p + ".mlp.fc1.weight"), "b_fc1": f32(p + ".mlp.fc1.bias"),
+            "w_fc2": f16(p + ".mlp.fc2.weight"), "b_fc2": f32(p + ".mlp.fc2.bias")})
+    return layers
+
+
+def encoder_layers(x, layers, B, *, heads, d, eps, act, causal=False):
+    """Pre-LN transformer encoder layers (CLIP text and vision towers, BERTEmbedder) over the fp32 residual stream
+    x [B*n, hidden]; returns the stream. Per layer: LayerNorm -> Q|K GEMM (bias "b_qk" when the layer has one) and V
+    GEMM (its bias folded into "b_o") -> attention of `heads` heads of width d -> out-projection + residual ->
+    LayerNorm -> fc1 with the `act` epilogue -> fc2 + residual. The attention width heads * d need not be hidden."""
+    n, w = x.shape[0] // B, heads * d
+    for L in layers:
+        y = ops.layernorm(x, *L["ln1"], eps=eps)
+        qk, _ = ops.gemm(y, L["w_qk"], bias=L.get("b_qk"), want_f16=True)            # [B*n, 2w]
+        v, _ = ops.gemm(y, L["w_v"], want_f16=True)
+        qk3 = qk.view(B, n, 2 * w)
+        vt = ops.transpose_f16(v.view(B, n, w))                                       # [B, w, pad8(n)]
+        o = ops.attention(qk3[:, :, :w], qk3[:, :, w:], vt, heads=heads, d=d, dpad=d, nq=n, nkv=n, scale=d ** -0.5,
+                          causal=causal)
+        _, x = ops.gemm(o.view(-1, w), L["w_o"], bias=L["b_o"], residual=x, want_f32=True)
+        y = ops.layernorm(x, *L["ln2"], eps=eps)
+        g, _ = ops.gemm(y, L["w_fc1"], bias=L["b_fc1"], act=act, want_f16=True)
+        _, x = ops.gemm(g, L["w_fc2"], bias=L["b_fc2"], residual=x, want_f32=True)
+    return x
 
 
 class _Transformer(nn.Module):
@@ -33,18 +77,13 @@ class _Transformer(nn.Module):
 
     def _load_from_state_dict(self, state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
                               error_msgs):
-        o = self._owner
-        # text_model.embeddings.position_ids is a buffer of older transformers versions (present in sd-v1 checkpoints)
-        sd = adopt_state_dict(o, state_dict, prefix, missing_keys, unexpected_keys, error_msgs,
-                              ignore=("text_model.embeddings.position_ids",))
-        if sd is None:
-            return
-        o._host_sd = sd
-        if o.W is not None:
-            o.pack_weights(o.W["device"])
+        self._owner._adopt(state_dict, prefix, missing_keys, unexpected_keys, error_msgs)
 
 
-class FrozenCLIPEmbedder(nn.Module):
+class FrozenCLIPEmbedder(PackedStage):
+    # text_model.embeddings.position_ids is a buffer of older transformers versions (present in sd-v1 checkpoints)
+    drop_prefixes = ("text_model.embeddings.position_ids",)
+
     def __init__(self, version="openai/clip-vit-large-patch14", device="cuda", max_length=77, config=None):
         super().__init__()
         self.cfg = dict(config or SD_V1_CLIP)
@@ -52,52 +91,23 @@ class FrozenCLIPEmbedder(nn.Module):
         self.device = device
         self.max_length = max_length
         self.shapes = clip_param_shapes(self.cfg)
-        self.W = None
-        self._host_sd = None
         self.transformer = _Transformer(self)
         self.tokenizer = None
 
+    def _load_from_state_dict(self, *args):
+        nn.Module._load_from_state_dict(self, *args)   # the keys sit one module below, in the shim, which adopts them
+
     def freeze(self):
         return self
-
-    def load_weights(self, sd, device):
-        for k, shape in self.shapes.items():
-            assert k in sd and tuple(sd[k].shape) == tuple(shape), k
-        self._host_sd = {k: sd[k] for k in self.shapes}
-        self.pack_weights(torch.device(device))
-        return self
-
-    def _apply(self, fn, *a, **k):
-        r = super()._apply(fn, *a, **k)
-        probe = fn(torch.empty(0))
-        if probe.is_cuda and self._host_sd is not None and (self.W is None or self.W["device"] != probe.device):
-            self.pack_weights(probe.device)
-        return r
 
     @torch.no_grad()
     def pack_weights(self, device):
         sd = {k: v.detach().to(device=device, dtype=torch.float32) for k, v in self._host_sd.items()}
         f32 = lambda k: sd[k].contiguous()
-        f16 = lambda k: sd[k].half().contiguous()
-        h = self.cfg["hidden_size"]
-        W = {"device": device, "tok": f32("text_model.embeddings.token_embedding.weight"),
-             "pos": f32("text_model.embeddings.position_embedding.weight"), "layers": []}
-        for i in range(self.cfg["num_hidden_layers"]):
-            p = f"text_model.encoder.layers.{i}"
-            wo = sd[p + ".self_attn.out_proj.weight"]
-            L = {"ln1": (f32(p + ".layer_norm1.weight"), f32(p + ".layer_norm1.bias")),
-                 "ln2": (f32(p + ".layer_norm2.weight"), f32(p + ".layer_norm2.bias")),
-                 "w_qk": torch.cat([sd[p + ".self_attn.q_proj.weight"], sd[p + ".self_attn.k_proj.weight"]],
-                                   0).half().contiguous(),
-                 "b_qk": torch.cat([sd[p + ".self_attn.q_proj.bias"], sd[p + ".self_attn.k_proj.bias"]]).contiguous(),
-                 "w_v": f16(p + ".self_attn.v_proj.weight"),
-                 "w_o": wo.half().contiguous(),
-                 "b_o": (sd[p + ".self_attn.out_proj.bias"] + wo @ sd[p + ".self_attn.v_proj.bias"]).contiguous(),
-                 "w_fc1": f16(p + ".mlp.fc1.weight"), "b_fc1": f32(p + ".mlp.fc1.bias"),
-                 "w_fc2": f16(p + ".mlp.fc2.weight"), "b_fc2": f32(p + ".mlp.fc2.bias")}
-            W["layers"].append(L)
-        W["ln_f"] = (f32("text_model.final_layer_norm.weight"), f32("text_model.final_layer_norm.bias"))
-        self.W = W
+        self.W = {"device": device, "tok": f32("text_model.embeddings.token_embedding.weight"),
+                  "pos": f32("text_model.embeddings.position_embedding.weight"),
+                  "layers": pack_clip_layers(sd, "text_model.encoder.layers", self.cfg["num_hidden_layers"]),
+                  "ln_f": (f32("text_model.final_layer_norm.weight"), f32("text_model.final_layer_norm.bias"))}
 
     @torch.no_grad()
     def encode_ids(self, ids):
@@ -111,18 +121,7 @@ class FrozenCLIPEmbedder(nn.Module):
         assert d == 64, "CLIP text heads are 64 wide"
         eps = self.cfg["layer_norm_eps"]
         x = ops.embed_tokens(ids.contiguous(), W["tok"], W["pos"])                     # [B*n, h] fp32
-        for L in W["layers"]:
-            y = ops.layernorm(x, *L["ln1"], eps=eps)
-            qk, _ = ops.gemm(y, L["w_qk"], bias=L["b_qk"], want_f16=True)             # [B*n, 2h]
-            v, _ = ops.gemm(y, L["w_v"], want_f16=True)                               # bias folded into b_o
-            qk3 = qk.view(B, n, 2 * h)
-            vt = ops.transpose_f16(v.view(B, n, h))                                   # [B, h, pad8(n)]
-            o = ops.attention(qk3[:, :, :h], qk3[:, :, h:], vt, heads=heads, d=d, dpad=d, nq=n, nkv=n,
-                              scale=d ** -0.5, causal=True)
-            _, x = ops.gemm(o.view(-1, h), L["w_o"], bias=L["b_o"], residual=x, want_f32=True)
-            y = ops.layernorm(x, *L["ln2"], eps=eps)
-            g, _ = ops.gemm(y, L["w_fc1"], bias=L["b_fc1"], act=ACT_QUICK_GELU, want_f16=True)
-            _, x = ops.gemm(g, L["w_fc2"], bias=L["b_fc2"], residual=x, want_f32=True)
+        x = encoder_layers(x, W["layers"], B, heads=heads, d=d, eps=eps, act=ACT_QUICK_GELU, causal=True)
         _, z = ops.layernorm(x, *W["ln_f"], eps=eps, want_f32=True)
         return z.view(B, n, h)
 

@@ -15,43 +15,17 @@ SpatialRescaler, the cond stage of the semantic-synthesis LDMs: drop-in for
 from __future__ import annotations
 
 import torch
-import torch.nn as nn
 
 from . import ops
-from .util import adopt_state_dict
+from .util import PackedStage
 
 
-class ClassEmbedder(nn.Module):
+class ClassEmbedder(PackedStage):
     def __init__(self, embed_dim, n_classes=1000, key="class"):
         super().__init__()
         self.key = key
         self.embed_dim, self.n_classes = int(embed_dim), int(n_classes)
         self.shapes = {"embedding.weight": (self.n_classes, self.embed_dim)}
-        self.W = None
-        self._host_sd = None
-
-    def _load_from_state_dict(self, state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
-                              error_msgs):
-        sd = adopt_state_dict(self, state_dict, prefix, missing_keys, unexpected_keys, error_msgs)
-        if sd is None:
-            return
-        self._host_sd = sd
-        if self.W is not None:
-            self.pack_weights(self.W["device"])
-
-    def load_weights(self, sd, device):
-        for k, shape in self.shapes.items():
-            assert k in sd and tuple(sd[k].shape) == tuple(shape), k
-        self._host_sd = {k: sd[k] for k in self.shapes}
-        self.pack_weights(torch.device(device))
-        return self
-
-    def _apply(self, fn, *a, **k):
-        r = super()._apply(fn, *a, **k)
-        probe = fn(torch.empty(0))
-        if probe.is_cuda and self._host_sd is not None and (self.W is None or self.W["device"] != probe.device):
-            self.pack_weights(probe.device)
-        return r
 
     @torch.no_grad()
     def pack_weights(self, device):
@@ -77,7 +51,7 @@ class ClassEmbedder(nn.Module):
         return out.view(-1, 1, self.embed_dim)
 
 
-class SpatialRescaler(nn.Module):
+class SpatialRescaler(PackedStage):
     """Drop-in for `ldm.modules.encoders.modules.SpatialRescaler` (modules.py:106-134): n_stages bilinear x0.5
     interpolations, then the optional `channel_mapper` 1x1 conv in_channels -> out_channels (state-dict keys
     `channel_mapper.weight` [out, in, 1, 1] and, with bias, `channel_mapper.bias`). Only the configuration every
@@ -111,18 +85,8 @@ class SpatialRescaler(nn.Module):
             self.shapes["channel_mapper.weight"] = (self.out_channels, self.in_channels, 1, 1)
             if bias:
                 self.shapes["channel_mapper.bias"] = (self.out_channels,)
-        self.W = None
-        self._host_sd = None if self.shapes else {}
-
-    _load_from_state_dict = ClassEmbedder._load_from_state_dict
-    load_weights = ClassEmbedder.load_weights
-
-    def _apply(self, fn, *a, **k):
-        r = super()._apply(fn, *a, **k)
-        probe = fn(torch.empty(0))
-        if probe.is_cuda and self._host_sd is not None and (self.W is None or self.W["device"] != probe.device):
-            self.pack_weights(probe.device)
-        return r
+        if not self.shapes:   # nothing to load: .cuda() packs right away
+            self._host_sd = {}
 
     @torch.no_grad()
     def pack_weights(self, device):

@@ -11,26 +11,17 @@ decision (sdb_safety_scores). State-dict keys are diffusers' (`vision_model.visi
 """
 from __future__ import annotations
 
-import ctypes as C
 import math
 
 import numpy as np
 import torch
-import torch.nn as nn
 
 from . import lib as _l
 from . import ops
 from .arch import CLIP_IMAGE_MEAN, CLIP_IMAGE_STD, SD_V1_SAFETY, safety_param_shapes
-from .ops import ACT_QUICK_GELU
-from .util import adopt_state_dict
-
-
-def _ptr(t):
-    return None if t is None else C.c_void_p(t.data_ptr())
-
-
-def _stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+from .clip import encoder_layers, pack_clip_layers
+from .ops import ACT_QUICK_GELU, _ptr, _stream
+from .util import PackedStage
 
 
 def _bicubic(x):
@@ -121,52 +112,20 @@ class CLIPImagePreprocessor:
         return out
 
 
-class _VisionModel(nn.Module):
-    """Holds the `vision_model.*` keys of the checkpoint (diffusers nests a CLIPVisionModel there)."""
+class StableDiffusionSafetyChecker(PackedStage):
+    drop_prefixes = ("vision_model.vision_model.embeddings.position_ids",)
 
-    def __init__(self):
-        super().__init__()
-
-
-class StableDiffusionSafetyChecker(nn.Module):
     def __init__(self, config=None, device="cuda"):
         super().__init__()
         self.cfg = dict(config or SD_V1_SAFETY)
         self.device = device
         self.shapes = safety_param_shapes(self.cfg)
-        self.W = None
-        self._host_sd = None
         self.feature_extractor = CLIPImagePreprocessor(self.cfg["image_size"])
-
-    def _load_from_state_dict(self, state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
-                              error_msgs):
-        sd = adopt_state_dict(self, state_dict, prefix, missing_keys, unexpected_keys, error_msgs,
-                              ignore=("vision_model.vision_model.embeddings.position_ids",))
-        if sd is None:
-            return
-        self._host_sd = sd
-        if self.W is not None:
-            self.pack_weights(self.W["device"])
-
-    def load_weights(self, sd, device):
-        for k, shape in self.shapes.items():
-            assert k in sd and tuple(sd[k].shape) == tuple(shape), k
-        self._host_sd = {k: sd[k] for k in self.shapes}
-        self.pack_weights(torch.device(device))
-        return self
-
-    def _apply(self, fn, *a, **k):
-        r = super()._apply(fn, *a, **k)
-        probe = fn(torch.empty(0))
-        if probe.is_cuda and self._host_sd is not None and (self.W is None or self.W["device"] != probe.device):
-            self.pack_weights(probe.device)
-        return r
 
     @torch.no_grad()
     def pack_weights(self, device):
         sd = {k: v.detach().to(device=device, dtype=torch.float32) for k, v in self._host_sd.items()}
         f32 = lambda k: sd[k].contiguous()
-        f16 = lambda k: sd[k].half().contiguous()
         cfg = self.cfg
         h, P = cfg["hidden_size"], cfg["patch_size"]
         v = "vision_model.vision_model"
@@ -177,22 +136,9 @@ class StableDiffusionSafetyChecker(nn.Module):
         W = {"device": device, "w_patch": wp, "kpad": kpad, "pos_patches": pos[1:].contiguous(),
              "cls_pos": (sd[f"{v}.embeddings.class_embedding"] + pos[0]).contiguous(),
              "ln_pre": (f32(f"{v}.pre_layrnorm.weight"), f32(f"{v}.pre_layrnorm.bias")),
-             "ln_post": (f32(f"{v}.post_layernorm.weight"), f32(f"{v}.post_layernorm.bias")), "layers": []}
-        for i in range(cfg["num_hidden_layers"]):
-            p = f"{v}.encoder.layers.{i}"
-            wo = sd[p + ".self_attn.out_proj.weight"]
-            W["layers"].append({
-                "ln1": (f32(p + ".layer_norm1.weight"), f32(p + ".layer_norm1.bias")),
-                "ln2": (f32(p + ".layer_norm2.weight"), f32(p + ".layer_norm2.bias")),
-                "w_qk": torch.cat([sd[p + ".self_attn.q_proj.weight"], sd[p + ".self_attn.k_proj.weight"]], 0).half().contiguous(),
-                "b_qk": torch.cat([sd[p + ".self_attn.q_proj.bias"], sd[p + ".self_attn.k_proj.bias"]]).contiguous(),
-                "w_v": f16(p + ".self_attn.v_proj.weight"),
-                "w_o": wo.half().contiguous(),
-                # softmax rows sum to 1: the value bias passes through the attention unchanged -> fold it through out_proj
-                "b_o": (sd[p + ".self_attn.out_proj.bias"] + wo @ sd[p + ".self_attn.v_proj.bias"]).contiguous(),
-                "w_fc1": f16(p + ".mlp.fc1.weight"), "b_fc1": f32(p + ".mlp.fc1.bias"),
-                "w_fc2": f16(p + ".mlp.fc2.weight"), "b_fc2": f32(p + ".mlp.fc2.bias")})
-        W["w_proj"] = f16("visual_projection.weight")
+             "ln_post": (f32(f"{v}.post_layernorm.weight"), f32(f"{v}.post_layernorm.bias")),
+             "layers": pack_clip_layers(sd, f"{v}.encoder.layers", cfg["num_hidden_layers"])}
+        W["w_proj"] = sd["visual_projection.weight"].half().contiguous()
         W["concept"], W["special"] = f32("concept_embeds"), f32("special_care_embeds")
         W["concept_w"], W["special_w"] = f32("concept_embeds_weights"), f32("special_care_embeds_weights")
         self.W = W
@@ -219,17 +165,7 @@ class StableDiffusionSafetyChecker(nn.Module):
             ops.axpby(W["cls_pos"], 1.0, 0.0, out=x[b, 0])
             ops.gemm(patches[b * g * g:(b + 1) * g * g], W["w_patch"], residual=W["pos_patches"], out_f32=x[b, 1:])
         _, x = ops.layernorm(x.view(B * n, h), *W["ln_pre"], eps=eps, want_f32=True)
-        for L in W["layers"]:
-            y = ops.layernorm(x, *L["ln1"], eps=eps)
-            qk, _ = ops.gemm(y, L["w_qk"], bias=L["b_qk"], want_f16=True)
-            v, _ = ops.gemm(y, L["w_v"], want_f16=True)
-            qk3 = qk.view(B, n, 2 * h)
-            vt = ops.transpose_f16(v.view(B, n, h))
-            o = ops.attention(qk3[:, :, :h], qk3[:, :, h:], vt, heads=heads, d=d, dpad=d, nq=n, nkv=n, scale=d ** -0.5)
-            _, x = ops.gemm(o.view(-1, h), L["w_o"], bias=L["b_o"], residual=x, want_f32=True)
-            y = ops.layernorm(x, *L["ln2"], eps=eps)
-            gq, _ = ops.gemm(y, L["w_fc1"], bias=L["b_fc1"], act=ACT_QUICK_GELU, want_f16=True)
-            _, x = ops.gemm(gq, L["w_fc2"], bias=L["b_fc2"], residual=x, want_f32=True)
+        x = encoder_layers(x, W["layers"], B, heads=heads, d=d, eps=eps, act=ACT_QUICK_GELU)
         cls = torch.empty((B, h), dtype=torch.float32, device=pix.device)
         xv = x.view(B, n, h)
         for b in range(B):

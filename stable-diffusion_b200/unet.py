@@ -19,12 +19,11 @@ from __future__ import annotations
 import math
 
 import torch
-import torch.nn as nn
 
 from . import ops
 from .arch import unet_param_shapes, unet_plan
 from .ops import ACT_GEGLU, ACT_SILU
-from .util import adopt_state_dict
+from .util import PackedStage
 
 
 def _dpad(d):
@@ -88,7 +87,7 @@ def _pack_geglu(w, b):  # [8C, C]: rows [0,4C) value, [4C,8C) gate -> per accumu
     return w[perm].contiguous().half(), b[perm].contiguous().float()
 
 
-class UNetModel(nn.Module):
+class UNetModel(PackedStage):
     # "fp16x3": the 1x1 convs that act on the raw residual stream (ResBlock skip_connection, SpatialTransformer
     # proj_in / proj_out) and the final 320->4 conv run with hi/lo-split fp16 operands (three tensor-core passes,
     # ~fp32 operand precision); everything else single-pass fp16. These few layers (5% of the FLOPs) carry ~60% of the
@@ -147,7 +146,6 @@ class UNetModel(nn.Module):
             # entries must also divide the GEMM tile widths (the GEMM drops the fused statistics otherwise): 192
             # channels -> 6 per group -> entries of 2; SD-v1's 10 divides the 160-wide tiles
             self._sg = math.gcd(self._sg, 16)
-        self.W = None           # packed weights (device)
         self._ctx_ref = None    # the context tensor whose cross-attention K/V are cached (strong reference)
         self._ctx_ver = -1
         self._ctx_kv = None
@@ -162,36 +160,9 @@ class UNetModel(nn.Module):
         self.autotune = True          # graph mode: pick (block_n, split-K) per GEMM problem by measurement before capture
 
     # ------------------------------------------------------------------ weights
-    def _load_from_state_dict(self, state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
-                              error_msgs):
-        sd = adopt_state_dict(self, state_dict, prefix, missing_keys, unexpected_keys, error_msgs)
-        if sd is None:
-            return
-        self._host_sd = sd
-        if self.W is not None:
-            self.pack_weights(self.W["device"])
-
-    def load_weights(self, sd, device):
-        """sd: UNetModel.state_dict()-style mapping (reference key names). Packs to kernel-native fp16 layouts."""
-        for k, shape in self.shapes.items():
-            assert k in sd, f"missing key {k}"
-            assert tuple(sd[k].shape) == tuple(shape), (k, tuple(sd[k].shape), shape)
-        self._host_sd = {k: sd[k] for k in self.shapes}
-        self.pack_weights(torch.device(device))
-        return self
-
-    def _apply(self, fn, *a, **k):  # .cuda()/.to(device) triggers packing, like moving an nn.Module's parameters
-        r = super()._apply(fn, *a, **k)
-        probe = fn(torch.empty(0))
-        if probe.is_cuda and getattr(self, "_host_sd", None) is not None and (self.W is None or self.W["device"] != probe.device):
-            self.pack_weights(probe.device)
-        return r
-
     def set_weight_set(self, name, sd):
         """Register another state dict of this architecture (UNetModel keys) under `name`, e.g. the EMA weights."""
-        for k, shape in self.shapes.items():
-            assert k in sd and tuple(sd[k].shape) == tuple(shape), f"weight set {name}: {k} missing or misshapen"
-        self._alt_sd[name] = {k: sd[k] for k in self.shapes}
+        self._alt_sd[name] = self._checked(sd, f"weight set {name}")
         self._packed.pop(name, None)
 
     def has_weight_set(self, name):

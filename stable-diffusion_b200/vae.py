@@ -8,12 +8,11 @@ model.py:178-202) runs in the d = 512 flash kernel (sdb_attention, dpad 512; oth
 from __future__ import annotations
 
 import torch
-import torch.nn as nn
 
 from . import ops
 from .arch import vae_param_shapes
 from .unet import _pack_conv3, _pack_conv3_padk
-from .util import adopt_state_dict
+from .util import PackedStage
 
 
 def _sg(c):
@@ -51,41 +50,18 @@ class DiagonalGaussianDistribution:
         return self.mean
 
 
-class ConvAutoencoder(nn.Module):
-    """The Encoder / Decoder of model.py:368-568 (attention in the mid block only) and the weight plumbing shared by the
+class ConvAutoencoder(PackedStage):
+    """The Encoder / Decoder of model.py:368-568 (attention in the mid block only) and the weight packing shared by the
     first stages: AutoencoderKL below and VQModelInterface (vq.py). Both have a quant_conv and a post_quant_conv (1x1,
     <= 16 channels, fp32), packed here; a subclass sets `shapes` and packs anything else it has (the codebook)."""
+
+    drop_prefixes = ("loss.",)   # the training loss's tensors
 
     def __init__(self, shapes):
         super().__init__()
         self.shapes = shapes
-        self.W = None
-        self._host_sd = None
 
     # ------------------------------------------------------------------ weights
-    def _load_from_state_dict(self, state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
-                              error_msgs):
-        sd = adopt_state_dict(self, state_dict, prefix, missing_keys, unexpected_keys, error_msgs, ignore=("loss.",))
-        if sd is None:
-            return
-        self._host_sd = sd
-        if self.W is not None:
-            self.pack_weights(self.W["device"])
-
-    def load_weights(self, sd, device):
-        for k, shape in self.shapes.items():
-            assert k in sd and tuple(sd[k].shape) == tuple(shape), k
-        self._host_sd = {k: sd[k] for k in self.shapes}
-        self.pack_weights(torch.device(device))
-        return self
-
-    def _apply(self, fn, *a, **k):
-        r = super()._apply(fn, *a, **k)
-        probe = fn(torch.empty(0))
-        if probe.is_cuda and self._host_sd is not None and (self.W is None or self.W["device"] != probe.device):
-            self.pack_weights(probe.device)
-        return r
-
     @torch.no_grad()
     def pack_weights(self, device):
         sd = {k: v.detach().to(device=device, dtype=torch.float32) for k, v in self._host_sd.items()}
