@@ -71,6 +71,27 @@ TINY_CIN_UNET = dict(image_size=16, in_channels=3, out_channels=3, model_channel
                      num_res_blocks=1, channel_mult=[1, 6, 15], num_heads=1, use_spatial_transformer=True,
                      transformer_depth=1, context_dim=64)
 TINY_CIN_COND = dict(embed_dim=64, n_classes=1001, key="class_label")
+# the class-conditional ImageNet LDM-VQ-8 (models/ldm/cin256/config.yaml, configs/latent-diffusion/cin-ldm-vq-f8.yaml):
+# spatial transformers with heads of num_head_channels 32 (8 / 16 / 32 heads at widths 256 / 512 / 1024) at every level
+# of a 32x32x4 latent, cross-attention on a one-token ClassEmbedder context. n_classes stays at the reference default
+# 1000, so this model has no unconditional label. The VQ-f8 first stage has AttnBlocks inside its 32x32 level (512 wide)
+# as well as in the mid block.
+CIN256_F8_UNET = dict(image_size=32, in_channels=4, out_channels=4, model_channels=256, attention_resolutions=[4, 2, 1],
+                      num_res_blocks=2, channel_mult=[1, 2, 4], num_head_channels=32, use_spatial_transformer=True,
+                      transformer_depth=1, context_dim=512)
+CIN256_F8_COND = dict(embed_dim=512, n_classes=1000, key="class_label")
+VQ_F8 = dict(embed_dim=4, n_embed=16384, ddconfig=dict(double_z=False, z_channels=4, resolution=256, in_channels=3, out_ch=3,
+                                                        ch=128, ch_mult=[1, 2, 2, 4], num_res_blocks=2, attn_resolutions=[32],
+                                                        dropout=0.0))
+# small members for tests: 2 / 4 heads of d = 32 at two levels and in the middle block; a four-level (f8) first stage
+# with level attention at 32x32 (128 wide: the per-image GEMM path) and at 8x8 (512 wide: the d = 512 flash kernel)
+TINY_CIN_F8_UNET = dict(image_size=16, in_channels=4, out_channels=4, model_channels=64, attention_resolutions=[1, 2],
+                        num_res_blocks=1, channel_mult=[1, 2], num_head_channels=32, use_spatial_transformer=True,
+                        transformer_depth=1, context_dim=64)
+TINY_CIN_F8_COND = dict(embed_dim=64, n_classes=1000, key="class_label")
+TINY_VQ_F8 = dict(embed_dim=4, n_embed=512, ddconfig=dict(double_z=False, z_channels=4, resolution=64, in_channels=3,
+                                                          out_ch=3, ch=64, ch_mult=[1, 2, 2, 8], num_res_blocks=1,
+                                                          attn_resolutions=[32, 8], dropout=0.0))
 # VQModelInterface first stages (models/first_stage_models/vq-f4/config.yaml) and a small member
 VQ_F4 = dict(embed_dim=3, n_embed=8192, ddconfig=dict(double_z=False, z_channels=3, resolution=256, in_channels=3, out_ch=3,
                                                        ch=128, ch_mult=[1, 2, 4], num_res_blocks=2, attn_resolutions=[],
@@ -314,31 +335,41 @@ def _attn_shapes(p, pre, c):
 
 def vae_param_shapes(cfg):
     """Keys as AutoencoderKL.state_dict() (encoder.*, decoder.*, quant_conv.*, post_quant_conv.*) — 248 tensors.
-    ddconfig.attn_type "none" (make_attn, model.py:205-211: nn.Identity) drops the mid-block attention keys."""
+    ddconfig.attn_type "none" (make_attn, model.py:205-211: nn.Identity) drops the mid-block attention keys.
+    A level whose resolution (ddconfig.resolution halved per level, independent of the input size) is in
+    attn_resolutions has one AttnBlock per ResnetBlock (`encoder.down.{l}.attn.{b}`, `decoder.up.{l}.attn.{b}`)."""
     dd = cfg["ddconfig"]
     ch, mult, nrb = dd["ch"], dd["ch_mult"], dd["num_res_blocks"]
     zc = dd["z_channels"]
-    assert not dd["attn_resolutions"], "SD v1 VAE has attention only in the mid block"
+    attn_res = set(dd["attn_resolutions"])
     attn_type = dd.get("attn_type", "vanilla")
     if attn_type == "linear":
         raise NotImplementedError("ddconfig attn_type 'linear' (LinAttnBlock) is not supported")
     assert attn_type in ("vanilla", "none"), f"attn_type {attn_type} unknown"
     mid_attn = attn_type == "vanilla"
+    if not mid_attn:        # every make_attn is nn.Identity: no level attention keys either
+        attn_res = set()
     p = OrderedDict()
     # encoder (model.py:368-432)
     p["encoder.conv_in.weight"] = (ch, dd["in_channels"], 3, 3)
     p["encoder.conv_in.bias"] = (ch,)
     in_mult = [1] + list(mult)
     bi = ch
+    res = dd["resolution"]
     for lvl in range(len(mult)):
         bi = ch * in_mult[lvl]
         bo = ch * mult[lvl]
+        attn = OrderedDict()
         for b in range(nrb):
             _resnet_shapes(p, f"encoder.down.{lvl}.block.{b}", bi, bo)
             bi = bo
+            if res in attn_res:
+                _attn_shapes(attn, f"encoder.down.{lvl}.attn.{b}", bo)
+        p.update(attn)                  # the level's `attn` ModuleList is registered after its `block` list
         if lvl != len(mult) - 1:
             p[f"encoder.down.{lvl}.downsample.conv.weight"] = (bi, bi, 3, 3)
             p[f"encoder.down.{lvl}.downsample.conv.bias"] = (bi,)
+            res //= 2
     _resnet_shapes(p, "encoder.mid.block_1", bi, bi)
     if mid_attn:
         _attn_shapes(p, "encoder.mid.attn_1", bi)
@@ -357,15 +388,20 @@ def vae_param_shapes(cfg):
         _attn_shapes(p, "decoder.mid.attn_1", bi)
     _resnet_shapes(p, "decoder.mid.block_2", bi, bi)
     ups = OrderedDict()
+    res = dd["resolution"] // 2 ** (len(mult) - 1)
     for lvl in reversed(range(len(mult))):
-        q = OrderedDict()
+        q, attn = OrderedDict(), OrderedDict()
         bo = ch * mult[lvl]
         for b in range(nrb + 1):
             _resnet_shapes(q, f"decoder.up.{lvl}.block.{b}", bi, bo)
             bi = bo
+            if res in attn_res:
+                _attn_shapes(attn, f"decoder.up.{lvl}.attn.{b}", bo)
+        q.update(attn)
         if lvl != 0:
             q[f"decoder.up.{lvl}.upsample.conv.weight"] = (bi, bi, 3, 3)
             q[f"decoder.up.{lvl}.upsample.conv.bias"] = (bi,)
+            res *= 2
         ups[lvl] = q
     for lvl in range(len(mult)):
         p.update(ups[lvl])

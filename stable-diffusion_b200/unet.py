@@ -2,7 +2,8 @@
 reference's `ldm.modules.diffusionmodules.openaimodel.UNetModel` (constructor kwargs openaimodel.py:443-469,
 `forward(x, timesteps, context)` openaimodel.py:710-742, state-dict keys unchanged).
 
-Two members of the reference's UNet family run: the SD-v1 spatial-transformer UNet (cross-attention on a context), and
+Two members of the reference's UNet family run: the SD-v1 spatial-transformer UNet (cross-attention on a context, with
+num_heads heads, or heads of num_head_channels as in the cin256 LDM-VQ-8), and
 the unconditional AttentionBlock UNet (use_spatial_transformer=False, e.g. LSUN-Churches) with any combination of
 use_scale_shift_norm and resblock_updown, or with plain ResBlocks and heads of num_head_channels (the VQ-f4 models).
 
@@ -110,10 +111,13 @@ class UNetModel(PackedStage):
             assert num_head_channels != -1, "Either num_heads or num_head_channels has to be set"
         # the sdb200 path covers the configuration SD v1 ships (v1-inference.yaml:29-44) and the unconditional
         # AttentionBlock family (models/ldm/lsun_churches256/config.yaml: scale-shift norm, up/down ResBlocks;
-        # configs/latent-diffusion/*-ldm-vq-4.yaml: plain ResBlocks with num_head_channels)
+        # configs/latent-diffusion/*-ldm-vq-4.yaml: plain ResBlocks with num_head_channels). Spatial transformers take
+        # num_head_channels when it alone sets the heads (models/ldm/cin256: num_heads left at -1); the reference
+        # silently ignores num_heads when both are given, so that combination is rejected.
         plain = not (use_spatial_transformer or use_scale_shift_norm or resblock_updown)
+        st_nhc = use_spatial_transformer and num_heads == -1
         unsupported = dict(dims=dims != 2, num_classes=num_classes is not None, n_embed=n_embed is not None,
-                           num_head_channels=num_head_channels != -1 and not plain, dropout=dropout != 0,
+                           num_head_channels=num_head_channels != -1 and not (plain or st_nhc), dropout=dropout != 0,
                            conv_resample=not conv_resample, use_new_attention_order=bool(use_new_attention_order),
                            num_heads_upsample=num_heads_upsample not in (-1, num_heads))
         if use_spatial_transformer:
@@ -199,7 +203,6 @@ class UNetModel(PackedStage):
         x3 = self.precision == "fp16x3"
         W["x3"] = x3
         one = (lambda w: _pack_hilo_1x1(w)) if x3 else (lambda w: w.half().contiguous())
-        heads = self.num_heads
         mc = self.model_channels
         W["te0_w"], W["te0_b"] = f16("time_embed.0.weight"), f32("time_embed.0.bias")
         W["te2_w"], W["te2_b"] = f16("time_embed.2.weight"), f32("time_embed.2.bias")
@@ -243,10 +246,11 @@ class UNetModel(PackedStage):
             return s
 
         def pack_st(pre, a):
+            """SpatialTransformer with the plan's heads of dhead channels (num_heads, or ch / num_head_channels)."""
             ch, d = a["ch"], a["dhead"]
             dp = _dpad(d)
             tb = pre + ".transformer_blocks.0"
-            s = {"ch": ch, "d": d, "dpad": dp, "heads": heads, "tb": tb}
+            s = {"ch": ch, "d": d, "dpad": dp, "heads": a["heads"], "tb": tb}
             s["gn"] = (f32(pre + ".norm.weight"), f32(pre + ".norm.bias"))
             s["w_in"], s["b_in"] = one(sd[pre + ".proj_in.weight"].reshape(ch, ch)), f32(pre + ".proj_in.bias")
             s["w_out"], s["b_out"] = one(sd[pre + ".proj_out.weight"].reshape(ch, ch)), f32(pre + ".proj_out.bias")

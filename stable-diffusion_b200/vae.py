@@ -51,9 +51,10 @@ class DiagonalGaussianDistribution:
 
 
 class ConvAutoencoder(PackedStage):
-    """The Encoder / Decoder of model.py:368-568 (attention in the mid block only) and the weight packing shared by the
-    first stages: AutoencoderKL below and VQModelInterface (vq.py). Both have a quant_conv and a post_quant_conv (1x1,
-    <= 16 channels, fp32), packed here; a subclass sets `shapes` and packs anything else it has (the codebook)."""
+    """The Encoder / Decoder of model.py:368-568 (attention in the mid block, and inside the levels at attn_resolutions)
+    and the weight packing shared by the first stages: AutoencoderKL below and VQModelInterface (vq.py). Both have a
+    quant_conv and a post_quant_conv (1x1, <= 16 channels, fp32), packed here; a subclass sets `shapes` and packs
+    anything else it has (the codebook)."""
 
     drop_prefixes = ("loss.",)   # the training loss's tensors
 
@@ -98,13 +99,15 @@ class ConvAutoencoder(PackedStage):
             out = []
             lvl = 0
             while f"{pre}.{lvl}.block.0.norm1.weight" in sd:
-                blocks = []
+                blocks, attns = [], []
                 b = 0
                 while f"{pre}.{lvl}.block.{b}.norm1.weight" in sd:
                     blocks.append(resnet(f"{pre}.{lvl}.block.{b}"))
+                    # a level at one of attn_resolutions has an AttnBlock after each ResnetBlock
+                    attns.append(attn(f"{pre}.{lvl}.attn.{b}") if f"{pre}.{lvl}.attn.{b}.q.weight" in sd else None)
                     b += 1
                 rs = conv3(f"{pre}.{lvl}.{kind}.conv") if f"{pre}.{lvl}.{kind}.conv.weight" in sd else None
-                out.append({"blocks": blocks, "resample": rs})
+                out.append({"blocks": list(zip(blocks, attns)), "resample": rs})
                 lvl += 1
             return out
 
@@ -194,6 +197,15 @@ class ConvAutoencoder(PackedStage):
                           rows_per_sample=n, want_stats=True, stats_group=_sg(c))
         return out.view(nb, H, Wd, c)
 
+    def _level_blocks(self, lvl, h):
+        """The ResnetBlocks of one Encoder / Decoder level, each followed by its AttnBlock where the level has them
+        (model.py:446-449, 557-560)."""
+        for r, a in lvl["blocks"]:
+            h = self._resnet(r, h)
+            if a is not None:
+                h = self._attn(a, h)
+        return h
+
     def _decoder(self, h):
         """Decoder.forward (model.py:535-568) on the fp32 NHWC output of post_quant_conv; returns fp32 NHWC."""
         D = self.W["decoder"]
@@ -203,8 +215,7 @@ class ConvAutoencoder(PackedStage):
             h = self._attn(D["attn"], h)
         h = self._resnet(D["mid2"], h)
         for lvl in reversed(D["levels"]):
-            for r in lvl["blocks"]:
-                h = self._resnet(r, h)
+            h = self._level_blocks(lvl, h)
             if lvl["resample"] is not None:   # Upsample: nearest 2x + conv (model.py:42-57)
                 h = self._conv3(lvl["resample"], x16=ops.upsample2x(h))
         hn, _ = ops.groupnorm(h, *D["gn_out"], eps=1e-6, silu=True)
@@ -216,8 +227,7 @@ class ConvAutoencoder(PackedStage):
         xh, _ = ops.nchw_to_nhwc(x.contiguous().float())
         h = self._conv3(E["conv_in"], x32=xh)
         for lvl in E["levels"]:
-            for r in lvl["blocks"]:
-                h = self._resnet(r, h)
+            h = self._level_blocks(lvl, h)
             if lvl["resample"] is not None:   # Downsample: pad (0,1,0,1) + conv stride 2 pad 0 (model.py:60-79)
                 # straight from the NHWC activation through strided TMA boxes (conv_shift 1 = pad right / bottom only)
                 nb, H, Wd, c = h.shape

@@ -3,7 +3,8 @@
 no remap). State-dict keys unchanged (`encoder.*`, `decoder.*`, `quantize.embedding.weight`, `quant_conv.*`,
 `post_quant_conv.*`); the loss is training-only and its keys are ignored.
 
-The Encoder / Decoder are the AutoencoderKL ones (vae.ConvAutoencoder). The quantizer is one kernel (sdb_vq_quantize):
+The Encoder / Decoder are the AutoencoderKL ones (vae.ConvAutoencoder), including AttnBlocks inside the levels at
+ddconfig.attn_resolutions (VQ-f8: one per ResnetBlock of the 32x32 level). The quantizer is one kernel (sdb_vq_quantize):
 nearest codebook entry by sum(z^2) + sum(e^2) - 2 z.e with the lowest index winning ties, and the straight-through
 value z + (e - z) in fp32, as the reference computes it. sum(e^2) is computed once per weight load.
 """
@@ -26,7 +27,6 @@ class VQModelInterface(ConvAutoencoder):
             raise NotImplementedError("sdb200.VQModelInterface: remap, sane_index_shape and use_ema are not supported")
         assert n_embed is not None, "n_embed is required"
         assert not ddconfig["double_z"], "VQ first stages have double_z False"
-        assert not ddconfig.get("attn_resolutions"), "attention only in the mid block"
         cfg = dict(embed_dim=embed_dim, n_embed=n_embed, ddconfig=dict(ddconfig))
         super().__init__(vq_param_shapes(cfg))
         self.cfg = cfg
