@@ -320,13 +320,26 @@ int sdb_spatial_rescale(const float* x_nchw, int32_t nb, int32_t cin, int32_t h,
  * its window, ascending. Bit-identical to sdb_spatial_rescale on the one-hot. The channel map (weight) is required. */
 int sdb_seg_labels_rescale(const uint8_t* labels, int32_t nb, int32_t cin, int32_t h, int32_t w, int32_t n_stages,
                            const float* weight, const float* bias, int32_t cout, float* out_nchw, sdb_stream_t stream);
+/* Exact top-k by inner product (knn.cu; the score_brute_force searcher of scripts/knn2img.py): db fp16 [n, dim]
+ * row-major (n < 2^31), queries fp16 [b, dim]; dim a multiple of 64, <= 768; 1 <= b <= 64; 1 <= k <= min(64, n).
+ * out_score fp32 [b, k] and out_idx int64 [b, k] hold each query's k best rows by fp32 dot product, score descending,
+ * the lower row first on equal scores. Two launches: per-CTA candidate lists into the workspace (ws_score fp32 and
+ * ws_idx int32, ws_entries >= sdb_knn_workspace(n, b, k) each), then their merge. Deterministic, no atomics. */
+int64_t sdb_knn_workspace(int64_t n, int32_t b, int32_t k);
+int sdb_knn_topk(const void* db, int64_t n, int32_t dim, const void* queries, int32_t b, int32_t k, float* ws_score,
+                 int32_t* ws_idx, int64_t ws_entries, float* out_score, int64_t* out_idx, sdb_stream_t stream);
+/* Row pooling of CLIP's text embedding (FrozenCLIPTextEmbedder): out fp32 [b, dim] = x fp32 row
+ * b * n_ctx + argmax(ids[b, :n_ctx]) (the EOT token; the first maximum) when ids (int64 [b, n_ctx]) is given, else
+ * row b; normalize != 0 divides each row by its L2 norm in fp32. */
+int sdb_rows_pool(const float* x, const int64_t* ids, int32_t b, int32_t n_ctx, int32_t dim, int32_t normalize,
+                  float* out, sdb_stream_t stream);
 /* out = a*x + b (latent scaling z/0.18215, ddpm.py:713) */
 int sdb_axpby(const float* x, float a, float b, int64_t n, float* out, sdb_stream_t stream);
 /* out = a*x + b*y (DDIMSampler.stochastic_encode, ddim.py:206-220; q_sample, ddpm.py:274-277) */
 int sdb_axpby2(const float* x, const float* y, float a, float b, int64_t n, float* out, sdb_stream_t stream);
 
-/* 1x1 conv with <= 16 channels in fp32 (post_quant_conv 4->4 with the 1/scale_factor folded in as alpha,
- * quant_conv 8->8; autoencoder.py:302-303,326,331): out[p, j] = sum_c (alpha x[p, c]) w[j, c] + b[j] */
+/* 1x1 conv with <= 32 channels in fp32 (post_quant_conv 4->4 with the 1/scale_factor folded in as alpha,
+ * quant_conv 8->8, KL-f16's 32->32; autoencoder.py:302-303,326,331): out[p, j] = sum_c (alpha x[p, c]) w[j, c] + b[j] */
 int sdb_pointwise_small(const float* x, int64_t npix, int32_t cin, int32_t cout, const float* w, const float* b,
                         float alpha, float* out, sdb_stream_t stream);
 /* CLIP token + position embedding gather (transformers CLIPTextEmbeddings): ids int64 [rows] -> fp32 [rows, dim] */

@@ -144,6 +144,27 @@ LAION_BERT = dict(n_embed=1280, n_layer=32, vocab_size=30522, max_seq_len=77)
 # small members for tests: the attention's inner width stays 8 x 64 = 512
 TINY_BERT = dict(n_embed=128, n_layer=2, vocab_size=1000, max_seq_len=77)
 TINY_LAION_UNET = dict(TINY_UNET, context_dim=128)
+# the retrieval-augmented diffusion model (configs/retrieval-augmented-diffusion/768x768.yaml, scripts/knn2img.py): a
+# 48x48x16 latent, spatial transformers with heads of num_head_channels 32 (14 / 28 / 42 heads at widths 448 / 896 /
+# 1344, 56 in the middle block) cross-attending to CLIP ViT-L/14's projected text embedding and its retrieved
+# neighbours (768 wide, 1 + k tokens); a KL-f16 first stage (16 latent channels, five levels, AttnBlocks at 16x16).
+RDM_UNET = dict(image_size=48, in_channels=16, out_channels=16, model_channels=448, attention_resolutions=[4, 2, 1],
+                num_res_blocks=2, channel_mult=[1, 2, 3, 4], use_scale_shift_norm=False, resblock_updown=False,
+                num_head_channels=32, use_spatial_transformer=True, transformer_depth=1, context_dim=768,
+                use_checkpoint=True)
+KL_F16 = dict(embed_dim=16, ddconfig=dict(double_z=True, z_channels=16, resolution=256, in_channels=3, out_ch=3, ch=128,
+                                          ch_mult=[1, 1, 2, 2, 4], num_res_blocks=2, attn_resolutions=[16], dropout=0.0))
+# FrozenCLIPTextEmbedder: the CLIP text tower with the text projection (transformers CLIPModel's text_projection)
+CLIP_TEXT_PROJ = dict(SD_V1_CLIP, projection_dim=768)
+# small members for tests: 2 / 4 heads of d = 32; a five-level (f16) KL first stage with level attention at 16x16 (128
+# wide: the per-image path) and at 4x4 (512 wide: the d = 512 flash kernel); a 64-wide projected tiny CLIP
+TINY_RDM_UNET = dict(image_size=16, in_channels=16, out_channels=16, model_channels=64, attention_resolutions=[1, 2],
+                     num_res_blocks=1, channel_mult=[1, 2], num_head_channels=32, use_spatial_transformer=True,
+                     transformer_depth=1, context_dim=64)
+TINY_KL_F16 = dict(embed_dim=16, ddconfig=dict(double_z=True, z_channels=16, resolution=64, in_channels=3, out_ch=3,
+                                               ch=64, ch_mult=[1, 1, 2, 2, 8], num_res_blocks=1,
+                                               attn_resolutions=[16, 4], dropout=0.0))
+TINY_CLIP_TEXT_PROJ = dict(TINY_CLIP, projection_dim=64)
 
 
 # ------------------------------------------------------------------------------------------------ UNet
@@ -473,6 +494,14 @@ def clip_param_shapes(cfg):
         p[f"{pre}.layer_norm2.bias"] = (h,)
     p["text_model.final_layer_norm.weight"] = (h,)
     p["text_model.final_layer_norm.bias"] = (h,)
+    return p
+
+
+def clip_text_proj_param_shapes(cfg):
+    """The text half of transformers CLIPModel.state_dict(): `text_model.*` and `text_projection.weight`
+    [projection_dim, hidden] (no bias), for FrozenCLIPTextEmbedder."""
+    p = clip_param_shapes(cfg)
+    p["text_projection.weight"] = (cfg["projection_dim"], cfg["hidden_size"])
     return p
 
 

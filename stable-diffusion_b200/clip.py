@@ -19,7 +19,7 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .arch import SD_V1_CLIP, clip_param_shapes
+from .arch import CLIP_TEXT_PROJ, SD_V1_CLIP, clip_param_shapes, clip_text_proj_param_shapes
 from .ops import ACT_QUICK_GELU
 from .util import PackedStage
 
@@ -162,3 +162,70 @@ class FrozenCLIPEmbedder(PackedStage):
 
     def encode(self, text):
         return self(text)
+
+
+class FrozenCLIPTextEmbedder(FrozenCLIPEmbedder):
+    """Drop-in for `ldm.modules.encoders.modules.FrozenCLIPTextEmbedder` (modules.py:165-194), the text encoder of the
+    retrieval-augmented model (scripts/knn2img.py): `encode(text) -> (B, 1, projection_dim)`, CLIP's `encode_text`
+    (the text tower above, the final LayerNorm, the row at the EOT token, `@ text_projection`) divided by its L2 norm.
+
+    Weights are read in the transformers `CLIPModel` layout of the same ViT-L/14 checkpoint: `text_model.*` and
+    `text_projection.weight`; the vision tower's keys are ignored. Prompts are tokenized as `clip.tokenize`: BOS +
+    tokens + EOT, zero padding, and an error for prompts longer than max_length tokens. `version` is a directory with
+    the CLIP vocab.json + merges.txt (or `tokenizer` a CLIPBPETokenizer). n_repeat copies the embedding along the token
+    axis, as the reference's encode (knn2img.py keeps 1)."""
+
+    drop_prefixes = FrozenCLIPEmbedder.drop_prefixes + ("vision_model.", "visual_projection.", "logit_scale")
+    _load_from_state_dict = PackedStage._load_from_state_dict   # the keys sit at this level: no `transformer.` shim
+
+    def __init__(self, version="ViT-L/14", device="cuda", max_length=77, n_repeat=1, normalize=True, config=None,
+                 tokenizer=None):
+        super().__init__(version=version, device=device, max_length=max_length, config=config or CLIP_TEXT_PROJ)
+        del self.transformer
+        self.shapes = clip_text_proj_param_shapes(self.cfg)
+        self.n_repeat, self.normalize = n_repeat, normalize
+        self.tokenizer = tokenizer
+
+    @torch.no_grad()
+    def pack_weights(self, device):
+        super().pack_weights(device)
+        self.W["proj"] = self._host_sd["text_projection.weight"].to(device=device, dtype=torch.float16).contiguous()
+
+    def tokenize(self, text):
+        """list[str] -> int64 [B, max_length] as `clip.tokenize(text)` (truncate=False)."""
+        if self.tokenizer is None:
+            from .tokenizer import CLIPBPETokenizer
+            if not os.path.exists(os.path.join(str(self.version), "vocab.json")):
+                raise RuntimeError(f"CLIP vocabulary not found: pass a directory with vocab.json + merges.txt as "
+                                   f"`version` (got {self.version!r}), or token ids to encode_ids()")
+            self.tokenizer = CLIPBPETokenizer.from_dir(str(self.version), self.max_length)
+        tok = self.tokenizer
+        if isinstance(text, str):
+            text = [text]
+        ids = torch.zeros((len(text), self.max_length), dtype=torch.long)
+        for i, t in enumerate(text):
+            row = [tok.bos_id] + tok.tokenize_ids(t) + [tok.eos_id]
+            if len(row) > self.max_length:
+                raise RuntimeError(f"Input {t} is too long for context length {self.max_length}")
+            ids[i, :len(row)] = torch.tensor(row)
+        return ids
+
+    @torch.no_grad()
+    def encode_ids(self, ids):
+        """ids: int64 [B, n] on the GPU, EOT = the largest id of each row -> fp32 [B, projection_dim], normalised when
+        `normalize` (the reference's forward)."""
+        ids = ids.contiguous()
+        h = super().encode_ids(ids)                                                     # [B, n, hidden], final LN
+        pooled = ops.rows_pool(h.view(-1, h.shape[-1]), ids)                           # the EOT rows
+        z = ops.linear_small(pooled, self.W["proj"])
+        return ops.rows_pool(z, normalize=True) if self.normalize else z
+
+    def forward(self, text):
+        ids = text if torch.is_tensor(text) else self.tokenize(text)
+        return self.encode_ids(ids.to(self.W["device"]).long())
+
+    def encode(self, text):
+        z = self(text)
+        if z.ndim == 2:
+            z = z[:, None, :]
+        return z.expand(-1, self.n_repeat, -1).contiguous() if self.n_repeat != 1 else z

@@ -472,7 +472,7 @@ extern "C" int sdb_axpby(const float* x, float a, float b, int64_t n, float* out
 extern "C" int sdb_pointwise_small(const float* x, int64_t npix, int32_t cin, int32_t cout, const float* w,
                                    const float* b, float alpha, float* out, sdb_stream_t stream) {
   SDB_REC(sdb_pointwise_small(x, npix, cin, cout, w, b, alpha, out, s_));
-  SDB_CHECK(x && w && out && cin > 0 && cin <= 16 && cout > 0 && cout <= 16, "sdb_pointwise_small: bad arguments");
+  SDB_CHECK(x && w && out && cin > 0 && cin <= 32 && cout > 0 && cout <= 32,"sdb_pointwise_small: bad arguments");
   pointwise_small_kernel<<<grid_for(static_cast<size_t>(npix) * cout), 256, 0, ST>>>(
       x, static_cast<size_t>(npix), cin, cout, w, b, alpha, out);
   SDB_LAUNCH_CHECK();

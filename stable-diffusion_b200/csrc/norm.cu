@@ -10,7 +10,8 @@
 namespace sdb {
 
 constexpr int GN_THREADS = 256;
-constexpr int GN_MAX_CPT = 12;  // channels per thread: C <= 3072
+constexpr int GN_CPT = 12;      // channels per thread of the statistics pass: C <= 3072
+constexpr int GN_MAX_CPT = 14;  // C <= 3584 (the retrieval-augmented UNet's widest skip concat) takes a 14-channel variant
 
 constexpr int GN_MAX_SLABS = 128;
 
@@ -19,6 +20,7 @@ constexpr int GN_MAX_SLABS = 128;
 // thread. Per-channel partials are combined in shared memory, reduced per group by one warp each and written as
 // per-block partials (no contended atomics); the last block of each sample (ticket counter) folds the partials in
 // fp64 and publishes mean / rstd.
+template <int CPT>
 __global__ void __launch_bounds__(GN_THREADS)
     gn_stats_kernel(const float* __restrict__ x0, const float* __restrict__ x1, int c0, int c1, int hw, int groups,
                     int rows_per_block, int cw, float eps, float* __restrict__ partial,
@@ -38,13 +40,13 @@ __global__ void __launch_bounds__(GN_THREADS)
   const int tc = threadIdx.x % cw;
   const int tr = threadIdx.x / cw;
   const int rstep = GN_THREADS / cw;
-  float s[GN_MAX_CPT], q[GN_MAX_CPT];
+  float s[CPT], q[CPT];
 #pragma unroll
-  for (int j = 0; j < GN_MAX_CPT; ++j) s[j] = q[j] = 0.f;
+  for (int j = 0; j < CPT; ++j) s[j] = q[j] = 0.f;
   const size_t base = static_cast<size_t>(n) * hw;
   for (int r = r0 + tr; r < r1; r += 4 * rstep) {
 #pragma unroll
-    for (int j = 0; j < GN_MAX_CPT; ++j) {
+    for (int j = 0; j < CPT; ++j) {
       const int c = tc + j * cw;
       if (c < C) {
         float v[4];
@@ -63,7 +65,7 @@ __global__ void __launch_bounds__(GN_THREADS)
     }
   }
 #pragma unroll
-  for (int j = 0; j < GN_MAX_CPT; ++j) {
+  for (int j = 0; j < CPT; ++j) {
     int c = tc + j * cw;
     if (c < C) {
       if (rstep == 1) {
@@ -543,7 +545,7 @@ extern "C" int sdb_groupnorm(const float* x0, const float* x1, int32_t c0, int32
   slabs = (hw + rows_per_block - 1) / rows_per_block;
   dim3 grid(slabs, nb);
   if (!fused_stats) {
-    gn_stats_kernel<<<grid, GN_THREADS, 2 * C * sizeof(float), st>>>(x0, x1, c0, c1, hw, groups, rows_per_block, cw,
+    (C > GN_THREADS * GN_CPT ? gn_stats_kernel<GN_MAX_CPT> : gn_stats_kernel<GN_CPT>)<<<grid, GN_THREADS, 2 * C * sizeof(float), st>>>(x0, x1, c0, c1, hw, groups, rows_per_block, cw,
                                                                       eps, partial, counter, meanrstd);
     SDB_LAUNCH_CHECK();
   }
@@ -578,7 +580,7 @@ extern "C" int sdb_layernorm(const float* x, int32_t rows, int32_t c, const floa
   SDB_REC(sdb_layernorm(x, rows, c, gamma, beta, eps, out_f16, out_f32, s_));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   SDB_CHECK(x && gamma && beta && (out_f16 || out_f32), "sdb_layernorm: null pointer");
-  SDB_CHECK(c <= 32 * 48, "sdb_layernorm: C=%d too large", c);
+  SDB_CHECK(c <= 32 * 56, "sdb_layernorm: C=%d too large", c);
   // one warp per row; fewer warps per block at small row counts so the grid still covers the machine
   int warps_per_block = rows >= 8 * 2 * sm_count() ? 8 : rows >= 4 * 2 * sm_count() ? 4 : rows >= 2 * 2 * sm_count() ? 2 : 1;
   int blocks = (rows + warps_per_block - 1) / warps_per_block;
@@ -606,7 +608,8 @@ extern "C" int sdb_layernorm(const float* x, int32_t rows, int32_t c, const floa
   else if (npl <= 20) SDB_LN(20);
   else if (npl <= 24) SDB_LN(24);
   else if (npl <= 40) SDB_LN(40);
-  else SDB_LN(48);
+  else if (npl <= 48) SDB_LN(48);
+  else SDB_LN(56);   // the retrieval-augmented UNet's middle block (1792)
 #undef SDB_LN
   SDB_LAUNCH_CHECK();
   return 0;
@@ -661,7 +664,7 @@ extern "C" int sdb_groupnorm_mod(const float* x, int32_t c, int32_t nb, int32_t 
     int slabs = std::max(1, std::min(std::min((hw + rstep - 1) / rstep, GN_MAX_SLABS), (sm_count() * 4 + nb - 1) / nb));
     int rows_per_block = (hw + slabs - 1) / slabs;
     slabs = (hw + rows_per_block - 1) / rows_per_block;
-    gn_stats_kernel<<<dim3(slabs, nb), GN_THREADS, 2 * c * sizeof(float), st>>>(x, nullptr, c, 0, hw, groups,
+    (c > GN_THREADS * GN_CPT ? gn_stats_kernel<GN_MAX_CPT> : gn_stats_kernel<GN_CPT>)<<<dim3(slabs, nb), GN_THREADS, 2 * c * sizeof(float), st>>>(x, nullptr, c, 0, hw, groups,
                                                                                  rows_per_block, cw, eps, partial, counter,
                                                                                  meanrstd);
     SDB_LAUNCH_CHECK();

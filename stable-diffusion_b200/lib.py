@@ -117,6 +117,9 @@ SIGNATURES = {
     "sdb_patch_fold": ([_P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _I, _I, _P, _P], C.c_int),
     "sdb_spatial_rescale": ([_P, _I, _I, _I, _I, _I, _P, _P, _I, _P, _P], C.c_int),
     "sdb_seg_labels_rescale": ([_P, _I, _I, _I, _I, _I, _P, _P, _I, _P, _P], C.c_int),
+    "sdb_knn_workspace": ([_L, _I, _I], C.c_int64),
+    "sdb_knn_topk": ([_P, _L, _I, _P, _I, _I, _P, _P, _L, _P, _P, _P], C.c_int),
+    "sdb_rows_pool": ([_P, _P, _I, _I, _I, _I, _P, _P], C.c_int),
     # post-processing (safety.cu)
     "sdb_resample_u8": ([_P, _P, _I, _I, _I, _I, _I, _P, _P, _I, _I, _P, _P], C.c_int),
     "sdb_clip_normalize": ([_P, _I, _I, _I, _I, _F, _F, _F, _F, _F, _F, _P, _P], C.c_int),

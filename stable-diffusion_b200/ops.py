@@ -635,6 +635,46 @@ def seg_labels_rescale(labels_u8, cin, n_stages, weight, bias=None):
     return out
 
 
+KNN_MAX_QUERIES = 64   # queries per sdb_knn_topk launch
+
+
+def knn_topk(db, queries, k):
+    """Exact top-k by inner product (sdb_knn_topk): db fp16 [n, dim], queries fp16 [b <= 64, dim] -> (scores fp32
+    [b, k], rows int64 [b, k]), score descending, the lower row first on equal scores."""
+    _chk16(db, "db")
+    _chk16(queries, "queries")
+    n, dim = db.shape
+    b = queries.shape[0]
+    assert queries.shape == (b, dim), (tuple(queries.shape), dim)
+    need = int(_l.load().sdb_knn_workspace(n, b, k))
+    ws_s = torch.empty(max(need, 1), dtype=torch.float32, device=db.device)
+    ws_i = torch.empty(max(need, 1), dtype=torch.int32, device=db.device)
+    scores = torch.empty((b, k), dtype=torch.float32, device=db.device)
+    rows = torch.empty((b, k), dtype=torch.int64, device=db.device)
+    _l.check(_l.load().sdb_knn_topk(_ptr(db), n, dim, _ptr(queries), b, k, _ptr(ws_s), _ptr(ws_i), need, _ptr(scores),
+                                    _ptr(rows), _stream()), "sdb_knn_topk")
+    _count(2)
+    return scores, rows
+
+
+def rows_pool(x, ids=None, normalize=False):
+    """x fp32 [rows, dim] -> fp32 [b, dim]: with ids (int64 [b, n_ctx]) the row at each sequence's largest id (CLIP's EOT
+    token), else every row; normalize divides each row by its L2 norm (sdb_rows_pool)."""
+    _chk32(x, "x")
+    dim = x.shape[-1]
+    if ids is not None:
+        assert ids.dtype == torch.int64 and ids.is_cuda and ids.is_contiguous() and ids.dim() == 2
+        b, n_ctx = ids.shape
+        assert x.numel() == b * n_ctx * dim, (tuple(x.shape), tuple(ids.shape))
+    else:
+        b, n_ctx = x.numel() // dim, 0
+    out = torch.empty((b, dim), dtype=torch.float32, device=x.device)
+    _l.check(_l.load().sdb_rows_pool(_ptr(x), _ptr(ids), b, n_ctx, dim, int(normalize), _ptr(out), _stream()),
+             "sdb_rows_pool")
+    _count()
+    return out
+
+
 def upsample2x(x):
     _chk32(x, "x")
     nb, h, w, c = x.shape

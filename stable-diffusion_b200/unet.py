@@ -271,7 +271,9 @@ class UNetModel(PackedStage):
             out = []
             for kind, pre, a in layers:
                 if kind == "conv_in":
-                    out.append((kind, {"w": _pack_conv3_padk(sd[pre + ".weight"], 64), "b": f32(pre + ".bias"),
+                    # K = 9 * in_channels zero-padded to the GEMM's 64-wide K step (64 up to 7 channels, 192 for 16)
+                    kpad = (9 * a["cin"] + 63) // 64 * 64
+                    out.append((kind, {"w": _pack_conv3_padk(sd[pre + ".weight"], kpad), "b": f32(pre + ".bias"),
                                        "cout": a["cout"]}))
                 elif kind == "res":
                     out.append((kind, pack_res(pre, a)))
@@ -526,10 +528,10 @@ class UNetModel(PackedStage):
             elif kind == "conv_in":
                 if isinstance(h, tuple):    # concat route: (x, conditioning), both NCHW, one im2col for the pair
                     nb, _, H, Wd = h[0].shape
-                    col = ops.im2col3x3_concat(h[0], h[1], 64)
+                    col = ops.im2col3x3_concat(h[0], h[1], p["w"].shape[1])
                 else:
                     nb, H, Wd, c = h.shape
-                    col = ops.im2col3x3(h, 1, 1, H, Wd, 64)
+                    col = ops.im2col3x3(h, 1, 1, H, Wd, p["w"].shape[1])
                 _, o = ops.gemm(col, p["w"], bias=p["b"], want_f32=True, rows_per_sample=H * Wd, want_stats=True, stats_group=self._sg)
                 h = o.view(nb, H, Wd, p["cout"])
         return h
@@ -585,10 +587,13 @@ class UNetModel(PackedStage):
             _, o = ops.gemm(hn, W["w_out"], taps=9, bias=W["b_out"], want_f32=True)
         return ops.nhwc_to_nchw(o.view(nb, H, Wd, self.out_channels))
 
-    def _graph_for(self, shape, kvs, concat_shape=None):
+    def _graph_for(self, shape, kvs, concat_shape=None, ctx_tokens=None):
         """Capture one UNet evaluation (~400 kernels) as a CUDA graph with static x / t / eps / K,V buffers, and a static
-        conditioning buffer on the concat route."""
+        conditioning buffer on the concat route. The static K,V buffers are per context token count, so a conditional
+        UNet keeps one graph per (shape, ctx_tokens): text-only and text + neighbours contexts share a latent shape."""
         key = shape if concat_shape is None else (shape, concat_shape)
+        if ctx_tokens is not None:
+            key = (key, ctx_tokens)
         g = self._graphs.get(key)
         if g is None:
             dev = self.W["device"]
@@ -681,7 +686,7 @@ class UNetModel(PackedStage):
         if self.use_cuda_graph:
             if not cached:
                 self.set_context(context)
-            g = self._graph_for(tuple(x.shape), self._ctx_kv)
+            g = self._graph_for(tuple(x.shape), self._ctx_kv, ctx_tokens=context.shape[1])
             assert g["kvs"] is self._ctx_kv or all(a[1].data_ptr() == b[1].data_ptr() for a, b in zip(g["kvs"], self._ctx_kv))
             if x.data_ptr() != g["x"].data_ptr():
                 g["x"].copy_(x)

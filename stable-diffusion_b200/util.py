@@ -29,6 +29,7 @@ TARGET_MAP = {
     "ldm.models.autoencoder.AutoencoderKL": "sdb200.vae.AutoencoderKL",
     "ldm.models.autoencoder.VQModelInterface": "sdb200.vq.VQModelInterface",
     "ldm.modules.encoders.modules.FrozenCLIPEmbedder": "sdb200.clip.FrozenCLIPEmbedder",
+    "ldm.modules.encoders.modules.FrozenCLIPTextEmbedder": "sdb200.clip.FrozenCLIPTextEmbedder",
     "ldm.modules.encoders.modules.ClassEmbedder": "sdb200.encoders.ClassEmbedder",
     "ldm.modules.encoders.modules.BERTEmbedder": "sdb200.bert.BERTEmbedder",
     "ldm.modules.encoders.modules.SpatialRescaler": "sdb200.encoders.SpatialRescaler",

@@ -2,7 +2,9 @@
 (`encode(x) -> posterior`, `decode(z) -> image`; autoencoder.py:285-333) over the VAE Encoder/Decoder of
 ldm/modules/diffusionmodules/model.py:368-568. State-dict keys unchanged (`encoder.*`, `decoder.*`, `quant_conv.*`,
 `post_quant_conv.*`). Same kernels as the UNet: wgmma implicit-GEMM convs, fp32 GroupNorm (eps 1e-6) + SiLU
-producing the fp16 operand, fp32 residual stream. The single-head mid-block attention (c=512, N=h*w;
+producing the fp16 operand, fp32 residual stream. Any latent width the 1x1 quant convs take (<= 16: SD-v1's 4,
+KL-f16's 16) and AttnBlocks inside the levels at ddconfig.attn_resolutions (KL-f16: at 16x16) run; posterior sampling
+is for 4 latent channels. The single-head mid-block attention (c=512, N=h*w;
 model.py:178-202) runs in the d = 512 flash kernel (sdb_attention, dpad 512; other widths: QK^T GEMM -> fp32 row softmax -> PV GEMM per image), with the value bias folded through proj_out (softmax rows sum to 1).
 """
 from __future__ import annotations
@@ -26,7 +28,6 @@ class DiagonalGaussianDistribution:
     def __init__(self, moments_nhwc, nb, h, w, zc):
         self._m = moments_nhwc  # fp32 [nb*h*w, 2*zc]
         self.nb, self.h, self.w, self.zc = nb, h, w, zc
-        assert zc == 4, "SD first stage has 4 latent channels"
 
     @property
     def parameters(self):
@@ -41,6 +42,8 @@ class DiagonalGaussianDistribution:
         return torch.clamp(self.parameters[:, self.zc:], -30.0, 20.0)
 
     def sample(self, noise=None, scale=1.0):
+        if self.zc != 4:
+            raise NotImplementedError(f"sampling the posterior of a {self.zc}-channel first stage (sdb_vae_sample: 4)")
         if noise is None:  # the reference draws on the CPU generator then moves (distributions.py:36)
             noise = torch.randn((self.nb, self.zc, self.h, self.w)).to(self._m.device)
         z = ops.vae_sample(self._m, noise.contiguous().float(), self.nb, self.h * self.w, scale)
@@ -247,7 +250,11 @@ class AutoencoderKL(ConvAutoencoder):
     def __init__(self, ddconfig, lossconfig=None, embed_dim=4, ckpt_path=None, ignore_keys=(), image_key="image",
                  colorize_nlabels=None, monitor=None):
         assert ddconfig["double_z"], "AutoencoderKL needs double_z"
-        assert not ddconfig.get("attn_resolutions"), "SD-v1 VAE: attention only in the mid block"
+        # every reference KL config names level resolutions only (kl-f16: [16], kl-f32: [16, 8]); an entry no level reaches
+        # builds nothing in the reference and means the config was written for another geometry
+        levels = [ddconfig["resolution"] // 2 ** i for i in range(len(ddconfig["ch_mult"]))]
+        unreached = sorted(set(ddconfig.get("attn_resolutions") or ()) - set(levels))
+        assert not unreached, f"attn_resolutions {unreached} name no level of this first stage (levels at {levels})"
         cfg = dict(embed_dim=embed_dim, ddconfig=dict(ddconfig))
         super().__init__(vae_param_shapes(cfg))
         self.cfg = cfg
