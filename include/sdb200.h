@@ -333,6 +333,23 @@ int sdb_knn_topk(const void* db, int64_t n, int32_t dim, const void* queries, in
  * row b; normalize != 0 divides each row by its L2 norm in fp32. */
 int sdb_rows_pool(const float* x, const int64_t* ids, int32_t b, int32_t n_ctx, int32_t dim, int32_t normalize,
                   float* out, sdb_stream_t stream);
+/* ---- CLIP image embedding of retrieval databases (clip_image.cu; FrozenClipImageEmbedder, modules.py:197-229) ----
+ * Preprocessing of a ragged batch straight into the patch-embedding GEMM's operand: each image is resized to
+ * size x size as F.interpolate(mode='bicubic', align_corners=True) does on CUDA (kornia.geometry.resize with
+ * antialias=False; A = -0.75, border taps clamped, a copy when both sides match), then (x + 1) / 2 and (x - m) / s per
+ * channel, rounded to fp16 patch rows [nb * (size/patch)^2, kpad], k = (c * patch + py) * patch + px, zero-padded to
+ * kpad (a multiple of 64). table int64 [nb, 3] (device) = (H, W, element offset in src) per image. src is fp32 NCHW
+ * [3, H, W] per image in [-1, 1] (src_u8 0) or uint8 HWC [H, W, 3] (src_u8 1), read as x / 127.5 - 1.
+ * resized (optional) fp32 [nb, 3, size, size] receives the interpolated values before (x + 1) / 2. */
+int sdb_clip_resize_patches(const void* src, int32_t src_u8, const int64_t* table, int32_t nb, int32_t size,
+                            int32_t patch, int32_t kpad, float m0, float m1, float m2, float s0, float s1, float s2,
+                            void* patches_f16, float* resized, sdb_stream_t stream);
+/* CLIPVisionEmbeddings after the patch GEMM: x fp32 [nb, np + 1, dim], row 0 = cls_pos [dim] (class embedding +
+ * pos[0]), row 1 + p = pe[b * np + p] + pos_patches[p]; pe fp32 [nb * np, dim]. dim % 4 == 0, 16-byte aligned. */
+int sdb_vit_embed(const float* pe, const float* cls_pos, const float* pos_patches, int32_t nb, int32_t np, int32_t dim,
+                  float* x, sdb_stream_t stream);
+/* out fp32 [rows, dim] = x row r * row_stride (the class token of each sequence before ln_post) */
+int sdb_rows_gather(const float* x, int32_t rows, int64_t row_stride, int32_t dim, float* out, sdb_stream_t stream);
 /* out = a*x + b (latent scaling z/0.18215, ddpm.py:713) */
 int sdb_axpby(const float* x, float a, float b, int64_t n, float* out, sdb_stream_t stream);
 /* out = a*x + b*y (DDIMSampler.stochastic_encode, ddim.py:206-220; q_sample, ddpm.py:274-277) */

@@ -7,8 +7,9 @@
 The prompt is encoded by FrozenCLIPTextEmbedder (CLIP ViT-L/14's projected, normalised text embedding, (B, 1, 768)).
 With --use_neighbors the Searcher (sdb200.retrieval) loads data/rdm/retrieval_databases/<database>/*.npz, takes the
 --knn rows of the largest dot product with the normalised query, exactly, on the GPU, and appends their normalised
-embeddings: (B, 1 + knn, 768). The unconditional conditioning is zeros_like(c) when --scale is not 1; DDIM (or PLMS)
-samples the [16, H/16, W/16] latent inside ema_scope() on the CUDA-graph path, and decode_first_stage (KL-f16) gives the
+embeddings: (B, 1 + knn, 768). --database_dir DIR reads the shards from DIR instead (a database built by
+scripts/build_rdm_database.py, which the fixed --database names cannot point at). The unconditional conditioning is
+zeros_like(c) when --scale is not 1; DDIM (or PLMS) samples the [16, H/16, W/16] latent inside ema_scope() on the CUDA-graph path, and decode_first_stage (KL-f16) gives the
 images, written as samples/NNNNN.png and one grid per --n_iter, as the reference does.
 
 CLIP's weights are read in the transformers CLIPModel layout (`text_model.*`, `text_projection.weight`; the vision
@@ -119,6 +120,9 @@ def get_parser():
     p.add_argument("--ckpt", type=str, default="models/rdm/rdm768x768/model.ckpt")
     p.add_argument("--clip_type", type=str, default="ViT-L/14")
     p.add_argument("--database", type=str, default="artbench-surrealism", choices=DATABASES)
+    p.add_argument("--database_dir", type=str, default=None,
+                   help="a database directory of .npz shards (e.g. from scripts/build_rdm_database.py); overrides the "
+                        "--database path")
     p.add_argument("--use_neighbors", default=False, action="store_true")
     p.add_argument("--knn", default=10, type=int)
     p.add_argument("--random_init", action="store_true", help="seeded random weights instead of checkpoints")
@@ -167,7 +171,7 @@ def main(argv=None):
     os.makedirs(sample_path, exist_ok=True)
     base_count = len(os.listdir(sample_path))
     grid_count = len(os.listdir(opt.outdir)) - 1
-    searcher = Searcher(opt.database, device=device) if opt.use_neighbors else None
+    searcher = Searcher(opt.database, device=device, path=opt.database_dir) if opt.use_neighbors else None
 
     written = []
     t0 = time.time()

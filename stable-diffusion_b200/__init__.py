@@ -7,9 +7,10 @@ __version__ = "0.1.0"
 
 import sys as _sys
 
-from . import arch, bert, checkpoint, clip, diffusion, dist, encoders, lib, ops, pipeline, retrieval, safety, samplers, tokenizer, unet, util, vae, vq  # noqa: E402,F401
+from . import arch, bert, checkpoint, clip, clip_image, diffusion, dist, encoders, lib, ops, pipeline, retrieval, safety, samplers, tokenizer, unet, util, vae, vq  # noqa: E402,F401
 from .bert import BERTEmbedder  # noqa: E402,F401
 from .clip import FrozenCLIPEmbedder, FrozenCLIPTextEmbedder  # noqa: E402,F401
+from .clip_image import FrozenClipImageEmbedder  # noqa: E402,F401
 from .diffusion import LatentDiffusion  # noqa: E402,F401
 from .encoders import ClassEmbedder, SpatialRescaler  # noqa: E402,F401
 from .safety import StableDiffusionSafetyChecker  # noqa: E402,F401

@@ -165,6 +165,12 @@ TINY_KL_F16 = dict(embed_dim=16, ddconfig=dict(double_z=True, z_channels=16, res
                                                ch=64, ch_mult=[1, 1, 2, 2, 8], num_res_blocks=1,
                                                attn_resolutions=[16, 4], dropout=0.0))
 TINY_CLIP_TEXT_PROJ = dict(TINY_CLIP, projection_dim=64)
+# FrozenClipImageEmbedder (the retriever that embeds RDM databases): the CLIP ViT-L/14 vision tower with the visual
+# projection (transformers CLIPModel's visual_projection); the tiny member's 64-wide embeddings match TINY_RDM_UNET
+CLIP_VISION_PROJ = dict(hidden_size=1024, intermediate_size=4096, num_hidden_layers=24, num_attention_heads=16,
+                        image_size=224, patch_size=14, projection_dim=768, layer_norm_eps=1e-5)
+TINY_CLIP_VISION_PROJ = dict(hidden_size=128, intermediate_size=256, num_hidden_layers=2, num_attention_heads=2,
+                             image_size=56, patch_size=14, projection_dim=64, layer_norm_eps=1e-5)
 
 
 # ------------------------------------------------------------------------------------------------ UNet
@@ -502,6 +508,36 @@ def clip_text_proj_param_shapes(cfg):
     [projection_dim, hidden] (no bias), for FrozenCLIPTextEmbedder."""
     p = clip_param_shapes(cfg)
     p["text_projection.weight"] = (cfg["projection_dim"], cfg["hidden_size"])
+    return p
+
+
+def clip_vision_proj_param_shapes(cfg):
+    """The vision half of transformers CLIPModel.state_dict() (= CLIPVisionModelWithProjection's): `vision_model.*`
+    and `visual_projection.weight` [projection_dim, hidden] (no bias), for FrozenClipImageEmbedder."""
+    h, inter = cfg["hidden_size"], cfg["intermediate_size"]
+    npos = (cfg["image_size"] // cfg["patch_size"]) ** 2 + 1
+    p = OrderedDict()
+    p["vision_model.embeddings.class_embedding"] = (h,)
+    p["vision_model.embeddings.patch_embedding.weight"] = (h, 3, cfg["patch_size"], cfg["patch_size"])
+    p["vision_model.embeddings.position_embedding.weight"] = (npos, h)
+    p["vision_model.pre_layrnorm.weight"] = (h,)
+    p["vision_model.pre_layrnorm.bias"] = (h,)
+    for i in range(cfg["num_hidden_layers"]):
+        pre = f"vision_model.encoder.layers.{i}"
+        for n in ("k_proj", "v_proj", "q_proj", "out_proj"):
+            p[f"{pre}.self_attn.{n}.weight"] = (h, h)
+            p[f"{pre}.self_attn.{n}.bias"] = (h,)
+        p[f"{pre}.layer_norm1.weight"] = (h,)
+        p[f"{pre}.layer_norm1.bias"] = (h,)
+        p[f"{pre}.mlp.fc1.weight"] = (inter, h)
+        p[f"{pre}.mlp.fc1.bias"] = (inter,)
+        p[f"{pre}.mlp.fc2.weight"] = (h, inter)
+        p[f"{pre}.mlp.fc2.bias"] = (h,)
+        p[f"{pre}.layer_norm2.weight"] = (h,)
+        p[f"{pre}.layer_norm2.bias"] = (h,)
+    p["vision_model.post_layernorm.weight"] = (h,)
+    p["vision_model.post_layernorm.bias"] = (h,)
+    p["visual_projection.weight"] = (cfg["projection_dim"], h)
     return p
 
 

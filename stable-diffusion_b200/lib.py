@@ -120,6 +120,10 @@ SIGNATURES = {
     "sdb_knn_workspace": ([_L, _I, _I], C.c_int64),
     "sdb_knn_topk": ([_P, _L, _I, _P, _I, _I, _P, _P, _L, _P, _P, _P], C.c_int),
     "sdb_rows_pool": ([_P, _P, _I, _I, _I, _I, _P, _P], C.c_int),
+    # CLIP image embedding (clip_image.cu)
+    "sdb_clip_resize_patches": ([_P, _I, _P, _I, _I, _I, _I, _F, _F, _F, _F, _F, _F, _P, _P, _P], C.c_int),
+    "sdb_vit_embed": ([_P, _P, _P, _I, _I, _I, _P, _P], C.c_int),
+    "sdb_rows_gather": ([_P, _I, _L, _I, _P, _P], C.c_int),
     # post-processing (safety.cu)
     "sdb_resample_u8": ([_P, _P, _I, _I, _I, _I, _I, _P, _P, _I, _I, _P, _P], C.c_int),
     "sdb_clip_normalize": ([_P, _I, _I, _I, _I, _F, _F, _F, _F, _F, _F, _P, _P], C.c_int),

@@ -675,6 +675,48 @@ def rows_pool(x, ids=None, normalize=False):
     return out
 
 
+def clip_resize_patches(src, table, size, patch, kpad, mean, std, want_resized=False):
+    """Ragged-batch CLIP image preprocessing (sdb_clip_resize_patches): src packed images, fp32 (NCHW each, in [-1, 1])
+    or uint8 (HWC each), table int64 cuda [nb, 3] = (H, W, element offset) -> (fp16 patch rows [nb * (size/patch)^2,
+    kpad], fp32 [nb, 3, size, size] resized values before (x + 1) / 2, or None)."""
+    assert src.is_cuda and src.is_contiguous() and src.dtype in (torch.float32, torch.uint8), "src: contiguous cuda fp32 / uint8"
+    assert table.dtype == torch.int64 and table.is_cuda and table.is_contiguous() and table.dim() == 2 and table.shape[1] == 3
+    nb = table.shape[0]
+    g = size // patch
+    patches = torch.empty((nb * g * g, kpad), dtype=torch.float16, device=src.device)
+    resized = torch.empty((nb, 3, size, size), dtype=torch.float32, device=src.device) if want_resized else None
+    _l.check(_l.load().sdb_clip_resize_patches(_ptr(src), int(src.dtype == torch.uint8), _ptr(table), nb, size, patch,
+                                               kpad, *mean, *std, _ptr(patches), _ptr(resized), _stream()),
+             "sdb_clip_resize_patches")
+    _count()
+    return patches, resized
+
+
+def vit_embed(pe, cls_pos, pos_patches, nb):
+    """pe fp32 [nb * np, dim] (patch GEMM output) -> the token sequence fp32 [nb * (np + 1), dim] (sdb_vit_embed)."""
+    _chk32(pe, "pe")
+    _chk32(cls_pos, "cls_pos")
+    _chk32(pos_patches, "pos_patches")
+    np_, dim = pos_patches.shape
+    assert pe.shape == (nb * np_, dim) and cls_pos.shape == (dim,)
+    x = torch.empty((nb * (np_ + 1), dim), dtype=torch.float32, device=pe.device)
+    _l.check(_l.load().sdb_vit_embed(_ptr(pe), _ptr(cls_pos), _ptr(pos_patches), nb, np_, dim, _ptr(x), _stream()),
+             "sdb_vit_embed")
+    _count()
+    return x
+
+
+def rows_gather(x, rows, row_stride):
+    """x fp32 [>= (rows - 1) * row_stride + 1, dim] -> fp32 [rows, dim] of every row_stride-th row (sdb_rows_gather)."""
+    _chk32(x, "x")
+    dim = x.shape[-1]
+    assert x.numel() // dim >= (rows - 1) * row_stride + 1
+    out = torch.empty((rows, dim), dtype=torch.float32, device=x.device)
+    _l.check(_l.load().sdb_rows_gather(_ptr(x), rows, row_stride, dim, _ptr(out), _stream()), "sdb_rows_gather")
+    _count()
+    return out
+
+
 def upsample2x(x):
     _chk32(x, "x")
     nb, h, w, c = x.shape

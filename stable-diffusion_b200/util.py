@@ -30,6 +30,7 @@ TARGET_MAP = {
     "ldm.models.autoencoder.VQModelInterface": "sdb200.vq.VQModelInterface",
     "ldm.modules.encoders.modules.FrozenCLIPEmbedder": "sdb200.clip.FrozenCLIPEmbedder",
     "ldm.modules.encoders.modules.FrozenCLIPTextEmbedder": "sdb200.clip.FrozenCLIPTextEmbedder",
+    "ldm.modules.encoders.modules.FrozenClipImageEmbedder": "sdb200.clip_image.FrozenClipImageEmbedder",
     "ldm.modules.encoders.modules.ClassEmbedder": "sdb200.encoders.ClassEmbedder",
     "ldm.modules.encoders.modules.BERTEmbedder": "sdb200.bert.BERTEmbedder",
     "ldm.modules.encoders.modules.SpatialRescaler": "sdb200.encoders.SpatialRescaler",
