@@ -17,44 +17,56 @@ constexpr int GN_MAX_SLABS = 128;
 
 // pass 1: per (sample, group) mean / rstd. grid = (slabs, nb). Thread t owns channel (t % cw) [+ k*cw] of rows
 // (t / cw) + k * (256 / cw): consecutive threads read consecutive channels (coalesced), four rows in flight per
-// thread. Per-channel partials are combined in shared memory, reduced per group by one warp each and written as
-// per-block partials (no contended atomics); the last block of each sample (ticket counter) folds the partials in
-// fp64 and publishes mean / rstd.
+// thread. Sums are taken around a per-(sample, group) pivot (x at row 0, the group's first channel) that every block
+// reads alike, so a mean far from zero does not cancel away the variance: fp32 E[(x-p)^2] - E[x-p]^2 keeps its
+// accuracy where E[x^2] - E[x]^2 would lose (mean/std)^2 of it. Each row lane parks its per-channel partials in its
+// own shared-memory slot and a fixed-order sum combines them (bit-reproducible: shared-memory float atomics from
+// more than two lanes would add in scheduling order); each group is reduced by one warp and written as per-block
+// partials; the last block of each sample (ticket counter) folds the partials in fp64 and publishes mean / rstd.
+// Three resident blocks per SM (80 registers, no spills).
 template <int CPT>
-__global__ void __launch_bounds__(GN_THREADS)
+__global__ void __launch_bounds__(GN_THREADS, 3)
     gn_stats_kernel(const float* __restrict__ x0, const float* __restrict__ x1, int c0, int c1, int hw, int groups,
                     int rows_per_block, int cw, float eps, float* __restrict__ partial,
                     unsigned int* __restrict__ counter, float* __restrict__ meanrstd) {
-  extern __shared__ float gn_smem[];  // [2][C]
+  extern __shared__ float gn_smem[];  // [2][rstep][C] partials | [C] pivot of each channel's group
   __shared__ bool is_last;
+  __shared__ float piv[64];
   const int C = c0 + c1;
   const int cpg = C / groups;
   const int n = blockIdx.y;
   const int slabs = gridDim.x;
   const int r0 = blockIdx.x * rows_per_block;
   const int r1 = min(hw, r0 + rows_per_block);
-  float* sum_s = gn_smem;
-  float* sum_q = gn_smem + C;
-  for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) gn_smem[i] = 0.f;
-  __syncthreads();
   const int tc = threadIdx.x % cw;
   const int tr = threadIdx.x / cw;
   const int rstep = GN_THREADS / cw;
+  float* sum_s = gn_smem;
+  float* sum_q = gn_smem + rstep * C;
+  float* piv_c = gn_smem + 2 * rstep * C;
+  const size_t base = static_cast<size_t>(n) * hw;
+  if (threadIdx.x < groups) {
+    const int c = threadIdx.x * cpg;
+    piv[threadIdx.x] = c < c0 ? x0[base * c0 + c] : x1[base * c1 + (c - c0)];
+  }
+  __syncthreads();
+  for (int c = threadIdx.x; c < C; c += GN_THREADS) piv_c[c] = piv[c / cpg];
+  __syncthreads();
   float s[CPT], q[CPT];
 #pragma unroll
   for (int j = 0; j < CPT; ++j) s[j] = q[j] = 0.f;
-  const size_t base = static_cast<size_t>(n) * hw;
   for (int r = r0 + tr; r < r1; r += 4 * rstep) {
 #pragma unroll
     for (int j = 0; j < CPT; ++j) {
       const int c = tc + j * cw;
       if (c < C) {
+        const float p = piv_c[c];
         float v[4];
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
           const int rr = r + u * rstep;
           v[u] = 0.f;
-          if (rr < r1) v[u] = c < c0 ? x0[(base + rr) * c0 + c] : x1[(base + rr) * c1 + (c - c0)];
+          if (rr < r1) v[u] = (c < c0 ? x0[(base + rr) * c0 + c] : x1[(base + rr) * c1 + (c - c0)]) - p;
         }
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
@@ -66,15 +78,10 @@ __global__ void __launch_bounds__(GN_THREADS)
   }
 #pragma unroll
   for (int j = 0; j < CPT; ++j) {
-    int c = tc + j * cw;
+    const int c = tc + j * cw;
     if (c < C) {
-      if (rstep == 1) {
-        sum_s[c] = s[j];
-        sum_q[c] = q[j];
-      } else {
-        atomicAdd(&sum_s[c], s[j]);
-        atomicAdd(&sum_q[c], q[j]);
-      }
+      sum_s[tr * C + c] = s[j];
+      sum_q[tr * C + c] = q[j];
     }
   }
   __syncthreads();
@@ -83,8 +90,10 @@ __global__ void __launch_bounds__(GN_THREADS)
   for (int g = warp; g < groups; g += GN_THREADS / 32) {
     float a = 0.f, b = 0.f;
     for (int c = lane; c < cpg; c += 32) {
-      a += sum_s[g * cpg + c];
-      b += sum_q[g * cpg + c];
+      for (int k = 0; k < rstep; ++k) {
+        a += sum_s[k * C + g * cpg + c];
+        b += sum_q[k * C + g * cpg + c];
+      }
     }
 #pragma unroll
     for (int o = 16; o; o >>= 1) {
@@ -116,10 +125,10 @@ __global__ void __launch_bounds__(GN_THREADS)
       b += __shfl_xor_sync(0xffffffffu, b, o);
     }
     if (lane == 0) {
-      double m = a / cnt;
-      double v = b / cnt - m * m;
+      const double d = a / cnt;   // mean - pivot
+      double v = b / cnt - d * d;
       if (v < 0) v = 0;
-      meanrstd[(static_cast<size_t>(n) * groups + g) * 2] = static_cast<float>(m);
+      meanrstd[(static_cast<size_t>(n) * groups + g) * 2] = static_cast<float>(static_cast<double>(piv[g]) + d);
       meanrstd[(static_cast<size_t>(n) * groups + g) * 2 + 1] = static_cast<float>(1.0 / sqrt(v + static_cast<double>(eps)));
     }
   }
@@ -523,6 +532,12 @@ extern "C" int sdb_groupnorm(const float* x0, const float* x1, int32_t c0, int32
   SDB_CHECK(groups > 0 && groups <= 64 && C % groups == 0, "sdb_groupnorm: C=%d not divisible by groups=%d", C, groups);
   SDB_CHECK(c0 % 4 == 0 && c1 % 4 == 0, "sdb_groupnorm: channel counts must be multiples of 4");
   SDB_CHECK(C <= GN_THREADS * GN_MAX_CPT, "sdb_groupnorm: C=%d too large", C);
+  // the apply pass reads x as float4 and writes fp16 quads as 8-byte words
+  SDB_CHECK(((reinterpret_cast<uintptr_t>(x0) | reinterpret_cast<uintptr_t>(x1)) & 15) == 0,
+            "sdb_groupnorm: x0 / x1 must be 16-byte aligned");
+  SDB_CHECK(((reinterpret_cast<uintptr_t>(out_f16) | reinterpret_cast<uintptr_t>(raw_f16) |
+              reinterpret_cast<uintptr_t>(out_lo_f16) | reinterpret_cast<uintptr_t>(raw_lo_f16)) & 7) == 0,
+            "sdb_groupnorm: fp16 outputs must be 8-byte aligned");
   // workspace layout: [nb][GN_MAX_SLABS][groups][2] float partials | [nb][groups][2] float mean/rstd | [nb] tickets
   float* partial = static_cast<float*>(stats_ws);
   float* meanrstd = partial + static_cast<size_t>(nb) * GN_MAX_SLABS * groups * 2;
@@ -545,7 +560,7 @@ extern "C" int sdb_groupnorm(const float* x0, const float* x1, int32_t c0, int32
   slabs = (hw + rows_per_block - 1) / rows_per_block;
   dim3 grid(slabs, nb);
   if (!fused_stats) {
-    (C > GN_THREADS * GN_CPT ? gn_stats_kernel<GN_MAX_CPT> : gn_stats_kernel<GN_CPT>)<<<grid, GN_THREADS, 2 * C * sizeof(float), st>>>(x0, x1, c0, c1, hw, groups, rows_per_block, cw,
+    (C > GN_THREADS * GN_CPT ? gn_stats_kernel<GN_MAX_CPT> : gn_stats_kernel<GN_CPT>)<<<grid, GN_THREADS, (2 * rstep + 1) * C * sizeof(float), st>>>(x0, x1, c0, c1, hw, groups, rows_per_block, cw,
                                                                       eps, partial, counter, meanrstd);
     SDB_LAUNCH_CHECK();
   }
@@ -637,6 +652,9 @@ extern "C" int sdb_groupnorm_mod(const float* x, int32_t c, int32_t nb, int32_t 
   SDB_CHECK(groups > 0 && groups <= 32 && c % groups == 0, "sdb_groupnorm_mod: C=%d not divisible by groups=%d", c, groups);
   SDB_CHECK(c % 4 == 0 && c <= GN_THREADS * GN_MAX_CPT, "sdb_groupnorm_mod: C=%d must be a multiple of 4, <= %d", c,
             GN_THREADS * GN_MAX_CPT);
+  // the apply pass reads x as float4 and writes fp16 quads as 8-byte words
+  SDB_CHECK((reinterpret_cast<uintptr_t>(x) & 15) == 0, "sdb_groupnorm_mod: x must be 16-byte aligned");
+  SDB_CHECK((reinterpret_cast<uintptr_t>(out_f16) & 7) == 0, "sdb_groupnorm_mod: out must be 8-byte aligned");
   SDB_CHECK((scale == nullptr) == (shift == nullptr), "sdb_groupnorm_mod: scale and shift go together");
   SDB_CHECK(!scale || ldm >= c, "sdb_groupnorm_mod: modulation row stride %d < C %d", ldm, c);
   SDB_CHECK(resample >= 0 && resample <= 2, "sdb_groupnorm_mod: resample %d (0 none, 1 down, 2 up)", resample);
@@ -664,7 +682,7 @@ extern "C" int sdb_groupnorm_mod(const float* x, int32_t c, int32_t nb, int32_t 
     int slabs = std::max(1, std::min(std::min((hw + rstep - 1) / rstep, GN_MAX_SLABS), (sm_count() * 4 + nb - 1) / nb));
     int rows_per_block = (hw + slabs - 1) / slabs;
     slabs = (hw + rows_per_block - 1) / rows_per_block;
-    (c > GN_THREADS * GN_CPT ? gn_stats_kernel<GN_MAX_CPT> : gn_stats_kernel<GN_CPT>)<<<dim3(slabs, nb), GN_THREADS, 2 * c * sizeof(float), st>>>(x, nullptr, c, 0, hw, groups,
+    (c > GN_THREADS * GN_CPT ? gn_stats_kernel<GN_MAX_CPT> : gn_stats_kernel<GN_CPT>)<<<dim3(slabs, nb), GN_THREADS, (2 * rstep + 1) * c * sizeof(float), st>>>(x, nullptr, c, 0, hw, groups,
                                                                                  rows_per_block, cw, eps, partial, counter,
                                                                                  meanrstd);
     SDB_LAUNCH_CHECK();
