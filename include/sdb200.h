@@ -123,7 +123,8 @@ int sdb_gemm_plan(const sdb_gemm_desc* d, int32_t* out);
  * SpatialTransformers of the class-conditional ImageNet LDM at 384 / 576 / 960); they require heads == 1, d == dpad,
  * causal == 0, head_stride 0 or d, and ldq, ldk, ldvt, ldo, o_batch_stride multiples of 8.
  * Any other descriptor returns nonzero with a message in sdb_last_error() and launches nothing.
- * scale multiplies q.k before softmax (applied after the dot product, attention.py:180).
+ * scale multiplies q.k before softmax (applied after the dot product, attention.py:180); it must be positive and
+ * finite (the kernel takes the row maximum before scaling).
  * causal != 0 masks kv index > q index (CLIP text encoder).
  */
 typedef struct sdb_attn_desc {

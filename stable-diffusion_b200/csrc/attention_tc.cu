@@ -480,6 +480,8 @@ extern "C" int sdb_attention(const sdb_attn_desc* d, sdb_stream_t stream) {
   }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   SDB_CHECK(d && d->q && d->k && d->vt && d->out, "sdb_attention: null pointer");
+  // softmax_tile takes (row maximum of q.k) * scale as the maximum of the scaled logits
+  SDB_CHECK(d->scale > 0 && isfinite(d->scale), "sdb_attention: scale must be positive and finite (got %g)", d->scale);
   CUtensorMap tq, tk, tv;
   AttnArgs p{};
   p.nq = d->nq;
