@@ -53,7 +53,6 @@ The largest share of the bound used and the largest bias are printed per workloa
 """
 import ctypes as C
 import math
-import time
 from collections import defaultdict
 
 import pytest
@@ -61,34 +60,21 @@ import torch
 import torch.nn.functional as F
 
 import helpers  # noqa: F401  (puts the repository on sys.path)
-from sdb200 import arch, ops
+from sdb200 import ops
 from sdb200 import lib as _l
-from workloads import WORKLOADS as MODEL_WORKLOADS
-from workloads import _clip_image, _run_unet, _vq
+from sweeps import GUARD, NAN, Tally, check_coverage, eoff, record, ulp16
+from workloads import ATTENTION_WORKLOADS
 
-NAN = float("nan")
 TAU_P = 6e-4       # relative error of P (fp16 rounding + exp), relative to A = P |v|
 TAU_S = 4e-6       # fp32 logit accumulation, relative to smag A
 BIAS = 1.5e-5      # |mean signed relative error| of one launch
 ACC_RZ = 1.2e-8    # ... plus this per key: the truncating fp32 accumulation of O (measured 6.3e-9 with v > 0)
-GUARD = 16         # NaN elements before and after every output
 CHUNK = 1 << 26    # fp64 logits per reference chunk (512 MiB; a few temporaries of that size are alive at once)
 HEAVY = 1 << 28    # logits per launch above which only LIGHT_FAMILIES run
 AQ, AKV = 128, 64
 FAMILIES = ("randn1", "randn4", "posv", "uniform", "peaked", "rising", "falling", "jump", "bigv")
 LIGHT_FAMILIES = ("randn1", "posv", "uniform", "rising")
 WIDE_DV = {384: 128, 512: 128, 576: 96, 960: 160}
-
-
-def ulp16(x):
-    """Spacing of fp16 numbers at |x| (subnormal spacing below 2^-14)."""
-    e = torch.floor(torch.log2(x.abs().clamp_min(2.0 ** -14)))
-    return torch.exp2(e - 10)
-
-
-def _eoff(t):
-    """Element offset of t's data from the nearest 16-byte boundary."""
-    return (t.data_ptr() % 16) // t.element_size()
 
 
 def _c8(n):
@@ -220,33 +206,15 @@ def _ap(**kw):
 def _attn_sig(q, k, vt, *, heads, d, dpad, nq, nkv, scale, causal=False, out=None, head_stride=0):
     B = q.shape[0]
     shared = q.untyped_storage().data_ptr() == k.untyped_storage().data_ptr()
-    ldo, obs, oo = (heads * d, nq * heads * d, 0) if out is None else (out.stride(1), out.stride(0), _eoff(out))
+    ldo, obs, oo = (heads * d, nq * heads * d, 0) if out is None else (out.stride(1), out.stride(0), eoff(out))
     return _ap(B=B, heads=heads, nq=nq, nkv=nkv, d=d, dpad=dpad, hs=head_stride, causal=bool(causal),
                scale=float(scale), ldq=q.stride(1), ldk=k.stride(1), ldvt=vt.stride(1), ldo=ldo, qbs=q.stride(0),
-               kbs=k.stride(0), vbs=vt.stride(0), obs=obs, oq=_eoff(q), ok=_eoff(k), ov=_eoff(vt), oo=oo,
+               kbs=k.stride(0), vbs=vt.stride(0), obs=obs, oq=eoff(q), ok=eoff(k), ov=eoff(vt), oo=oo,
                k_rel=(k.data_ptr() - q.data_ptr()) // 2 if shared else None)
 
 
 def signature(p):
     return tuple(sorted((k, v) for k, v in p.items() if k != "fam"))
-
-
-class Recorder:
-    """Wraps ops.attention (through monkeypatch) and keeps the deduplicated problems in call order."""
-
-    def __init__(self):
-        self.seen, self.problems, self.calls = set(), [], 0
-
-    def wrap(self, fn):
-        def rec(*a, **kw):
-            p = _attn_sig(*a, **kw)
-            self.calls += 1
-            s = signature(p)
-            if s not in self.seen:
-                self.seen.add(s)
-                self.problems.append(p)
-            return fn(*a, **kw)
-        return rec
 
 
 def label(p):
@@ -515,11 +483,11 @@ def exact_checks(fam, p, X, v, info):
     return {}
 
 
-class Sweep:
+class Sweep(Tally):
     """Failures and calibration of one title (workload or synthetic group)."""
 
     def __init__(self, title):
-        self.title, self.failures, self.launches, self.t0 = title, [], 0, time.time()
+        super().__init__(title)
         self.share, self.bias = defaultdict(float), defaultdict(float)
 
     def fail(self, lab, chk, val):
@@ -584,14 +552,9 @@ class Sweep:
                 self.fail(lab, "head alone", f"h={h}")
             self.launches += 1
 
-    def finish(self, n_problems):
-        torch.cuda.synchronize()
-        print(f"\n{self.title}: {n_problems} problems, {self.launches} launches, {time.time() - self.t0:.1f} s; "
-              "largest share of the bound / largest |bias| per family: "
-              + ", ".join(f"{f} {self.share[f]:.3f} / {self.bias[f]:.1e}" for f in FAMILIES if f in self.share))
-        if self.failures:
-            rows = "\n".join(" | ".join(map(str, f)) for f in self.failures[:200])
-            pytest.fail(f"{self.title}: {len(self.failures)} failing (problem, check, value):\n{rows}")
+    def calibration(self):
+        return "largest share of the bound / largest |bias| per family: " + ", ".join(
+            f"{f} {self.share[f]:.3f} / {self.bias[f]:.1e}" for f in FAMILIES if f in self.share)
 
 
 def run_sweep(problems, title):
@@ -599,47 +562,20 @@ def run_sweep(problems, title):
     for i, p in enumerate(problems):
         sw.run(p, 1000 + i)
         torch.cuda.empty_cache()
-    sw.finish(len(problems))
-    return sw
+    sw.finish(len(problems), sw.calibration())
 
 
 # ------------------------------------------------------------------------------------------------ model workloads
-def _wl_vq_sr_tile(dev):
-    g = torch.Generator(device=dev).manual_seed(6)
-    _vq(arch.VQ_F4, dev).decode(torch.randn(1, 3, 128, 128, generator=g, device=dev))
-
-
-WORKLOADS = dict(MODEL_WORKLOADS)
-WORKLOADS.update({
-    "vq_f4_128x128_latent": _wl_vq_sr_tile,                                    # 16384 tokens at d = 512
-    "vit_l14_b37": lambda dev: _clip_image(arch.CLIP_VISION_PROJ, dev, 37),
-    "rdm_one_token_context": lambda dev: _run_unet(arch.RDM_UNET, [(2, 16, 48, 48)], dev, ctx=(1, 768)),
-})
-
-
-def catalogue(name, dev, monkeypatch):
-    rec = Recorder()
-    monkeypatch.setattr(ops, "AUTOTUNE", False)
-    monkeypatch.setattr(ops, "TUNED", {})
-    monkeypatch.setattr(ops, "attention", rec.wrap(ops.attention))
-    with torch.no_grad():
-        WORKLOADS[name](dev)
-    torch.cuda.synchronize()
-    monkeypatch.undo()
-    torch.cuda.empty_cache()
-    return rec
-
-
 @pytest.mark.gpu
 @pytest.mark.timeout(600)
-@pytest.mark.parametrize("name", list(WORKLOADS))
-def test_every_attention_launch_of_every_model(cuda_dev, monkeypatch, name):
-    rec = catalogue(name, cuda_dev, monkeypatch)
-    print(f"\n{name}: {rec.calls} calls, {len(rec.problems)} distinct problems")
-    assert rec.problems
+@pytest.mark.parametrize("name", list(ATTENTION_WORKLOADS))
+def test_every_attention_launch_of_every_model(cuda_dev, name):
+    calls, problems = record(ATTENTION_WORKLOADS[name], cuda_dev, {"attention": _attn_sig})
+    print(f"\n{name}: {calls} calls, {len(problems)} distinct problems")
+    assert problems
     if name == "rdm_one_token_context":     # the one-token context is folded into the out-projection: self-attention only
-        assert all(p["nq"] == p["nkv"] and p["k_rel"] is not None for p in rec.problems), [label(p) for p in rec.problems]
-    run_sweep(rec.problems, name)
+        assert all(p["nq"] == p["nkv"] and p["k_rel"] is not None for p in problems), [label(p) for p in problems]
+    run_sweep(problems, name)
     torch.cuda.empty_cache()
 
 
@@ -733,10 +669,7 @@ def test_attention_beyond_2g_elements(cuda_dev):
 @pytest.mark.gpu
 def test_attention_branch_coverage():
     """Every instance and every control-flow class of attention_tc.cu was launched by the sweeps above."""
-    if not COVER:
-        pytest.skip("the attention sweeps did not run in this session")
-    print("\ncoverage: " + ", ".join(f"{k} {COVER[k]}" for k in sorted(COVER)))
-    assert REQUIRED <= set(COVER), sorted(REQUIRED - set(COVER))
+    check_coverage(COVER, REQUIRED, "attention")
 
 
 # ------------------------------------------------------------------------------------------------ host guards
@@ -958,7 +891,7 @@ def test_signature_dedups_cpu():
     base = torch.zeros(2 * 64 * 320 + 8, dtype=torch.float16)
     o0 = base[:2 * 64 * 320].view(2, 64, 320)
     o2 = base[2:2 + 2 * 64 * 320].view(2, 64, 320)
-    assert s(out=o2) != s(out=o0) and _attn_sig(qk[:, :, :320], qk[:, :, 320:], vt, out=o2, **kw)["oo"] == (_eoff(base) + 2) % 8
+    assert s(out=o2) != s(out=o0) and _attn_sig(qk[:, :, :320], qk[:, :, 320:], vt, out=o2, **kw)["oo"] == (eoff(base) + 2) % 8
     ow = torch.zeros(2, 64, 326, dtype=torch.float16)[:, :, :320]
     assert _attn_sig(qk[:, :, :320], qk[:, :, 320:], vt, out=ow, **kw)["ldo"] == 326
     assert signature(dict(p, fam=("randn1",))) == signature(p)

@@ -12,6 +12,7 @@ import torch
 import helpers  # noqa: F401
 from helpers import golden, rel_l2
 from sdb200 import arch, ops
+from workloads import GEMM_MODEL_WORKLOADS
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(1800)]
 UCFG = {"tiny": arch.TINY_CIN_F8_UNET, "cin256": arch.CIN256_F8_UNET}
@@ -238,23 +239,11 @@ def test_sample_imagenet_script_cin256_tiny(cuda_dev, tmp_path):
 
 
 # ------------------------------------------------------------------------------------------------ GEMM plans
-def test_every_plan_of_every_cin256_gemm_problem(cuda_dev, monkeypatch):
+def test_every_plan_of_every_cin256_gemm_problem(cuda_dev):
     """The cin256 UNet at (6, 4, 32, 32) (the unguided batch of bench_cin.py) and the VQ-f8 decoder at 256²."""
-    from test_gemm_plans_gpu import Recorder, run_sweep
-    rec = Recorder(ops.gemm)
-    monkeypatch.setattr(ops, "AUTOTUNE", False)
-    monkeypatch.setattr(ops, "TUNED", {})
-    monkeypatch.setattr(ops, "gemm", rec)
-    gen = torch.Generator(device=cuda_dev).manual_seed(0)
-    with torch.no_grad():
-        u = _unet("cin256", cuda_dev)
-        c = torch.randn(6, 1, 512, generator=gen, device=cuda_dev)
-        u(torch.randn(6, 4, 32, 32, generator=gen, device=cuda_dev), torch.linspace(1, 981, 6, device=cuda_dev).round(),
-          context=c)
-        _vq("vq_f8", cuda_dev).decode(torch.randn(1, 4, 32, 32, generator=gen, device=cuda_dev))
-    monkeypatch.setattr(ops, "gemm", rec.orig)
-    torch.cuda.synchronize()
-    print(f"\ncin256 UNet (6, 4, 32²) and VQ-f8 decoder (1, 4, 32²): {len(rec.problems)} distinct GEMM problems")
-    assert rec.problems
-    run_sweep(rec.problems, cuda_dev, "cin256")
+    from test_gemm_plans_gpu import catalogue, run_sweep
+    problems = catalogue(GEMM_MODEL_WORKLOADS["cin256_f8"], cuda_dev)
+    print(f"\ncin256 UNet (6, 4, 32²) and VQ-f8 decoder (1, 4, 32²): {len(problems)} distinct GEMM problems")
+    assert problems
+    run_sweep(problems, cuda_dev, "cin256")
     torch.cuda.empty_cache()

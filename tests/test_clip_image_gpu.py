@@ -16,6 +16,7 @@ import helpers
 from helpers import golden, rel_l2
 from sdb200 import arch, ops
 from sdb200.clip_image import _table
+from workloads import GEMM_MODEL_WORKLOADS
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(1800)]
 
@@ -206,24 +207,11 @@ def test_build_database_search_and_knn2img(cuda_dev, tmp_path):
 
 
 # ------------------------------------------------------------------------------------------------ GEMM plans
-def test_every_plan_of_the_tower_gemm_problems(cuda_dev, monkeypatch):
+def test_every_plan_of_the_tower_gemm_problems(cuda_dev):
     """The ViT-L/14 tower's GEMMs at B = 1, 64 and 256 images (M = 256 B patch rows, 257 B token rows)."""
-    from test_gemm_plans_gpu import Recorder, run_sweep
-    emb = _embedder(arch.CLIP_VISION_PROJ, cuda_dev)
-    rec = Recorder(ops.gemm)
-    monkeypatch.setattr(ops, "AUTOTUNE", False)
-    monkeypatch.setattr(ops, "TUNED", {})
-    monkeypatch.setattr(ops, "gemm", rec)
-    g = torch.Generator(device=cuda_dev).manual_seed(0)
-    with torch.no_grad():
-        for B in (1, 64, 256):
-            patches = torch.randn(B * 256, emb.W["kpad"], generator=g, device=cuda_dev).half()
-            emb.embed_patches(patches, B)
-    monkeypatch.setattr(ops, "gemm", rec.orig)
-    torch.cuda.synchronize()
-    del emb
-    torch.cuda.empty_cache()
-    print(f"\nCLIP ViT-L/14 image tower at B = 1, 64, 256: {len(rec.problems)} distinct GEMM problems")
-    assert rec.problems
-    run_sweep(rec.problems, cuda_dev, "clip_image")
+    from test_gemm_plans_gpu import catalogue, run_sweep
+    problems = catalogue(GEMM_MODEL_WORKLOADS["clip_image"], cuda_dev)
+    print(f"\nCLIP ViT-L/14 image tower at B = 1, 64, 256: {len(problems)} distinct GEMM problems")
+    assert problems
+    run_sweep(problems, cuda_dev, "clip_image")
     torch.cuda.empty_cache()

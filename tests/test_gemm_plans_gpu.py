@@ -20,7 +20,7 @@ Bounds (calibrated on the default plans; the largest observed ratio is printed p
                    rel-L2 < REL_L2 * max(1, sqrt(K / 4608)): the unsplit plans of the 3x3 convs over the widest skip
                    concats (K = 9 x 2560 = 23040) reach 1.5e-5, default plans included
   fp16 output      |out - ref| <= ulp16(ref) + TAU * absref
-  SILU/QUICK_GELU  |out - ref| <= 1.2 TAU * absref + ACT_REL * |v| (+ one fp16 ulp for fp16 outputs)
+  SILU/QUICK_GELU/GELU  |out - ref| <= 1.2 TAU * absref + ACT_REL * |v| (+ one fp16 ulp for fp16 outputs)
   GEGLU            |out - ref| <= ulp16 + TAU (|gelu(g)| absref_x + 1.2 |x| absref_g) + ACT_REL |x| (|g| + 1)
   hi/lo            hi == fp16(f32); |hi + lo - f32| <= 2e-6 |f32| + 6e-8
   statistics       every slot finite, T as sdb_gemm_plan reports it, and the slots summed over T within 1e-5 of the
@@ -28,7 +28,6 @@ Bounds (calibrated on the default plans; the largest observed ratio is printed p
 """
 import ctypes as C
 import math
-import time
 from collections import defaultdict
 
 import pytest
@@ -39,9 +38,10 @@ import helpers  # noqa: F401  (puts the repository on sys.path)
 from helpers import rel_l2
 from sdb200 import arch, ops
 from sdb200 import lib as _l
-from sdb200.lib import ACT_GEGLU, ACT_NONE, ACT_QUICK_GELU, ACT_SILU
+from sdb200.lib import ACT_GEGLU, ACT_GELU, ACT_NONE, ACT_QUICK_GELU, ACT_SILU
+from sweeps import NAN, Tally, check_coverage, eoff, record, ulp16
+from workloads import GEMM_WORKLOADS, _unet
 
-NAN = float("nan")
 TAU = 1e-5        # elementwise bound of the fp32 accumulation, relative to the abs-value reference
 REL_L2 = 1e-5     # rel-L2 of fp32 outputs for K <= 4608, growing as sqrt(K) beyond (one 64-deep wgmma K step after another)
 ACT_REL = 4e-6    # __expf / rcp.approx / erf polynomial inside the epilogue activations, relative to |v|
@@ -117,6 +117,8 @@ def act_ref(v, av, act, bn):
     if act in (ACT_SILU, ACT_QUICK_GELU):
         s = 1.702 if act == ACT_QUICK_GELU else 1.0
         return v * torch.sigmoid(s * v), 1.2 * TAU * av + ACT_REL * v.abs()
+    if act == ACT_GELU:     # exact GELU; its slope is within [-0.17, 1.13], bound as SILU's
+        return _gelu64(v), 1.2 * TAU * av + ACT_REL * v.abs()
     M, n = v.shape      # GEGLU: each accumulator tile of bn columns is [bn/2 values | bn/2 gates]
     vv, aa = v.view(M, n // bn, 2, bn // 2), av.view(M, n // bn, 2, bn // 2)
     x, g, ax, ag = vv[:, :, 0], vv[:, :, 1], aa[:, :, 0], aa[:, :, 1]
@@ -125,18 +127,7 @@ def act_ref(v, av, act, bn):
     return out, bound.reshape(M, n // 2)
 
 
-def ulp16(x):
-    """Spacing of fp16 numbers at |x| (subnormal spacing below 2^-14)."""
-    e = torch.floor(torch.log2(x.abs().clamp_min(2.0 ** -14)))
-    return torch.exp2(e - 10)
-
-
 # ------------------------------------------------------------------------------------------------ problem catalogue
-def _eoff(t):
-    """Element offset of t's data from the nearest 16-byte boundary (alignment is what fast_possible tests)."""
-    return (t.data_ptr() % 16) // t.element_size()
-
-
 def signature(a0, b, kw):
     """Everything of one ops.gemm call that reaches the plan or the kernel, as a hashable tuple of items."""
     srcs = [a0] + [kw[k] for k in ("a1", "a2", "a3") if kw.get(k) is not None]
@@ -156,27 +147,18 @@ def signature(a0, b, kw):
         bias=kw.get("bias") is not None,
         film=None if film is None else (film.stride(0), film.storage_offset() % film.stride(0), film.shape[0]),
         rps=kw.get("rows_per_sample", 0),
-        res=None if res is None else (res.stride(0), _eoff(res)),
+        res=None if res is None else (res.stride(0), eoff(res)),
         act=act, f16=f16, f32=f32, lo=lo,
-        out_off=tuple(_eoff(kw[k]) if kw.get(k) is not None else 0 for k in ("out_f16", "out_f32", "out_f16_lo")),
+        out_off=tuple(eoff(kw[k]) if kw.get(k) is not None else 0 for k in ("out_f16", "out_f32", "out_f16_lo")),
         alpha=float(kw.get("alpha", 1.0)), stats=bool(kw.get("want_stats", False)), sg=kw.get("stats_group", 1),
         splits=kw.get("splits", 0), block_n=kw.get("block_n", 0), pair=kw.get("pair", 0),
         splitk_mode=kw.get("splitk_mode", 0))
     return tuple(sorted(p.items()))
 
 
-class Recorder:
-    """Wraps ops.gemm (through monkeypatch) and keeps the deduplicated signatures in call order."""
-
-    def __init__(self, orig):
-        self.orig, self.seen, self.problems = orig, set(), []
-
-    def __call__(self, a0, b, **kw):
-        s = signature(a0, b, kw)
-        if s not in self.seen:
-            self.seen.add(s)
-            self.problems.append(dict(s))
-        return self.orig(a0, b, **kw)
+def catalogue(workload, dev):
+    """The distinct ops.gemm problems of one run of workload(dev), in first-call order."""
+    return record(workload, dev, {"gemm": lambda a0, b, **kw: dict(signature(a0, b, kw))})[1]
 
 
 def label(p):
@@ -192,7 +174,7 @@ def label(p):
     if p["rps"]:
         bits.append(f"rps={p['rps']}")
     if p["act"]:
-        bits.append({1: "geglu", 2: "qgelu", 3: "silu"}[p["act"]])
+        bits.append({1: "geglu", 2: "qgelu", 3: "silu", 4: "gelu"}[p["act"]])
     if p["alpha"] != 1.0:
         bits.append(f"alpha={p['alpha']:g}")
     bits.append("out=" + "".join(k for k in ("f16", "f32", "lo") if p[k]))
@@ -544,118 +526,26 @@ def run_sweep(problems, dev, title):
     sms = _l.load().sdb_sm_count()
     ws = torch.empty(ops.WS_FLOATS, dtype=torch.float32, device=dev)
     arena = ops.StatsArena(dev, 8 * 1024 * 1024)
-    failures, calib = [], {}
-    t0 = time.time()
-    launches = 0
+    tally, calib = Tally(title, "problem, plan, check, value"), {}
     saved = (ops.AUTOTUNE, ops.TUNED, ops.ARENA)
     ops.AUTOTUNE, ops.TUNED, ops.ARENA = False, {}, arena
     try:
         for i, p in enumerate(problems):
             X = Operands(p, dev, 1000 + i)
-            launches += sweep_problem(X, failures, calib, sms, ws, arena)
+            tally.launches += sweep_problem(X, tally.failures, calib, sms, ws, arena)
             del X
     finally:
         ops.AUTOTUNE, ops.TUNED, ops.ARENA = saved
-    torch.cuda.synchronize()
-    dt = time.time() - t0
-    print(f"\n{title}: {len(problems)} problems, {launches} launches, {dt:.1f} s; largest share of each bound used (default plans / all plans): "
-          + ", ".join(f"{k} {v:.2f}" for k, v in sorted(calib.items())))
-    if failures:
-        rows = "\n".join(" | ".join(map(str, f)) for f in failures[:200])
-        pytest.fail(f"{title}: {len(failures)} failing (problem, plan, check, value):\n{rows}")
-    return launches
+    tally.finish(len(problems), "largest share of each bound used (default plans / all plans): "
+                 + ", ".join(f"{k} {v:.2f}" for k, v in sorted(calib.items())))
 
 
 # ------------------------------------------------------------------------------------------------ model workloads
-def _unet(cfg, dev, seed=11):
-    import sdb200
-    return sdb200.UNetModel(**cfg).load_weights(arch.random_state_dict(arch.unet_param_shapes(cfg), seed, device=dev), dev)
-
-
-def _run_unet(cfg, shapes, dev, ctx=None, concat=False):
-    net = _unet(cfg, dev)
-    g = torch.Generator(device=dev).manual_seed(0)
-    for s in shapes:
-        x = torch.randn(*s, generator=g, device=dev)
-        t = torch.linspace(1, 981, s[0], device=dev).round()
-        c = None if ctx is None else torch.randn(s[0], *ctx, generator=g, device=dev)
-        if concat:
-            net(x[:, :3].contiguous(), t, concat=x[:, 3:].contiguous())
-        else:
-            net(x, t, context=c)
-    del net
-
-
-def _wl_sdv1_unet(dev, shapes):
-    _run_unet(arch.SD_V1_UNET, shapes, dev, ctx=(77, 768))
-
-
-def _wl_sdv1_first(dev):
-    import sdb200
-    vae = sdb200.AutoencoderKL(**arch.SD_V1_VAE).load_weights(
-        arch.random_state_dict(arch.vae_param_shapes(arch.SD_V1_VAE), 12, device=dev), dev)
-    g = torch.Generator(device=dev).manual_seed(1)
-    vae.decode(torch.randn(1, 4, 64, 64, generator=g, device=dev))
-    vae.encode(torch.rand(1, 3, 512, 512, generator=g, device=dev) * 2 - 1)
-    del vae
-    clip = sdb200.FrozenCLIPEmbedder(config=arch.SD_V1_CLIP).load_weights(
-        arch.random_state_dict(arch.clip_param_shapes(arch.SD_V1_CLIP), 13, device=dev), dev)
-    clip.encode_ids(torch.randint(0, 49408, (2, 77), generator=g, device=dev))
-    del clip
-    chk = sdb200.StableDiffusionSafetyChecker(config=arch.SD_V1_SAFETY).load_weights(
-        arch.random_state_dict(arch.safety_param_shapes(arch.SD_V1_SAFETY), 14, device=dev), dev)
-    chk.image_embeds(torch.randn(1, 3, 224, 224, generator=g, device=dev))
-    del chk
-
-
-def _vq(cfg, dev):
-    import sdb200
-    return sdb200.VQModelInterface(**cfg).load_weights(arch.random_state_dict(arch.vq_param_shapes(cfg), 12, device=dev), dev)
-
-
-def _wl_celebahq(dev):
-    _run_unet(arch.CELEBAHQ_UNET, [(10, 3, 64, 64)], dev)
-    g = torch.Generator(device=dev).manual_seed(2)
-    _vq(arch.VQ_F4, dev).decode(torch.randn(1, 3, 64, 64, generator=g, device=dev))
-
-
-def _wl_inpaint(dev):
-    _run_unet(arch.INPAINTING_BIG_UNET, [(1, 7, 128, 128), (4, 7, 128, 128)], dev, concat=True)
-    g = torch.Generator(device=dev).manual_seed(3)
-    m = _vq(arch.VQ_F4_NOATTN, dev)
-    m.encode(torch.rand(1, 3, 512, 512, generator=g, device=dev) * 2 - 1)
-    m.decode(torch.randn(1, 3, 128, 128, generator=g, device=dev))
-
-
-WORKLOADS = {
-    "sdv1_unet_b2": lambda dev: _wl_sdv1_unet(dev, [(2, 4, 64, 64), (2, 4, 64, 96), (2, 4, 96, 64)]),
-    "sdv1_unet_b16": lambda dev: _wl_sdv1_unet(dev, [(16, 4, 64, 64)]),
-    "sdv1_vae_clip_safety": _wl_sdv1_first,
-    "lsun": lambda dev: _run_unet(arch.LSUN_CHURCHES_UNET, [(10, 4, 32, 32)], dev),
-    "celebahq": _wl_celebahq,
-    "cin256": lambda dev: _run_unet(arch.CIN256_V2_UNET, [(12, 3, 64, 64), (2, 3, 32, 32)], dev, ctx=(1, 512)),
-    "inpaint": _wl_inpaint,
-}
-
-
-def catalogue(name, dev, monkeypatch):
-    rec = Recorder(ops.gemm)
-    monkeypatch.setattr(ops, "AUTOTUNE", False)
-    monkeypatch.setattr(ops, "TUNED", {})
-    monkeypatch.setattr(ops, "gemm", rec)
-    with torch.no_grad():
-        WORKLOADS[name](dev)
-    monkeypatch.setattr(ops, "gemm", rec.orig)
-    torch.cuda.synchronize()
-    torch.cuda.empty_cache()
-    return rec.problems
-
-
 @pytest.mark.gpu
 @pytest.mark.timeout(900)
-@pytest.mark.parametrize("name", list(WORKLOADS))
-def test_every_plan_of_every_model_problem(cuda_dev, monkeypatch, name):
-    problems = catalogue(name, cuda_dev, monkeypatch)
+@pytest.mark.parametrize("name", list(GEMM_WORKLOADS))
+def test_every_plan_of_every_model_problem(cuda_dev, name):
+    problems = catalogue(GEMM_WORKLOADS[name], cuda_dev)
     print(f"\n{name}: {len(problems)} distinct GEMM problems")
     assert problems
     run_sweep(problems, cuda_dev, name)
@@ -743,11 +633,8 @@ def test_row_stride_beyond_output_width_keeps_guard_columns(cuda_dev):
 def test_branch_coverage_and_tuner_key():
     """Every branch class of sdb_gemm was launched by the sweeps above, and problems that share an autotuner cache key
     accept the same candidates (checked while sweeping; a collision is reported there)."""
-    if not COVER:
-        pytest.skip("the plan sweeps did not run in this session")
-    print("\ncoverage: " + ", ".join(f"{k} {COVER[k]}" for k in sorted(COVER)))
+    check_coverage(COVER, REQUIRED, "plan")
     print(f"tuner keys: {len(TUNER_KEYS)}, shared by two or more problems: {len(SHARED_KEYS)}")
-    assert REQUIRED <= set(COVER), sorted(REQUIRED - set(COVER))
 
 
 # ------------------------------------------------------------------------------------------------ ops.gemm layouts

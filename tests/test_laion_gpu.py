@@ -14,6 +14,7 @@ import test_gemm_plans_gpu as GP
 from helpers import golden, rel_l2
 from sdb200 import arch, ops
 from sdb200.lib import ACT_GELU
+from workloads import GEMM_MODEL_WORKLOADS
 
 pytestmark = pytest.mark.gpu
 BCFG = {"tiny": arch.TINY_BERT, "full": arch.LAION_BERT}
@@ -134,50 +135,15 @@ def test_gelu_epilogue_against_fp64(cuda_dev, f16):
 
 
 # ------------------------------------------------------------------------------------------------ GEMM plan sweep
-def _act_ref(orig):
-    def act_ref(v, av, act, bn):
-        if act == ACT_GELU:     # exact GELU in fp64; its slope is within [-0.17, 1.13], bound as SILU's
-            return 0.5 * v * (1.0 + torch.erf(v * 0.5 ** 0.5)), 1.2 * GP.TAU * av + GP.ACT_REL * v.abs()
-        return orig(v, av, act, bn)
-    return act_ref
-
-
-def _label(orig):
-    return lambda p: orig(dict(p, act=0)) + " gelu" if p["act"] == ACT_GELU else orig(p)
-
-
-@pytest.fixture
-def gelu_sweep(monkeypatch):
-    monkeypatch.setattr(GP, "act_ref", _act_ref(GP.act_ref))
-    monkeypatch.setattr(GP, "label", _label(GP.label))
-
-
-def _wl_laion(dev):
-    import sdb200
-    emb = sdb200.BERTEmbedder(**arch.LAION_BERT, use_tokenizer=False).load_weights(
-        arch.random_state_dict(arch.bert_param_shapes(arch.LAION_BERT), 13, device=dev), dev)
-    g = torch.Generator(device=dev).manual_seed(4)
-    emb.encode_ids(torch.randint(0, 30522, (6, 77), generator=g, device=dev))      # cond + uncond of batch 3
-    del emb
-    GP._run_unet(arch.LAION_UNET, [(2, 4, 64, 64), (6, 4, 64, 64)], dev, ctx=(77, 1280))
-
-
 @pytest.mark.timeout(900)
-def test_every_plan_of_every_laion_gemm_problem(cuda_dev, monkeypatch, gelu_sweep):
-    rec = GP.Recorder(ops.gemm)
-    monkeypatch.setattr(ops, "AUTOTUNE", False)
-    monkeypatch.setattr(ops, "TUNED", {})
-    monkeypatch.setattr(ops, "gemm", rec)
-    with torch.no_grad():
-        _wl_laion(cuda_dev)
-    monkeypatch.setattr(ops, "gemm", rec.orig)
-    torch.cuda.synchronize()
-    torch.cuda.empty_cache()
-    gelu = [p for p in rec.problems if p["act"] == ACT_GELU]
-    print(f"\nLAION BERT (6 x 77 tokens) + UNet (2 and 6, 4, 64²), context (77, 1280): {len(rec.problems)} distinct GEMM "
+def test_every_plan_of_every_laion_gemm_problem(cuda_dev):
+    """BERT on the cond + uncond ids of a batch of 3, then the UNet at batches 2 and 6."""
+    problems = GP.catalogue(GEMM_MODEL_WORKLOADS["laion"], cuda_dev)
+    gelu = [p for p in problems if p["act"] == ACT_GELU]
+    print(f"\nLAION BERT (6 x 77 tokens) + UNet (2 and 6, 4, 64²), context (77, 1280): {len(problems)} distinct GEMM "
           f"problems, {len(gelu)} with ACT_GELU")
     assert gelu and any(p["chans"] == (1280,) and p["n"] == 1280 * 4 for p in gelu)
-    GP.run_sweep(rec.problems, cuda_dev, "laion")
+    GP.run_sweep(problems, cuda_dev, "laion")
     torch.cuda.empty_cache()
 
 
@@ -192,5 +158,5 @@ GELU_SYNTHETIC = {
 
 
 @pytest.mark.timeout(600)
-def test_every_plan_of_synthetic_gelu_problems(cuda_dev, gelu_sweep):
+def test_every_plan_of_synthetic_gelu_problems(cuda_dev):
     GP.run_sweep(list(GELU_SYNTHETIC.values()), cuda_dev, "gelu synthetic")

@@ -27,7 +27,6 @@ The largest share of each bound used is printed per workload.
 """
 import ctypes as C
 import math
-import time
 from collections import defaultdict
 
 import pytest
@@ -37,28 +36,16 @@ import torch.nn.functional as F
 import helpers  # noqa: F401  (puts the repository on sys.path)
 from sdb200 import ops
 from sdb200 import lib as _l
+from sweeps import GUARD, NAN, Tally, check_coverage, eoff, record, signature, ulp16
 from workloads import WORKLOADS
 
-NAN = float("nan")
 TAU_N = 8e-6       # GroupNorm: statistics and apply, relative to |z||g| + |b|
 TAU_L = 4e-6       # LayerNorm: fp32 two-pass statistics in one warp
 APPLY_REL = 3e-7   # fp32 rounding of a = rstd g, b = beta - mean a and x a + b, relative to (|x| + |mean|) rstd |g|
 ACT_REL = 4e-6     # __expf / __fdividef inside SiLU, relative to |v|
-GUARD = 16         # NaN elements before and after every output
 GN_MAX_SLABS = 128
 LN_V2 = {320: 5, 512: 8, 640: 10, 768: 12, 1280: 20}
 LN_NPL = (2, 4, 10, 20, 24, 40, 48, 56)
-
-
-def ulp16(x):
-    """Spacing of fp16 numbers at |x| (subnormal spacing below 2^-14)."""
-    e = torch.floor(torch.log2(x.abs().clamp_min(2.0 ** -14)))
-    return torch.exp2(e - 10)
-
-
-def _eoff(t):
-    """Element offset of t's data from the nearest 16-byte boundary."""
-    return (t.data_ptr() % 16) // t.element_size()
 
 
 # ------------------------------------------------------------------------------------------------ host dispatch mirror
@@ -162,7 +149,7 @@ def _gn_sig(x0, gamma, beta, *, x1=None, groups=32, eps=1e-5, silu=False, want_r
     if not (cs0 is None or (x1 is not None and (cs1 is None or cs1[2] != sg)) or cpg % sg or c0 % sg or c1 % sg):
         stats = (cs0[1], cs1[1] if cs1 else 0, sg)
     return _gn(nb=nb, h=h, w=w, c0=c0, c1=c1, groups=groups, eps=eps, silu=bool(silu), raw=want_raw or want_raw_lo,
-               lo=want_lo, raw_lo=want_raw_lo, stats=stats, a0=_eoff(x0), a1=_eoff(x1) if x1 is not None else 0)
+               lo=want_lo, raw_lo=want_raw_lo, stats=stats, a0=eoff(x0), a1=eoff(x1) if x1 is not None else 0)
 
 
 def _gnmod_sig(x, gamma, beta, *, scale=None, shift=None, resample=0, groups=32, eps=1e-5, silu=True):
@@ -172,42 +159,20 @@ def _gnmod_sig(x, gamma, beta, *, scale=None, shift=None, resample=0, groups=32,
     if cs is not None and not ((c // groups) % cs[2] or c % cs[2]):
         stats = (cs[1], 0, cs[2])
     return _gn(kind="gnmod", nb=nb, h=h, w=w, c0=c, groups=groups, eps=eps, silu=bool(silu), stats=stats,
-               ldm=scale.stride(0) if scale is not None else 0, resample=resample, a0=_eoff(x))
+               ldm=scale.stride(0) if scale is not None else 0, resample=resample, a0=eoff(x))
 
 
 def _ln_sig(x, gamma, beta, eps=1e-5, want_f32=False):
     c = x.shape[-1]
-    return _ln(rows=x.numel() // c, c=c, eps=eps, f32=bool(want_f32), align=(_eoff(x), _eoff(gamma), _eoff(beta), 0))
+    return _ln(rows=x.numel() // c, c=c, eps=eps, f32=bool(want_f32), align=(eoff(x), eoff(gamma), eoff(beta), 0))
 
 
 def _sm_sig(x, scale):
     cols = x.shape[-1]
-    return _sm(rows=x.numel() // cols, cols=cols, scale=float(scale), align=_eoff(x))
+    return _sm(rows=x.numel() // cols, cols=cols, scale=float(scale), align=eoff(x))
 
 
 SIGS = {"groupnorm": _gn_sig, "groupnorm_mod": _gnmod_sig, "layernorm": _ln_sig, "softmax_rows": _sm_sig}
-
-
-def signature(p):
-    return tuple(sorted(p.items()))
-
-
-class Recorder:
-    """Wraps the four ops entry points (through monkeypatch) and keeps the deduplicated problems in call order."""
-
-    def __init__(self):
-        self.seen, self.problems, self.calls = set(), [], 0
-
-    def wrap(self, name, fn):
-        def rec(*a, **kw):
-            p = SIGS[name](*a, **kw)
-            self.calls += 1
-            s = signature(p)
-            if s not in self.seen:
-                self.seen.add(s)
-                self.problems.append(p)
-            return fn(*a, **kw)
-        return rec
 
 
 def label(p):
@@ -426,12 +391,12 @@ def check_ln(p, x, gamma, beta, o16, o32):
     return r
 
 
-class Sweep:
+class Sweep(Tally):
     """Failures and calibration of one title (workload or synthetic group)."""
 
     def __init__(self, title):
-        self.title, self.failures, self.calib, self.launches, self.t0 = title, [], {}, 0, time.time()
-        self.sms = _l.load().sdb_sm_count()
+        super().__init__(title)
+        self.calib, self.sms = {}, _l.load().sdb_sm_count()
 
     def record(self, lab, r, same):
         if not same:
@@ -525,49 +490,29 @@ class Sweep:
     def run(self, p, seed):
         return {"gn": self.gn, "gnmod": self.gn, "ln": self.ln, "softmax": self.softmax}[p["kind"]](p, seed)
 
-    def finish(self, n_problems):
-        torch.cuda.synchronize()
-        print(f"\n{self.title}: {n_problems} problems, {self.launches} launches, {time.time() - self.t0:.1f} s; largest "
-              "share of each bound used: " + ", ".join(f"{k} {v:.3f}" for k, v in sorted(self.calib.items())))
-        if self.failures:
-            rows = "\n".join(" | ".join(map(str, f)) for f in self.failures[:200])
-            pytest.fail(f"{self.title}: {len(self.failures)} failing (problem, check, value):\n{rows}")
+    def calibration(self):
+        return "largest share of each bound used: " + ", ".join(f"{k} {v:.3f}" for k, v in sorted(self.calib.items()))
 
 
 def run_sweep(problems, title):
     sw = Sweep(title)
     for i, p in enumerate(problems):
         sw.run(p, 1000 + i)
-    sw.finish(len(problems))
-    return sw
+    sw.finish(len(problems), sw.calibration())
 
 
 # ------------------------------------------------------------------------------------------------ model workloads
-def catalogue(name, dev, monkeypatch):
-    rec = Recorder()
-    monkeypatch.setattr(ops, "AUTOTUNE", False)
-    monkeypatch.setattr(ops, "TUNED", {})
-    for fn in SIGS:
-        monkeypatch.setattr(ops, fn, rec.wrap(fn, getattr(ops, fn)))
-    with torch.no_grad():
-        WORKLOADS[name](dev)
-    torch.cuda.synchronize()
-    monkeypatch.undo()
-    torch.cuda.empty_cache()
-    return rec
-
-
 @pytest.mark.gpu
 @pytest.mark.timeout(600)
 @pytest.mark.parametrize("name", list(WORKLOADS))
-def test_every_norm_launch_of_every_model(cuda_dev, monkeypatch, name):
-    rec = catalogue(name, cuda_dev, monkeypatch)
+def test_every_norm_launch_of_every_model(cuda_dev, name):
+    calls, problems = record(WORKLOADS[name], cuda_dev, SIGS)
     kinds = defaultdict(int)
-    for p in rec.problems:
+    for p in problems:
         kinds[p["kind"]] += 1
-    print(f"\n{name}: {rec.calls} calls, {len(rec.problems)} distinct problems ({dict(kinds)})")
-    assert rec.problems
-    run_sweep(rec.problems, name)
+    print(f"\n{name}: {calls} calls, {len(problems)} distinct problems ({dict(kinds)})")
+    assert problems
+    run_sweep(problems, name)
     torch.cuda.empty_cache()
 
 
@@ -661,7 +606,7 @@ def test_groupnorm_conditioning(cuda_dev):
                 outs = X.outputs()
                 X.launch(outs)
                 fused_beyond[(hw, ratio)] = check_gn(X, outs)["gn_elem"]
-    sw.finish(20)
+    sw.finish(20, sw.calibration())
     print("fused statistics at mean/std 256 (not asserted), share of the bound: "
           + ", ".join(f"hw {k[0]} ratio {k[1]:g}: {v:.2f}" for k, v in sorted(fused_beyond.items())))
 
@@ -669,10 +614,7 @@ def test_groupnorm_conditioning(cuda_dev):
 @pytest.mark.gpu
 def test_norm_branch_coverage():
     """Every dispatch branch of norm.cu was launched by the sweeps above."""
-    if not COVER:
-        pytest.skip("the norm sweeps did not run in this session")
-    print("\ncoverage: " + ", ".join(f"{k} {COVER[k]}" for k in sorted(COVER)))
-    assert REQUIRED <= set(COVER), sorted(REQUIRED - set(COVER))
+    check_coverage(COVER, REQUIRED, "norm")
 
 
 # ------------------------------------------------------------------------------------------------ host guards
@@ -797,7 +739,7 @@ def test_signature_dedups_cpu():
     assert signature(_gn_sig(torch.zeros(2, 4, 4, 321)[..., 1:].contiguous(), gm, gm)) == s()
     base = torch.zeros(2 * 16 * 320 + 4)
     off = base[1:1 + 2 * 16 * 320].view(2, 4, 4, 320)
-    assert _gn_sig(off, gm, gm)["a0"] == (_eoff(base) + 1) % 4 and signature(_gn_sig(off, gm, gm)) != s()
+    assert _gn_sig(off, gm, gm)["a0"] == (eoff(base) + 1) % 4 and signature(_gn_sig(off, gm, gm)) != s()
     x._sdb_stats = (torch.zeros(1), 7, 10)
     p = _gn_sig(x, gm, gm)
     assert p["stats"] == (7, 0, 10) and "stats(T7,0,sg10)" in label(p)

@@ -13,6 +13,7 @@ import helpers  # noqa: F401
 import rdm_oracle as RO
 from helpers import golden, rel_l2
 from sdb200 import arch, ops
+from workloads import GEMM_MODEL_WORKLOADS
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(1800)]
 UCFG = {"tiny": arch.TINY_RDM_UNET, "rdm": arch.RDM_UNET}
@@ -372,24 +373,12 @@ def test_knn2img_script_tiny(cuda_dev, tmp_path, monkeypatch, neighbors):
 
 
 # ------------------------------------------------------------------------------------------------ GEMM plans
-def test_every_plan_of_every_rdm_gemm_problem(cuda_dev, monkeypatch):
+def test_every_plan_of_every_rdm_gemm_problem(cuda_dev):
     """The RDM UNet at (6, 16, 48, 48) with an 11-token context (knn2img's guided batch of 3) and the KL-f16 decoder at
     a 24x24 latent (the decoder's widths at a smaller image)."""
-    from test_gemm_plans_gpu import Recorder, run_sweep
-    rec = Recorder(ops.gemm)
-    monkeypatch.setattr(ops, "AUTOTUNE", False)
-    monkeypatch.setattr(ops, "TUNED", {})
-    monkeypatch.setattr(ops, "gemm", rec)
-    gen = torch.Generator(device=cuda_dev).manual_seed(0)
-    with torch.no_grad():
-        u = _unet("rdm", cuda_dev)
-        c = torch.randn(6, 11, 768, generator=gen, device=cuda_dev)
-        u(torch.randn(6, 16, 48, 48, generator=gen, device=cuda_dev), torch.linspace(1, 981, 6, device=cuda_dev).round(),
-          context=c)
-        _kl("kl_f16", cuda_dev).decode(torch.randn(1, 16, 24, 24, generator=gen, device=cuda_dev))
-    monkeypatch.setattr(ops, "gemm", rec.orig)
-    torch.cuda.synchronize()
-    print(f"\nRDM UNet (6, 16, 48²) and KL-f16 decoder (1, 16, 24²): {len(rec.problems)} distinct GEMM problems")
-    assert rec.problems
-    run_sweep(rec.problems, cuda_dev, "rdm")
+    from test_gemm_plans_gpu import catalogue, run_sweep
+    problems = catalogue(GEMM_MODEL_WORKLOADS["rdm"], cuda_dev)
+    print(f"\nRDM UNet (6, 16, 48²) and KL-f16 decoder (1, 16, 24²): {len(problems)} distinct GEMM problems")
+    assert problems
+    run_sweep(problems, cuda_dev, "rdm")
     torch.cuda.empty_cache()

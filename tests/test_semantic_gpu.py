@@ -15,6 +15,7 @@ import helpers  # noqa: F401
 import semantic_oracle as SO
 from helpers import golden, rel_l2
 from sdb200 import arch, ops
+from workloads import GEMM_MODEL_WORKLOADS
 
 pytestmark = pytest.mark.gpu
 UCFG = {"tiny": arch.TINY_SEMANTIC_UNET, "big": arch.SEMANTIC_SYNTHESIS_UNET}
@@ -281,27 +282,10 @@ def test_script_writes_pngs(cuda_dev, tmp_path):
     assert Image.open(written[0]).size == (128, 64)
 
 
-def _wl_ss(dev):
-    import sdb200
-    u = sdb200.UNetModel(**arch.SEMANTIC_SYNTHESIS_UNET).load_weights(
-        arch.random_state_dict(arch.unet_param_shapes(arch.SEMANTIC_SYNTHESIS_UNET), 11, device=dev), dev)
-    g = torch.Generator(device=dev).manual_seed(0)
-    for nb, h, w in ((8, 64, 64), (1, 128, 128)):
-        x = torch.randn(nb, 3, h, w, generator=g, device=dev)
-        u(x, torch.linspace(1, 981, nb, device=dev).round(), concat=torch.randn(nb, 3, h, w, generator=g, device=dev))
-
-
-def test_every_plan_of_every_ss_gemm_problem(cuda_dev, monkeypatch):
-    from test_gemm_plans_gpu import Recorder, run_sweep
-    rec = Recorder(ops.gemm)
-    monkeypatch.setattr(ops, "AUTOTUNE", False)
-    monkeypatch.setattr(ops, "TUNED", {})
-    monkeypatch.setattr(ops, "gemm", rec)
-    with torch.no_grad():
-        _wl_ss(cuda_dev)
-    monkeypatch.setattr(ops, "gemm", rec.orig)
-    torch.cuda.synchronize()
-    print(f"\nsemantic-synthesis UNet (8, 3+3, 64²) and (1, 3+3, 128²): {len(rec.problems)} distinct GEMM problems")
-    assert rec.problems
-    run_sweep(rec.problems, cuda_dev, "semantic")
+def test_every_plan_of_every_ss_gemm_problem(cuda_dev):
+    from test_gemm_plans_gpu import catalogue, run_sweep
+    problems = catalogue(GEMM_MODEL_WORKLOADS["semantic"], cuda_dev)
+    print(f"\nsemantic-synthesis UNet (8, 3+3, 64²) and (1, 3+3, 128²): {len(problems)} distinct GEMM problems")
+    assert problems
+    run_sweep(problems, cuda_dev, "semantic")
     torch.cuda.empty_cache()

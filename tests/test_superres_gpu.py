@@ -13,6 +13,7 @@ import superres_oracle as S
 from helpers import golden, rel_l2
 from sdb200 import arch, diffusion, ops
 from sdb200.diffusion import split_geometry, split_tables
+from workloads import GEMM_MODEL_WORKLOADS
 
 pytestmark = pytest.mark.gpu
 UCFG = {"tiny": arch.TINY_BSR_UNET, "big": arch.BSR_SR_UNET}
@@ -256,32 +257,10 @@ def test_script_tiny_writes_4x_png(cuda_dev, tmp_path):
     assert Image.open(outdir / "a.png").size == (128, 96) and Image.open(outdir / "b.png").size == (768, 512)
 
 
-def _wl_bsr(dev):
-    import sdb200
-    u = sdb200.UNetModel(**arch.BSR_SR_UNET).load_weights(
-        arch.random_state_dict(arch.unet_param_shapes(arch.BSR_SR_UNET), 11, device=dev), dev)
-    g = torch.Generator(device=dev).manual_seed(0)
-    x = torch.randn(9, 3, 128, 128, generator=g, device=dev)
-    u(x, torch.linspace(1, 981, 9, device=dev).round(), concat=torch.randn(9, 3, 128, 128, generator=g, device=dev))
-    vq = sdb200.VQModelInterface(**arch.VQ_F4).load_weights(
-        arch.random_state_dict(arch.vq_param_shapes(arch.VQ_F4), 12, device=dev), dev)
-    # the tiled decode's tile batch: a 192² latent, 2 x 2 tiles of 128²
-    q = vq.post_quant(torch.randn(1, 3, 192, 192, generator=g, device=dev))
-    tiles, _ = ops.nchw_to_nhwc(ops.patch_unfold(ops.nhwc_to_nchw(q), (128, 128), (64, 64)))
-    vq._decoder(tiles)
-
-
-def test_every_plan_of_every_bsr_gemm_problem(cuda_dev, monkeypatch):
-    from test_gemm_plans_gpu import Recorder, run_sweep
-    rec = Recorder(ops.gemm)
-    monkeypatch.setattr(ops, "AUTOTUNE", False)
-    monkeypatch.setattr(ops, "TUNED", {})
-    monkeypatch.setattr(ops, "gemm", rec)
-    with torch.no_grad():
-        _wl_bsr(cuda_dev)
-    monkeypatch.setattr(ops, "gemm", rec.orig)
-    torch.cuda.synchronize()
-    print(f"\nbsr_sr UNet (9, 3+3, 128²) + tiled VQ-f4 decode: {len(rec.problems)} distinct GEMM problems")
-    assert rec.problems
-    run_sweep(rec.problems, cuda_dev, "bsr_sr")
+def test_every_plan_of_every_bsr_gemm_problem(cuda_dev):
+    from test_gemm_plans_gpu import catalogue, run_sweep
+    problems = catalogue(GEMM_MODEL_WORKLOADS["bsr_sr"], cuda_dev)
+    print(f"\nbsr_sr UNet (9, 3+3, 128²) + tiled VQ-f4 decode: {len(problems)} distinct GEMM problems")
+    assert problems
+    run_sweep(problems, cuda_dev, "bsr_sr")
     torch.cuda.empty_cache()

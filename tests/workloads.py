@@ -1,26 +1,32 @@
 """One eager forward of each model with random weights: the workloads whose kernel launches the sweeps record
-(test_norm_sweep_gpu.py, test_attention_sweep_gpu.py). WORKLOADS maps a name to a function of the device."""
+(test_norm_sweep_gpu.py, test_attention_sweep_gpu.py, test_gemm_plans_gpu.py and the GEMM plan sweeps in the model
+test files). Each table maps a name to a function of the device; a problem's operands are seeded by its index in the
+recorded list, so an entry's shapes and call order are part of what a sweep checks."""
 import torch
 
 import helpers  # noqa: F401  (puts the repository on sys.path)
-from sdb200 import arch
+from sdb200 import arch, ops
 
 
 def _sd(shapes_fn, cfg, seed, dev):
     return arch.random_state_dict(shapes_fn(cfg), seed, device=dev)
 
 
-def _run_unet(cfg, shapes, dev, ctx=None, concat=False):
+def _unet(cfg, dev):
     import sdb200
-    net = sdb200.UNetModel(**cfg).load_weights(_sd(arch.unet_param_shapes, cfg, 11, dev), dev)
+    return sdb200.UNetModel(**cfg).load_weights(_sd(arch.unet_param_shapes, cfg, 11, dev), dev)
+
+
+def _run_unet(cfg, shapes, dev, ctx=None, concat=0):
+    """One UNet evaluation per shape; concat > 0 passes the last `concat` channels as the concat conditioning."""
+    net = _unet(cfg, dev)
     g = torch.Generator(device=dev).manual_seed(0)
     for s in shapes:
         x = torch.randn(*s, generator=g, device=dev)
         t = torch.linspace(1, 981, s[0], device=dev).round()
         c = None if ctx is None else torch.randn(s[0], *ctx, generator=g, device=dev)
         if concat:
-            half = s[1] // 2 if concat is True else concat
-            net(x[:, :s[1] - half].contiguous(), t, concat=x[:, s[1] - half:].contiguous())
+            net(x[:, :s[1] - concat].contiguous(), t, concat=x[:, s[1] - concat:].contiguous())
         else:
             net(x, t, context=c)
     del net
@@ -50,10 +56,14 @@ def _bert(cfg, dev, ids):
                                                                  dev).encode_ids(ids)
 
 
-def _clip_image(cfg, dev, B):
+def _clip_image_embedder(cfg, dev):
     import sdb200
     e = sdb200.FrozenClipImageEmbedder("ViT-L/14", config=cfg)
-    e = e.load_weights(arch.random_state_dict(e.shapes, 16, device=dev), dev)
+    return e.load_weights(arch.random_state_dict(e.shapes, 16, device=dev), dev)
+
+
+def _clip_image(cfg, dev, B):
+    e = _clip_image_embedder(cfg, dev)
     g = torch.Generator(device=dev).manual_seed(5)
     e(torch.rand(B, 3, 224, 224, generator=g, device=dev) * 2 - 1)
 
@@ -76,34 +86,38 @@ def _wl_sdv1_first(dev):
     chk.image_embeds(torch.randn(1, 3, 224, 224, generator=g, device=dev))
 
 
-def _wl_laion(dev):
-    _bert(arch.LAION_BERT, dev, _ids(30522, 2, dev))
-    _run_unet(arch.LAION_UNET, [(2, 4, 64, 64)], dev, ctx=(77, 1280))
+def _wl_laion(dev, text_batch, unet_batches):
+    _bert(arch.LAION_BERT, dev, _ids(30522, text_batch, dev))
+    _run_unet(arch.LAION_UNET, [(nb, 4, 64, 64) for nb in unet_batches], dev, ctx=(77, 1280))
+
+
+def _wl_rdm_unet_kl(dev, nb):
+    g = torch.Generator(device=dev).manual_seed(2)
+    _run_unet(arch.RDM_UNET, [(nb, 16, 48, 48)], dev, ctx=(11, 768))
+    _vae(arch.KL_F16, dev).decode(torch.randn(1, 16, 24, 24, generator=g, device=dev))
 
 
 def _wl_rdm(dev):
-    g = torch.Generator(device=dev).manual_seed(2)
-    _run_unet(arch.RDM_UNET, [(2, 16, 48, 48)], dev, ctx=(11, 768))
-    _vae(arch.KL_F16, dev).decode(torch.randn(1, 16, 24, 24, generator=g, device=dev))
+    _wl_rdm_unet_kl(dev, 2)
     _clip(arch.CLIP_TEXT_PROJ, dev, _ids(49408, 2, dev))
     _clip_image(arch.CLIP_VISION_PROJ, dev, 2)
 
 
-def _wl_celebahq(dev):
+def _wl_celebahq(dev, nb):
     g = torch.Generator(device=dev).manual_seed(2)
-    _run_unet(arch.CELEBAHQ_UNET, [(2, 3, 64, 64)], dev)
+    _run_unet(arch.CELEBAHQ_UNET, [(nb, 3, 64, 64)], dev)
     _vq(arch.VQ_F4, dev).decode(torch.randn(1, 3, 64, 64, generator=g, device=dev))
 
 
-def _wl_cin_f8(dev):
+def _wl_cin_f8(dev, nb):
     g = torch.Generator(device=dev).manual_seed(2)
-    _run_unet(arch.CIN256_F8_UNET, [(2, 4, 32, 32)], dev, ctx=(1, 512))
+    _run_unet(arch.CIN256_F8_UNET, [(nb, 4, 32, 32)], dev, ctx=(1, 512))
     _vq(arch.VQ_F8, dev).decode(torch.randn(1, 4, 32, 32, generator=g, device=dev))
 
 
-def _wl_inpaint(dev):
+def _wl_inpaint(dev, batches):
     g = torch.Generator(device=dev).manual_seed(3)
-    _run_unet(arch.INPAINTING_BIG_UNET, [(1, 7, 128, 128)], dev, concat=4)
+    _run_unet(arch.INPAINTING_BIG_UNET, [(nb, 7, 128, 128) for nb in batches], dev, concat=4)
     m = _vq(arch.VQ_F4_NOATTN, dev)
     m.encode(torch.rand(1, 3, 512, 512, generator=g, device=dev) * 2 - 1)
     m.decode(torch.randn(1, 3, 128, 128, generator=g, device=dev))
@@ -113,6 +127,29 @@ def _wl_bsr(dev):
     g = torch.Generator(device=dev).manual_seed(3)
     _run_unet(arch.BSR_SR_UNET, [(1, 6, 128, 128)], dev, concat=3)
     _vq(arch.VQ_F4, dev).decode(torch.randn(1, 3, 64, 96, generator=g, device=dev))
+
+
+def _wl_bsr_tiled(dev):
+    """The UNet at a tiled sampling batch of 9 and the tiled decode's tile batch: a 192² latent, 2 x 2 tiles of 128²."""
+    g = torch.Generator(device=dev).manual_seed(3)
+    _run_unet(arch.BSR_SR_UNET, [(9, 6, 128, 128)], dev, concat=3)
+    vq = _vq(arch.VQ_F4, dev)
+    q = vq.post_quant(torch.randn(1, 3, 192, 192, generator=g, device=dev))
+    tiles, _ = ops.nchw_to_nhwc(ops.patch_unfold(ops.nhwc_to_nchw(q), (128, 128), (64, 64)))
+    vq._decoder(tiles)
+
+
+def _wl_vq_sr_tile(dev):
+    g = torch.Generator(device=dev).manual_seed(6)
+    _vq(arch.VQ_F4, dev).decode(torch.randn(1, 3, 128, 128, generator=g, device=dev))
+
+
+def _wl_clip_image_tower(dev):
+    """The ViT-L/14 tower from patch rows at B = 1, 64 and 256 images (M = 256 B patch rows, 257 B token rows)."""
+    e = _clip_image_embedder(arch.CLIP_VISION_PROJ, dev)
+    g = torch.Generator(device=dev).manual_seed(0)
+    for B in (1, 64, 256):
+        e.embed_patches(torch.randn(B * 256, e.W["kpad"], generator=g, device=dev).half(), B)
 
 
 def _wl_tiny(dev):
@@ -133,17 +170,48 @@ def _wl_tiny(dev):
     _clip_image(arch.TINY_CLIP_VISION_PROJ, dev, 2)
 
 
+# the norm sweep
 WORKLOADS = {
     "sdv1_unet_b2": lambda dev: _run_unet(arch.SD_V1_UNET, [(2, 4, 64, 64), (2, 4, 64, 96)], dev, ctx=(77, 768)),
     "sdv1_vae_clip_safety": _wl_sdv1_first,
-    "laion": _wl_laion,
+    "laion": lambda dev: _wl_laion(dev, 2, [2]),
     "rdm": _wl_rdm,
     "lsun": lambda dev: _run_unet(arch.LSUN_CHURCHES_UNET, [(2, 4, 32, 32)], dev),
-    "celebahq": _wl_celebahq,
+    "celebahq": lambda dev: _wl_celebahq(dev, 2),
     "cin256_v2": lambda dev: _run_unet(arch.CIN256_V2_UNET, [(2, 3, 64, 64)], dev, ctx=(1, 512)),
-    "cin256_f8": _wl_cin_f8,
-    "inpaint": _wl_inpaint,
+    "cin256_f8": lambda dev: _wl_cin_f8(dev, 2),
+    "inpaint": lambda dev: _wl_inpaint(dev, [1]),
     "bsr": _wl_bsr,
     "semantic": lambda dev: _run_unet(arch.SEMANTIC_SYNTHESIS_UNET, [(1, 6, 64, 64)], dev, concat=3),
     "tiny": _wl_tiny,
+}
+
+# the attention sweep
+ATTENTION_WORKLOADS = {
+    **WORKLOADS,
+    "vq_f4_128x128_latent": _wl_vq_sr_tile,                                    # 16384 tokens at d = 512
+    "vit_l14_b37": lambda dev: _clip_image(arch.CLIP_VISION_PROJ, dev, 37),
+    "rdm_one_token_context": lambda dev: _run_unet(arch.RDM_UNET, [(2, 16, 48, 48)], dev, ctx=(1, 768)),
+}
+
+# test_gemm_plans_gpu.py
+GEMM_WORKLOADS = {
+    "sdv1_unet_b2": lambda dev: _run_unet(arch.SD_V1_UNET, [(2, 4, 64, 64), (2, 4, 64, 96), (2, 4, 96, 64)], dev,
+                                          ctx=(77, 768)),
+    "sdv1_unet_b16": lambda dev: _run_unet(arch.SD_V1_UNET, [(16, 4, 64, 64)], dev, ctx=(77, 768)),
+    "sdv1_vae_clip_safety": _wl_sdv1_first,
+    "lsun": lambda dev: _run_unet(arch.LSUN_CHURCHES_UNET, [(10, 4, 32, 32)], dev),
+    "celebahq": lambda dev: _wl_celebahq(dev, 10),
+    "cin256": lambda dev: _run_unet(arch.CIN256_V2_UNET, [(12, 3, 64, 64), (2, 3, 32, 32)], dev, ctx=(1, 512)),
+    "inpaint": lambda dev: _wl_inpaint(dev, [1, 4]),
+}
+
+# the GEMM plan sweeps of the model test files, one entry per file
+GEMM_MODEL_WORKLOADS = {
+    "rdm": lambda dev: _wl_rdm_unet_kl(dev, 6),
+    "cin256_f8": lambda dev: _wl_cin_f8(dev, 6),
+    "clip_image": _wl_clip_image_tower,
+    "laion": lambda dev: _wl_laion(dev, 6, [2, 6]),
+    "bsr_sr": _wl_bsr_tiled,
+    "semantic": lambda dev: _run_unet(arch.SEMANTIC_SYNTHESIS_UNET, [(8, 6, 64, 64), (1, 6, 128, 128)], dev, concat=3),
 }
