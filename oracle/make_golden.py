@@ -22,25 +22,23 @@ sys.path.insert(0, HERE)
 
 import ldm_oracle as O  # noqa: E402
 import ref_harness as R  # noqa: E402
+from ref_harness import gen, rel  # noqa: E402
 import sdb200  # noqa: E402,F401
 from sdb200 import arch  # noqa: E402
 
 OUT = os.path.join(ROOT, "tests", "golden")
 UNET_SEED, VAE_SEED, CLIP_SEED, SAFETY_SEED = 11, 12, 13, 14
-
-
-def rel(a, b):
-    return float((a.double() - b.double()).norm() / b.double().norm())
+# LatentDiffusion with the v1-inference.yaml parameters; the cond stage is Identity (FrozenCLIPEmbedder needs weights)
+LD_COND = {"target": "torch.nn.Identity"}
+LD_PARAMS = dict(linear_start=0.00085, linear_end=0.0120, num_timesteps_cond=1, log_every_t=200, timesteps=1000,
+                 first_stage_key="jpg", cond_stage_key="txt", image_size=64, channels=4, cond_stage_trainable=False,
+                 conditioning_key="crossattn", monitor="val/loss_simple_ema", scale_factor=0.18215, use_ema=False)
 
 
 def save(name, obj):
     path = os.path.join(OUT, name)
     torch.save(obj, path)
     print(f"  wrote {name} ({os.path.getsize(path) / 1024:.0f} KiB)")
-
-
-def gen(shape, seed, scale=1.0):
-    return torch.randn(shape, generator=torch.Generator().manual_seed(seed)) * scale
 
 
 @torch.no_grad()
@@ -93,7 +91,7 @@ def vae_goldens():
 def pipeline_goldens():
     """Samplers + LatentDiffusion facade of the reference on a tiny model (real apply_model / DiffusionWrapper /
     register_schedule / decode_first_stage / get_first_stage_encoding code paths)."""
-    ld = R.build_latent_diffusion(arch.TINY_UNET, arch.TINY_VAE)
+    ld = R.build_ld(arch.TINY_UNET, arch.TINY_VAE, LD_COND, **LD_PARAMS)
     usd = arch.random_state_dict(arch.unet_param_shapes(arch.TINY_UNET), UNET_SEED)
     vsd = arch.random_state_dict(arch.vae_param_shapes(arch.TINY_VAE), VAE_SEED)
     ld.model.diffusion_model.load_state_dict(usd, strict=True)
@@ -172,7 +170,7 @@ def samplers_ext_goldens():
     of PLMSSampler / DDIMSampler (plms.py:147-150, ddim.py:144-147) with the q_sample draws recorded."""
     import contextlib
     import io
-    ld = R.build_latent_diffusion(arch.TINY_UNET, arch.TINY_VAE)
+    ld = R.build_ld(arch.TINY_UNET, arch.TINY_VAE, LD_COND, **LD_PARAMS)
     usd = arch.random_state_dict(arch.unet_param_shapes(arch.TINY_UNET), UNET_SEED)
     ld.model.diffusion_model.load_state_dict(usd, strict=True)
     plms, ddim = R.build_samplers(ld)
@@ -369,7 +367,7 @@ def nonsquare_goldens():
     # PLMS S=10, CFG 7.5 through the reference's LatentDiffusion facade at a 8x24 latent, then decode_first_stage
     import contextlib
     import io
-    ld = R.build_latent_diffusion(arch.TINY_UNET, arch.TINY_VAE)
+    ld = R.build_ld(arch.TINY_UNET, arch.TINY_VAE, LD_COND, **LD_PARAMS)
     usd = arch.random_state_dict(arch.unet_param_shapes(arch.TINY_UNET), UNET_SEED)
     vsd = arch.random_state_dict(arch.vae_param_shapes(arch.TINY_VAE), VAE_SEED)
     ld.model.diffusion_model.load_state_dict(usd, strict=True)

@@ -3,10 +3,10 @@ for the class-conditional ImageNet LDM (configs/latent-diffusion/cin256-v2.yaml;
 
 Run in the build container:  python oracle/make_golden_cin.py
 ldm/modules/encoders/modules.py imports `clip` and `kornia`, which are not installed and which ClassEmbedder does not use:
-they are stubbed like ref_harness.install() stubs omegaconf / taming. The VQ quantizer is oracle/vq_oracle.py's (as in
-make_golden_vq.py); LatentDiffusion, ClassEmbedder, UNetModel, VQModelInterface and DDIMSampler are the reference's own
-code. Weights come from stable-diffusion_b200/arch.random_state_dict (seeded); every vector is also evaluated with the
-oracle and the error printed.
+ref_harness.install() stubs them, and sets the VQ quantizer to oracle/vq_oracle.py's; LatentDiffusion, ClassEmbedder,
+UNetModel, VQModelInterface and DDIMSampler are the reference's own code. Weights come from
+stable-diffusion_b200/arch.random_state_dict (seeded); every vector is also evaluated with the oracle and the error
+printed.
 """
 from __future__ import annotations
 
@@ -24,53 +24,27 @@ sys.path.insert(0, HERE)
 
 import cin_oracle as CO  # noqa: E402
 import ldm_oracle as O  # noqa: E402
-import make_golden_vq as MV  # noqa: E402
 import ref_harness as R  # noqa: E402
+from ref_harness import gen, rel  # noqa: E402
 import vq_oracle as V  # noqa: E402
 from sdb200 import arch  # noqa: E402
 
 OUT = os.path.join(ROOT, "tests", "golden")
 UNET_SEED, VQ_SEED, COND_SEED = 11, 12, 13
 LINEAR_START, LINEAR_END = 0.0015, 0.0195
-
-
-def rel(a, b):
-    return float((a.double() - b.double()).norm() / b.double().norm())
-
-
-def gen(shape, seed, scale=1.0):
-    return scale * torch.randn(shape, generator=torch.Generator().manual_seed(seed))
-
-
-def install():
-    MV.install()
-    R._stub("clip")
-    R._stub("kornia")
-
-
-def build_cin_ld(unet_cfg, vq_cfg, cond_cfg):
-    """The reference's LatentDiffusion with the cin256-v2.yaml parameters."""
-    install()
-    from ldm.models.diffusion.ddpm import LatentDiffusion
-    with contextlib.redirect_stdout(io.StringIO()):
-        m = LatentDiffusion(
-            first_stage_config={"target": "ldm.models.autoencoder.VQModelInterface",
-                                "params": {"embed_dim": vq_cfg["embed_dim"], "n_embed": vq_cfg["n_embed"],
-                                           "ddconfig": vq_cfg["ddconfig"], "lossconfig": {"target": "torch.nn.Identity"}}},
-            cond_stage_config={"target": "ldm.modules.encoders.modules.ClassEmbedder", "params": dict(cond_cfg)},
-            unet_config={"target": "ldm.modules.diffusionmodules.openaimodel.UNetModel", "params": dict(unet_cfg)},
-            linear_start=LINEAR_START, linear_end=LINEAR_END, num_timesteps_cond=1, log_every_t=200, timesteps=1000,
-            first_stage_key="image", cond_stage_key="class_label", image_size=unet_cfg["image_size"],
-            channels=unet_cfg["in_channels"], cond_stage_trainable=True, conditioning_key="crossattn",
-            monitor="val/loss", use_ema=False)
-    return m.eval()
+# LatentDiffusion with the cin256-v2.yaml parameters; the cond stage is ClassEmbedder
+COND_TARGET = "ldm.modules.encoders.modules.ClassEmbedder"
+LD_PARAMS = dict(linear_start=LINEAR_START, linear_end=LINEAR_END, num_timesteps_cond=1, log_every_t=200,
+                 timesteps=1000, first_stage_key="image", cond_stage_key="class_label", cond_stage_trainable=True,
+                 conditioning_key="crossattn", monitor="val/loss", use_ema=False)
 
 
 @torch.no_grad()
 def main():
     out = {"unet_seed": UNET_SEED, "vq_seed": VQ_SEED, "cond_seed": COND_SEED, "linear_end": LINEAR_END}
     # the reference's key / shape list of the whole cin256-v2 model, so the CPU tests need no reference
-    ld = build_cin_ld(arch.CIN256_V2_UNET, arch.VQ_F4, arch.CIN256_V2_COND)
+    ld = R.build_ld(arch.CIN256_V2_UNET, arch.VQ_F4, {"target": COND_TARGET, "params": arch.CIN256_V2_COND},
+                    **LD_PARAMS)
     out["cin256_keys"] = [(k, tuple(v.shape)) for k, v in ld.state_dict().items()]
     del ld
 
@@ -80,7 +54,7 @@ def main():
         ("cin256", arch.CIN256_V2_UNET, arch.CIN256_V2_COND,
          [((2, 3, 32, 32), [981, 1]), ((2, 3, 64, 64), [700, 11]), ((1, 3, 16, 48), [501])]),
     ):
-        ld = build_cin_ld(cfg, arch.TINY_VQ, ccfg)
+        ld = R.build_ld(cfg, arch.TINY_VQ, {"target": COND_TARGET, "params": ccfg}, **LD_PARAMS)
         sd = arch.random_state_dict(arch.unet_param_shapes(cfg), UNET_SEED)
         csd = arch.random_state_dict(arch.class_embedder_param_shapes(ccfg), COND_SEED)
         ld.model.diffusion_model.load_state_dict(sd, strict=True)
@@ -97,7 +71,8 @@ def main():
         del ld
 
     # the notebook's sampling cell on the tiny model: DDIM-10, eta 0, scale 3.0, uc from label 1000, then decode
-    ld = build_cin_ld(arch.TINY_CIN_UNET, arch.TINY_VQ, arch.TINY_CIN_COND)
+    ld = R.build_ld(arch.TINY_CIN_UNET, arch.TINY_VQ, {"target": COND_TARGET, "params": arch.TINY_CIN_COND},
+                    **LD_PARAMS)
     usd = arch.random_state_dict(arch.unet_param_shapes(arch.TINY_CIN_UNET), UNET_SEED)
     vsd = arch.random_state_dict(arch.vq_param_shapes(arch.TINY_VQ), VQ_SEED)
     csd = arch.random_state_dict(arch.class_embedder_param_shapes(arch.TINY_CIN_COND), COND_SEED)

@@ -3,7 +3,7 @@ fp32 for the class-conditional ImageNet LDM-VQ-8 (models/ldm/cin256/config.yaml;
 cin-ldm-vq-f8.yaml has the same model node).
 
 Run in the build container:  python oracle/make_golden_cin_f8.py
-clip / kornia are stubbed as in make_golden_cin.py and the VQ quantizer is oracle/vq_oracle.py's (make_golden_vq.py);
+clip / kornia are stubbed and the VQ quantizer is oracle/vq_oracle.py's (ref_harness.install());
 LatentDiffusion, LitEma, ClassEmbedder, UNetModel, VQModelInterface (with its level AttnBlocks) and DDIMSampler are the
 reference's own code. Weights come from stable-diffusion_b200/arch.random_state_dict (seeded; the tiny model's EMA copy
 from its own seed); inputs are regenerated from the seeds stored next to the outputs. Decoded images are stored at every
@@ -27,16 +27,20 @@ sys.path.insert(0, HERE)
 
 import cin_f8_oracle as F8  # noqa: E402
 import cin_oracle as CO  # noqa: E402
-import make_golden_cin as CG  # noqa: E402
-import make_golden_vq as MV  # noqa: E402
 import ref_harness as R  # noqa: E402
+from ref_harness import gen, rel  # noqa: E402
 import uncond_oracle as U  # noqa: E402
-import vq_oracle as V  # noqa: E402
 from sdb200 import arch  # noqa: E402
 
 OUT = os.path.join(ROOT, "tests", "golden")
 UNET_SEED, VQ_SEED, COND_SEED, EMA_SEED = 11, 12, 13, 31
 LINEAR_START, LINEAR_END = 0.0015, 0.0195
+# LatentDiffusion with the cin256/config.yaml parameters (use_ema left at its default, True); the cond stage is
+# ClassEmbedder
+COND_TARGET = "ldm.modules.encoders.modules.ClassEmbedder"
+LD_PARAMS = dict(linear_start=LINEAR_START, linear_end=LINEAR_END, num_timesteps_cond=1, log_every_t=200,
+                 timesteps=1000, first_stage_key="image", cond_stage_key="class_label", cond_stage_trainable=True,
+                 conditioning_key="crossattn", monitor="val/loss_simple_ema")
 YAMLS = ("models/ldm/cin256/config.yaml", "configs/latent-diffusion/cin-ldm-vq-f8.yaml")
 # decoded images are stored at every IMAGE_STRIDE-th pixel in both directions (1/16 of the pixels, spread over the whole
 # image), which keeps the file small; the tests decode in full and compare the same pixels
@@ -47,28 +51,6 @@ def sub(x):
     return x[..., ::IMAGE_STRIDE, ::IMAGE_STRIDE].contiguous()
 
 
-def gen(shape, seed):
-    return torch.randn(shape, generator=torch.Generator().manual_seed(seed))
-
-
-def build_ld(unet_cfg, vq_cfg, cond_cfg):
-    """The reference's LatentDiffusion with the cin256/config.yaml parameters (use_ema left at its default, True)."""
-    CG.install()
-    from ldm.models.diffusion.ddpm import LatentDiffusion
-    with contextlib.redirect_stdout(io.StringIO()):
-        m = LatentDiffusion(
-            first_stage_config={"target": "ldm.models.autoencoder.VQModelInterface",
-                                "params": {"embed_dim": vq_cfg["embed_dim"], "n_embed": vq_cfg["n_embed"],
-                                           "ddconfig": vq_cfg["ddconfig"], "lossconfig": {"target": "torch.nn.Identity"}}},
-            cond_stage_config={"target": "ldm.modules.encoders.modules.ClassEmbedder", "params": dict(cond_cfg)},
-            unet_config={"target": "ldm.modules.diffusionmodules.openaimodel.UNetModel", "params": dict(unet_cfg)},
-            linear_start=LINEAR_START, linear_end=LINEAR_END, num_timesteps_cond=1, log_every_t=200, timesteps=1000,
-            first_stage_key="image", cond_stage_key="class_label", image_size=unet_cfg["image_size"],
-            channels=unet_cfg["in_channels"], cond_stage_trainable=True, conditioning_key="crossattn",
-            monitor="val/loss_simple_ema")
-    return m.eval()
-
-
 @torch.no_grad()
 def main():
     out = {"unet_seed": UNET_SEED, "vq_seed": VQ_SEED, "cond_seed": COND_SEED, "ema_seed": EMA_SEED,
@@ -77,7 +59,8 @@ def main():
     for rel_path in YAMLS:
         with open(os.path.join(R.REF, rel_path)) as f:
             out["yaml_nodes"][rel_path] = yaml.safe_load(f)["model"]
-    ld = build_ld(arch.CIN256_F8_UNET, arch.VQ_F8, arch.CIN256_F8_COND)
+    ld = R.build_ld(arch.CIN256_F8_UNET, arch.VQ_F8, {"target": COND_TARGET, "params": arch.CIN256_F8_COND},
+                    **LD_PARAMS)
     out["cin256_keys"] = [(k, tuple(v.shape)) for k, v in ld.state_dict().items()]
     out["alphas_cumprod"] = ld.alphas_cumprod.clone()
     del ld
@@ -89,7 +72,7 @@ def main():
         ("cin256", arch.CIN256_F8_UNET, arch.CIN256_F8_COND,
          [((2, 4, 32, 32), [981, 1]), ((2, 4, 64, 64), [700, 11]), ((1, 4, 16, 48), [501])]),
     ):
-        ld = build_ld(cfg, arch.TINY_VQ_F8, ccfg)
+        ld = R.build_ld(cfg, arch.TINY_VQ_F8, {"target": COND_TARGET, "params": ccfg}, **LD_PARAMS)
         sd = arch.random_state_dict(arch.unet_param_shapes(cfg), UNET_SEED)
         csd = arch.random_state_dict(arch.class_embedder_param_shapes(ccfg), COND_SEED)
         ld.model.diffusion_model.load_state_dict(sd, strict=True)
@@ -101,7 +84,7 @@ def main():
             c = ld.get_learned_conditioning({"class_label": labels})
             eps = ld.apply_model(x, t, c)
             mine = F8.unet_forward(sd, x, t, CO.class_embed(csd, labels))
-            print(f"unet {tag} {xs} t={ts}: eps std {float(eps.std()):.3f}  oracle rel-L2 {CG.rel(mine, eps):.2e}")
+            print(f"unet {tag} {xs} t={ts}: eps std {float(eps.std()):.3f}  oracle rel-L2 {rel(mine, eps):.2e}")
             out["unet"].append(dict(cfg=tag, x_seed=900 + i, shape=xs, t=t, labels=labels, c=c.clone(), eps=eps))
         del ld
 
@@ -112,22 +95,23 @@ def main():
         ("vq_f8", arch.VQ_F8, [(2, 4, 32, 32), (1, 4, 16, 48)], [(1, 3, 256, 256)]),
     ):
         sd = arch.random_state_dict(arch.vq_param_shapes(cfg), VQ_SEED)
-        m = MV.build_vq(cfg)
+        m = R.build_vq(cfg)
         m.load_state_dict(sd, strict=True)
         for j, ds in enumerate(decs):
             h = gen(ds, 920 + j)
             x = m.decode(h)
-            print(f"decode {tag} {ds} -> {tuple(x.shape)}: oracle rel {CG.rel(F8.vq_decode(sd, h), x):.2e}")
+            print(f"decode {tag} {ds} -> {tuple(x.shape)}: oracle rel {rel(F8.vq_decode(sd, h), x):.2e}")
             out["decode"].append(dict(cfg=tag, seed=920 + j, shape=ds, x_shape=tuple(x.shape), x=sub(x)))
         for j, es in enumerate(encs):
             img = gen(es, 930 + j).clamp(-1, 1)
             h = m.encode(img)
-            print(f"encode {tag} {es} -> {tuple(h.shape)}: oracle rel {CG.rel(F8.vq_encode(sd, img), h):.2e}")
+            print(f"encode {tag} {es} -> {tuple(h.shape)}: oracle rel {rel(F8.vq_encode(sd, img), h):.2e}")
             out["encode"].append(dict(cfg=tag, seed=930 + j, shape=es, h=h))
         del m
 
     # the tiny model sampled unguided inside ema_scope (EMA weights from their own seed): DDIM-10 at eta 0 and 1, decode
-    ld = build_ld(arch.TINY_CIN_F8_UNET, arch.TINY_VQ_F8, arch.TINY_CIN_F8_COND)
+    ld = R.build_ld(arch.TINY_CIN_F8_UNET, arch.TINY_VQ_F8, {"target": COND_TARGET, "params": arch.TINY_CIN_F8_COND},
+                    **LD_PARAMS)
     usd = arch.random_state_dict(arch.unet_param_shapes(arch.TINY_CIN_F8_UNET), UNET_SEED)
     esd = arch.random_state_dict(arch.unet_param_shapes(arch.TINY_CIN_F8_UNET), EMA_SEED)
     vsd = arch.random_state_dict(arch.vq_param_shapes(arch.TINY_VQ_F8), VQ_SEED)
@@ -135,9 +119,7 @@ def main():
     ld.model.diffusion_model.load_state_dict(usd, strict=True)
     ld.first_stage_model.load_state_dict(vsd, strict=True)
     ld.cond_stage_model.load_state_dict(csd, strict=True)
-    bufs = dict(ld.model_ema.named_buffers())
-    for k, v in esd.items():
-        bufs[("diffusion_model." + k).replace(".", "")].copy_(v)
+    R.load_ema(ld, esd)
     out["ema_keys"] = sorted(k for k in ld.state_dict() if k.startswith("model_ema."))
     _, ddim = R.build_samplers(ld)
     import ldm.models.diffusion.ddim as ddim_mod
@@ -161,7 +143,7 @@ def main():
         mine = U.ddim_sample_uncond(fn, x_T, ld.alphas_cumprod, 10, eta, torch.stack(draws) if eta else
                                     torch.zeros(10, B, *shape))
         print(f"ddim S=10 eta={eta} (EMA weights): sample std {float(s.std()):.3f}, {len(draws)} draws; oracle rel "
-              f"{CG.rel(mine, s):.2e}; decode oracle rel {CG.rel(F8.decode_first_stage(vsd, s), x_dec):.2e}")
+              f"{rel(mine, s):.2e}; decode oracle rel {rel(F8.decode_first_stage(vsd, s), x_dec):.2e}")
         out["ddim"][f"eta{int(eta)}"] = dict(sample=s, x_dec=sub(x_dec), n_noise=len(draws))
     path = os.path.join(OUT, "cin_f8.pt")
     torch.save(out, path)

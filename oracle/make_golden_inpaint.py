@@ -2,7 +2,7 @@
 fp32 for the LDM inpainting model (models/ldm/inpainting_big/config.yaml, scripts/inpaint.py).
 
 Run in the build container:  python oracle/make_golden_inpaint.py
-As in make_golden_vq.py, taming's quantizer is oracle/vq_oracle.py's restatement and the training loss is
+taming's quantizer is oracle/vq_oracle.py's restatement (set by ref_harness.install()) and the training loss is
 torch.nn.Identity (the config's DummyLoss only exists through taming). `make_batch` is the reference script's own
 function, called on PNG files written here; its `main` import (the training entry point) is stubbed with ldm.util's
 instantiate_from_config. The composite is the script's inline code, restated in oracle/inpaint_oracle.py.
@@ -27,50 +27,28 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, HERE)
 
 import inpaint_oracle as P  # noqa: E402
-import make_golden_vq as GV  # noqa: E402
 import ref_harness as R  # noqa: E402
+from ref_harness import gen  # noqa: E402
 import sdb200  # noqa: E402,F401
 from sdb200 import arch  # noqa: E402
 
 OUT = os.path.join(ROOT, "tests", "golden")
 UNET_SEED, VQ_SEED = 11, 12
 LINEAR_START, LINEAR_END = 0.0015, 0.0205
-
-
-def rel(a, b):
-    return float((a.double() - b.double()).norm() / b.double().norm())
-
-
-def gen(shape, seed, scale=1.0):
-    return scale * torch.randn(shape, generator=torch.Generator().manual_seed(seed))
+# LatentDiffusion with the inpainting_big config's parameters; the first stage is also the cond stage
+LD_PARAMS = dict(linear_start=LINEAR_START, linear_end=LINEAR_END, log_every_t=100, timesteps=1000, loss_type="l1",
+                 first_stage_key="image", cond_stage_key="masked_image", channels=3, concat_mode=True,
+                 monitor="val/loss")
 
 
 def ref_inpaint_module():
-    GV.install()
+    R.install()
     from ldm.util import instantiate_from_config
     sys.modules.setdefault("main", types.SimpleNamespace(instantiate_from_config=instantiate_from_config))
     spec = importlib.util.spec_from_file_location("ref_inpaint_script", os.path.join(R.REF, "scripts", "inpaint.py"))
     mod = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(mod)
     return mod
-
-
-def build_inpaint_ld(unet_cfg, vq_cfg, use_ema=True):
-    """The reference's LatentDiffusion with the inpainting_big config's parameters."""
-    GV.install()
-    from ldm.models.diffusion.ddpm import LatentDiffusion
-    with contextlib.redirect_stdout(io.StringIO()):
-        m = LatentDiffusion(
-            first_stage_config={"target": "ldm.models.autoencoder.VQModelInterface",
-                                "params": {"embed_dim": vq_cfg["embed_dim"], "n_embed": vq_cfg["n_embed"],
-                                           "monitor": "val/rec_loss", "ddconfig": vq_cfg["ddconfig"],
-                                           "lossconfig": {"target": "torch.nn.Identity"}}},
-            cond_stage_config="__is_first_stage__",
-            unet_config={"target": "ldm.modules.diffusionmodules.openaimodel.UNetModel", "params": dict(unet_cfg)},
-            linear_start=LINEAR_START, linear_end=LINEAR_END, log_every_t=100, timesteps=1000, loss_type="l1",
-            first_stage_key="image", cond_stage_key="masked_image", image_size=unet_cfg["image_size"], channels=3,
-            concat_mode=True, monitor="val/loss", use_ema=use_ema)
-    return m.eval()
 
 
 def synthetic_pair(h, w, seed, threshold=False):
@@ -108,7 +86,7 @@ def main():
     mod = ref_inpaint_module()
     out = {"unet_seed": UNET_SEED, "vq_seed": VQ_SEED, "linear_start": LINEAR_START, "linear_end": LINEAR_END}
     # the reference model's state-dict keys: cond_stage_model.* repeats first_stage_model.*
-    ld = build_inpaint_ld(arch.INPAINTING_BIG_UNET, arch.VQ_F4_NOATTN)
+    ld = R.build_ld(arch.INPAINTING_BIG_UNET, arch.VQ_F4_NOATTN, "__is_first_stage__", **LD_PARAMS)
     out["ld_keys"] = [(k, tuple(v.shape)) for k, v in ld.state_dict().items()]
     del ld
 
@@ -156,7 +134,7 @@ def main():
     out["vq"] = []
     for tag, cfg, size in (("tiny", arch.TINY_VQ_NOATTN, (2, 3, 32, 48)), ("big", arch.VQ_F4_NOATTN, (1, 3, 32, 48))):
         sd = arch.random_state_dict(arch.vq_param_shapes(cfg), VQ_SEED)
-        m = GV.build_vq(cfg)
+        m = R.build_vq(cfg)
         m.load_state_dict(sd, strict=True)
         img = gen(size, 930).clamp(-1, 1)
         h = m.encode(img)
@@ -165,7 +143,7 @@ def main():
         out["vq"].append(dict(cfg=tag, x=img, h=h, dec=x))
 
     # the script end to end on the tiny model: DDIM-10 from a recorded x_T, decode, composite
-    ld = build_inpaint_ld(arch.TINY_INPAINT_UNET, arch.TINY_VQ_NOATTN, use_ema=False)
+    ld = R.build_ld(arch.TINY_INPAINT_UNET, arch.TINY_VQ_NOATTN, "__is_first_stage__", use_ema=False, **LD_PARAMS)
     ld.model.diffusion_model.load_state_dict(arch.random_state_dict(arch.unet_param_shapes(arch.TINY_INPAINT_UNET),
                                                                     UNET_SEED), strict=True)
     ld.first_stage_model.load_state_dict(arch.random_state_dict(arch.vq_param_shapes(arch.TINY_VQ_NOATTN), VQ_SEED),

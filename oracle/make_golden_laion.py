@@ -4,7 +4,7 @@ fp32 for the LAION-400M text-to-image LDM (configs/latent-diffusion/txt2img-1p4B
 
 Run in the build container:  python oracle/make_golden_laion.py
 ldm/modules/encoders/modules.py imports `clip` and `kornia`, which are not installed and which BERTEmbedder does not use:
-they are stubbed as in make_golden_cin.py. BERTEmbedder is always built with use_tokenizer=False and fed token ids
+ref_harness.install() stubs them. BERTEmbedder is always built with use_tokenizer=False and fed token ids
 (use_tokenizer=True would fetch the bert-base-uncased tokenizer). LatentDiffusion, BERTEmbedder, UNetModel,
 AutoencoderKL and PLMSSampler are the reference's own code. Weights come from stable-diffusion_b200/arch.random_state_dict
 (seeded); every vector is also evaluated with the oracle and the error printed.
@@ -30,20 +30,24 @@ sys.path.insert(0, HERE)
 
 import bert_oracle as BO  # noqa: E402
 import ldm_oracle as O  # noqa: E402
-import make_golden_cin as MC  # noqa: E402
 import ref_harness as R  # noqa: E402
+from ref_harness import gen, rel  # noqa: E402
 from sdb200 import arch  # noqa: E402
 
 OUT = os.path.join(ROOT, "tests", "golden")
 UNET_SEED, VAE_SEED, BERT_SEED = 11, 12, 13
+# LatentDiffusion with the txt2img-1p4B-eval.yaml parameters
+LD_PARAMS = dict(linear_start=0.00085, linear_end=0.012, num_timesteps_cond=1, log_every_t=200, timesteps=1000,
+                 first_stage_key="image", cond_stage_key="caption", image_size=32, channels=4,
+                 cond_stage_trainable=True, conditioning_key="crossattn", monitor="val/loss_simple_ema",
+                 scale_factor=0.18215, use_ema=False)
 
 
-def rel(a, b):
-    return float((a.double() - b.double()).norm() / b.double().norm())
-
-
-def gen(shape, seed, scale=1.0):
-    return scale * torch.randn(shape, generator=torch.Generator().manual_seed(seed))
+def bert_cond(cfg):
+    """The cond stage node: BERTEmbedder without tokenizer."""
+    return {"target": "ldm.modules.encoders.modules.BERTEmbedder",
+            "params": {"n_embed": cfg["n_embed"], "n_layer": cfg["n_layer"], "vocab_size": cfg["vocab_size"],
+                       "use_tokenizer": False}}
 
 
 def prompt_ids(vocab_size, seed, n_tok=20, B=2):
@@ -59,35 +63,16 @@ def prompt_ids(vocab_size, seed, n_tok=20, B=2):
     return ids
 
 
-def build_laion_ld(unet_cfg, vae_cfg, bert_cfg):
-    """The reference's LatentDiffusion with the txt2img-1p4B-eval.yaml parameters (BERTEmbedder without tokenizer)."""
-    MC.install()
-    from ldm.models.diffusion.ddpm import LatentDiffusion
-    with contextlib.redirect_stdout(io.StringIO()):
-        m = LatentDiffusion(
-            first_stage_config={"target": "ldm.models.autoencoder.AutoencoderKL",
-                                "params": {"embed_dim": vae_cfg["embed_dim"], "monitor": "val/rec_loss",
-                                           "ddconfig": vae_cfg["ddconfig"], "lossconfig": {"target": "torch.nn.Identity"}}},
-            cond_stage_config={"target": "ldm.modules.encoders.modules.BERTEmbedder",
-                               "params": {"n_embed": bert_cfg["n_embed"], "n_layer": bert_cfg["n_layer"],
-                                          "vocab_size": bert_cfg["vocab_size"], "use_tokenizer": False}},
-            unet_config={"target": "ldm.modules.diffusionmodules.openaimodel.UNetModel", "params": dict(unet_cfg)},
-            linear_start=0.00085, linear_end=0.012, num_timesteps_cond=1, log_every_t=200, timesteps=1000,
-            first_stage_key="image", cond_stage_key="caption", image_size=32, channels=4, cond_stage_trainable=True,
-            conditioning_key="crossattn", monitor="val/loss_simple_ema", scale_factor=0.18215, use_ema=False)
-    return m.eval()
-
-
 @torch.no_grad()
 def main():
     out = {"unet_seed": UNET_SEED, "vae_seed": VAE_SEED, "bert_seed": BERT_SEED}
-    ld = build_laion_ld(arch.LAION_UNET, arch.SD_V1_VAE, arch.LAION_BERT)
+    ld = R.build_ld(arch.LAION_UNET, arch.SD_V1_VAE, bert_cond(arch.LAION_BERT), **LD_PARAMS)
     out["laion_keys"] = [(k, tuple(v.shape)) for k, v in ld.state_dict().items()]
     del ld
 
     out["bert"] = []
     for tag, cfg, seed in (("tiny", arch.TINY_BERT, 500), ("full", arch.LAION_BERT, 501)):
-        MC.install()
+        R.install()
         from ldm.modules.encoders.modules import BERTEmbedder
         ref = BERTEmbedder(n_embed=cfg["n_embed"], n_layer=cfg["n_layer"], vocab_size=cfg["vocab_size"],
                            use_tokenizer=False).eval()
@@ -119,7 +104,7 @@ def main():
         del unet, sd
 
     # scripts/txt2img.py --laion400m on the tiny model: uc from the empty prompt, guided PLMS-10, decode
-    ld = build_laion_ld(arch.TINY_LAION_UNET, arch.TINY_VAE, arch.TINY_BERT)
+    ld = R.build_ld(arch.TINY_LAION_UNET, arch.TINY_VAE, bert_cond(arch.TINY_BERT), **LD_PARAMS)
     usd = arch.random_state_dict(arch.unet_param_shapes(arch.TINY_LAION_UNET), UNET_SEED)
     vsd = arch.random_state_dict(arch.vae_param_shapes(arch.TINY_VAE), VAE_SEED)
     bsd = arch.random_state_dict(arch.bert_param_shapes(arch.TINY_BERT), BERT_SEED)

@@ -20,6 +20,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, HERE)
 
 import ref_harness as R  # noqa: E402
+from ref_harness import gen, rel  # noqa: E402
 import uncond_oracle as U  # noqa: E402
 import ldm_oracle as O  # noqa: E402
 import sdb200  # noqa: E402,F401
@@ -29,33 +30,12 @@ OUT = os.path.join(ROOT, "tests", "golden")
 UNET_SEED, VAE_SEED, EMA_SEED = 11, 12, 31
 CFGS = {"tiny_attn": arch.TINY_ATTN_UNET, "tiny_attn_plain": arch.TINY_ATTN_PLAIN_UNET, "lsun": arch.LSUN_CHURCHES_UNET}
 SCALE_FACTOR = 0.37
-
-
-def rel(a, b):
-    return float((a.double() - b.double()).norm() / b.double().norm())
-
-
-def gen(shape, seed):
-    return torch.randn(shape, generator=torch.Generator().manual_seed(seed))
-
-
-def build_uncond_ld(unet_cfg, vae_cfg, timesteps=1000, use_ema=False):
-    """The reference's LatentDiffusion with the LSUN-Churches config parameters (unconditional, scale_by_std)."""
-    R.install()
-    from ldm.models.diffusion.ddpm import LatentDiffusion
-    with contextlib.redirect_stdout(io.StringIO()):
-        m = LatentDiffusion(
-            first_stage_config={"target": "ldm.models.autoencoder.AutoencoderKL",
-                                "params": {"embed_dim": vae_cfg["embed_dim"], "monitor": "val/rec_loss",
-                                           "ddconfig": vae_cfg["ddconfig"], "lossconfig": {"target": "torch.nn.Identity"}}},
-            cond_stage_config="__is_unconditional__",
-            unet_config={"target": "ldm.modules.diffusionmodules.openaimodel.UNetModel", "params": dict(unet_cfg)},
-            linear_start=0.0015, linear_end=0.0155, num_timesteps_cond=1, log_every_t=200, timesteps=timesteps,
-            loss_type="l1", first_stage_key="image", cond_stage_key="image", image_size=unet_cfg["image_size"],
-            channels=4, cond_stage_trainable=False, concat_mode=False, scale_by_std=True, monitor="val/loss_simple_ema",
-            use_ema=use_ema)
-    m.scale_factor.fill_(SCALE_FACTOR)
-    return m.eval()
+# LatentDiffusion with the LSUN-Churches config parameters (unconditional, scale_by_std); each model built here then
+# gets scale_factor = SCALE_FACTOR in place of the one scale_by_std would measure on the first training batch
+LD_PARAMS = dict(linear_start=0.0015, linear_end=0.0155, num_timesteps_cond=1, log_every_t=200, timesteps=1000,
+                 loss_type="l1", first_stage_key="image", cond_stage_key="image", channels=4,
+                 cond_stage_trainable=False, concat_mode=False, scale_by_std=True, monitor="val/loss_simple_ema",
+                 use_ema=False)
 
 
 class Recorder:
@@ -102,7 +82,8 @@ def main():
     B, shape = 2, [4, 16, 16]
 
     # DDIM S=10, eta=1, unconditional (sample_diffusion.py convsample_ddim), then decode_first_stage
-    ld = build_uncond_ld(arch.TINY_ATTN_UNET, arch.TINY_VAE)
+    ld = R.build_ld(arch.TINY_ATTN_UNET, arch.TINY_VAE, "__is_unconditional__", **LD_PARAMS)
+    ld.scale_factor.fill_(SCALE_FACTOR)
     ld.model.diffusion_model.load_state_dict(usd, strict=True)
     ld.first_stage_model.load_state_dict(vsd, strict=True)
     _, ddim = R.build_samplers(ld)
@@ -122,7 +103,8 @@ def main():
         out["sched_" + k] = getattr(ld, k).clone()
 
     # ancestral DDPM (progressive_denoising, sample_diffusion.py --vanilla) on a 20-step schedule
-    ld20 = build_uncond_ld(arch.TINY_ATTN_UNET, arch.TINY_VAE, timesteps=20)
+    ld20 = R.build_ld(arch.TINY_ATTN_UNET, arch.TINY_VAE, "__is_unconditional__", **dict(LD_PARAMS, timesteps=20))
+    ld20.scale_factor.fill_(SCALE_FACTOR)
     ld20.model.diffusion_model.load_state_dict(usd, strict=True)
     ld20.first_stage_model.load_state_dict(vsd, strict=True)
     x_T = gen((B, *shape), 830)
@@ -137,12 +119,11 @@ def main():
                             x_dec=ld20.decode_first_stage(s_anc))
 
     # EMA: model_ema buffers (LitEma names) hold other weights; ema_scope() must switch to them
-    lde = build_uncond_ld(arch.TINY_ATTN_UNET, arch.TINY_VAE, use_ema=True)
+    lde = R.build_ld(arch.TINY_ATTN_UNET, arch.TINY_VAE, "__is_unconditional__", **dict(LD_PARAMS, use_ema=True))
+    lde.scale_factor.fill_(SCALE_FACTOR)
     lde.model.diffusion_model.load_state_dict(usd, strict=True)
     esd = arch.random_state_dict(arch.unet_param_shapes(arch.TINY_ATTN_UNET), EMA_SEED)
-    bufs = dict(lde.model_ema.named_buffers())
-    for k, v in esd.items():
-        bufs[("diffusion_model." + k).replace(".", "")].copy_(v)
+    R.load_ema(lde, esd)
     x = gen((B, *shape), 840)
     t = torch.tensor([700, 3])
     raw = lde.apply_model(x, t, None)

@@ -2,7 +2,7 @@
 fp32 for the retrieval-augmented diffusion model (configs/retrieval-augmented-diffusion/768x768.yaml, scripts/knn2img.py).
 
 Run in the build container:  python oracle/make_golden_rdm.py
-clip / kornia are stubbed as in make_golden_laion.py (the model's cond stage is torch.nn.Identity; the CLIP text
+clip / kornia are stubbed by ref_harness.install() (the model's cond stage is torch.nn.Identity; the CLIP text
 embedder is checked against transformers on the GPU instead). LatentDiffusion, LitEma, UNetModel, AutoencoderKL (KL-f16,
 with its level AttnBlocks), DDIMSampler and PLMSSampler are the reference's own code. Weights come from
 stable-diffusion_b200/arch.random_state_dict (seeded; the tiny model's EMA copy from its own seed); inputs are regenerated
@@ -27,9 +27,9 @@ ROOT = os.path.dirname(HERE)
 sys.path.insert(0, ROOT)
 sys.path.insert(0, HERE)
 
-import make_golden_cin as MC  # noqa: E402
 import rdm_oracle as RO  # noqa: E402
 import ref_harness as R  # noqa: E402
+from ref_harness import gen, rel  # noqa: E402
 from sdb200 import arch  # noqa: E402
 
 OUT = os.path.join(ROOT, "tests", "golden")
@@ -39,38 +39,21 @@ SCALE_FACTOR = 0.22765929
 IMAGE_STRIDE = 8
 EPS_STRIDE = 2
 GUIDANCE = 5.0
+# LatentDiffusion with the 768x768.yaml parameters (use_ema left at its default, True); the cond stage is Identity
+LD_PARAMS = dict(linear_start=0.0015, linear_end=0.015, num_timesteps_cond=1, log_every_t=200, timesteps=1000,
+                 first_stage_key="jpg", cond_stage_key="nix", cond_stage_trainable=False, conditioning_key="crossattn",
+                 monitor="val/loss_simple_ema", scale_by_std=False, scale_factor=SCALE_FACTOR)
+LD_COND = {"target": "torch.nn.Identity"}
 
 
 def sub(x):
     return x[..., ::IMAGE_STRIDE, ::IMAGE_STRIDE].contiguous()
 
 
-def gen(shape, seed):
-    return torch.randn(shape, generator=torch.Generator().manual_seed(seed))
-
-
 def unit_rows(shape, seed):
     """Conditioning tokens as the embedder and the searcher give them: rows of unit L2 norm."""
     x = gen(shape, seed)
     return x / torch.linalg.norm(x, dim=-1, keepdim=True)
-
-
-def build_ld(unet_cfg, vae_cfg, use_ema=True):
-    """The reference's LatentDiffusion with the 768x768.yaml parameters (use_ema left at its default, True)."""
-    MC.install()
-    from ldm.models.diffusion.ddpm import LatentDiffusion
-    with contextlib.redirect_stdout(io.StringIO()):
-        m = LatentDiffusion(
-            first_stage_config={"target": "ldm.models.autoencoder.AutoencoderKL",
-                                "params": {"monitor": "val/rec_loss", "embed_dim": vae_cfg["embed_dim"],
-                                           "ddconfig": vae_cfg["ddconfig"], "lossconfig": {"target": "torch.nn.Identity"}}},
-            cond_stage_config={"target": "torch.nn.Identity"},
-            unet_config={"target": "ldm.modules.diffusionmodules.openaimodel.UNetModel", "params": dict(unet_cfg)},
-            linear_start=0.0015, linear_end=0.015, num_timesteps_cond=1, log_every_t=200, timesteps=1000,
-            first_stage_key="jpg", cond_stage_key="nix", image_size=unet_cfg["image_size"],
-            channels=unet_cfg["in_channels"], cond_stage_trainable=False, conditioning_key="crossattn",
-            monitor="val/loss_simple_ema", scale_by_std=False, scale_factor=SCALE_FACTOR, use_ema=use_ema)
-    return m.eval()
 
 
 @torch.no_grad()
@@ -80,7 +63,7 @@ def main():
            "scale_factor": SCALE_FACTOR, "guidance": GUIDANCE}
     with open(os.path.join(R.REF, YAML)) as f:
         out["yaml_node"] = yaml.safe_load(f)["model"]
-    ld = build_ld(arch.RDM_UNET, arch.KL_F16)
+    ld = R.build_ld(arch.RDM_UNET, arch.KL_F16, LD_COND, **LD_PARAMS)
     out["rdm_keys"] = [(k, tuple(v.shape)) for k, v in ld.state_dict().items()]
     out["alphas_cumprod"] = ld.alphas_cumprod.clone()
     del ld
@@ -103,7 +86,7 @@ def main():
             eps = unet(x, t, context=c)
             mine = RO.unet_forward(sd, x, t, c)
             print(f"unet {tag} {xs} ctx {n_ctx} t={ts}: eps std {float(eps.std()):.3f}  oracle rel-L2 "
-                  f"{MC.rel(mine, eps):.2e}")
+                  f"{rel(mine, eps):.2e}")
             out["unet"].append(dict(cfg=tag, seed=seed, shape=xs, n_ctx=n_ctx, t=t,
                                     eps=eps[..., ::EPS_STRIDE, ::EPS_STRIDE].contiguous()))
         del unet, sd
@@ -120,26 +103,24 @@ def main():
         for j, ds in enumerate(decs):
             z = gen(ds, 920 + j)
             x = m.decode(z)
-            print(f"decode {tag} {ds} -> {tuple(x.shape)}: oracle rel {MC.rel(RO.kl_decode(sd, z), x):.2e}")
+            print(f"decode {tag} {ds} -> {tuple(x.shape)}: oracle rel {rel(RO.kl_decode(sd, z), x):.2e}")
             out["decode"].append(dict(cfg=tag, seed=920 + j, shape=ds, x_shape=tuple(x.shape), x=sub(x)))
         for j, es in enumerate(encs):
             img = gen(es, 930 + j).clamp(-1, 1)
             moments = m.encode(img).parameters
             print(f"encode {tag} {es} -> {tuple(moments.shape)}: oracle rel "
-                  f"{MC.rel(RO.kl_encode_moments(sd, img), moments):.2e}")
+                  f"{rel(RO.kl_encode_moments(sd, img), moments):.2e}")
             out["encode"].append(dict(cfg=tag, seed=930 + j, shape=es, moments=moments.clone()))
         del m
 
     # the tiny model, guided (uc = 0) inside ema_scope: DDIM-10 at eta 0 and 1, PLMS-10; c = [text | 2 neighbours]
-    ld = build_ld(arch.TINY_RDM_UNET, arch.TINY_KL_F16)
+    ld = R.build_ld(arch.TINY_RDM_UNET, arch.TINY_KL_F16, LD_COND, **LD_PARAMS)
     usd = arch.random_state_dict(arch.unet_param_shapes(arch.TINY_RDM_UNET), UNET_SEED)
     esd = arch.random_state_dict(arch.unet_param_shapes(arch.TINY_RDM_UNET), EMA_SEED)
     vsd = arch.random_state_dict(arch.vae_param_shapes(arch.TINY_KL_F16), VAE_SEED)
     ld.model.diffusion_model.load_state_dict(usd, strict=True)
     ld.first_stage_model.load_state_dict(vsd, strict=True)
-    bufs = dict(ld.model_ema.named_buffers())
-    for k, v in esd.items():
-        bufs[("diffusion_model." + k).replace(".", "")].copy_(v)
+    R.load_ema(ld, esd)
     plms, ddim = R.build_samplers(ld)
     import ldm.models.diffusion.ddim as ddim_mod
     B, shape = 2, (16, 16, 16)
@@ -170,7 +151,7 @@ def main():
             mine = RO.ddim_sample(fn, x_T, c, uc, GUIDANCE, ld.alphas_cumprod, 10, eta,
                                   torch.stack(draws) if eta else torch.zeros(10, B, *shape))
         print(f"{name} S=10 (EMA weights, scale {GUIDANCE}): sample std {float(s.std()):.3f}, {len(draws)} draws; oracle "
-              f"rel {MC.rel(mine, s):.2e}; decode oracle rel {MC.rel(RO.decode_first_stage(vsd, s), x_dec):.2e}")
+              f"rel {rel(mine, s):.2e}; decode oracle rel {rel(RO.decode_first_stage(vsd, s), x_dec):.2e}")
         out["sampling"][name] = dict(sample=s, x_dec=sub(x_dec), n_noise=len(draws))
     path = os.path.join(OUT, "rdm.pt")
     torch.save(out, path)

@@ -3,7 +3,7 @@ CPU fp32 for the LDM semantic-synthesis models (models/ldm/semantic_synthesis256
 
 Run in the build container:  python oracle/make_golden_semantic.py
 The cond stage is the reference's SpatialRescaler, fed as DDPM.get_input feeds it (np.eye(182)[labels] -> NCHW float).
-clip / kornia are stubbed as in make_golden_cin.py and the VQ quantizer is oracle/vq_oracle.py's (make_golden_vq.py);
+clip / kornia are stubbed and the VQ quantizer is oracle/vq_oracle.py's (ref_harness.install());
 LatentDiffusion, SpatialRescaler, UNetModel, VQModelInterface and DDIMSampler are the reference's own code. Weights come
 from stable-diffusion_b200/arch.random_state_dict (seeded); label maps and soft maps are regenerated from seeds
 (oracle/semantic_oracle.py), so only outputs are stored. Every cond output is also computed by the oracle and must equal
@@ -24,8 +24,8 @@ ROOT = os.path.dirname(HERE)
 sys.path.insert(0, ROOT)
 sys.path.insert(0, HERE)
 
-import make_golden_cin as CG  # noqa: E402
 import ref_harness as R  # noqa: E402
+from ref_harness import gen  # noqa: E402
 import semantic_oracle as SO  # noqa: E402
 from sdb200 import arch  # noqa: E402
 
@@ -43,11 +43,12 @@ COND_CASES = [
     ("tiny_bias", "tiny_bias", "voronoi", 30, 46, 26),
     ("tiny", "tiny", "voronoi", 64, 64, 27),
 ]
+# LatentDiffusion with the semantic_synthesis config's parameters; the cond stage is SpatialRescaler
+COND_TARGET = "ldm.modules.encoders.modules.SpatialRescaler"
+LD_PARAMS = dict(linear_start=LINEAR_START, linear_end=LINEAR_END, log_every_t=100, timesteps=1000, loss_type="l1",
+                 first_stage_key="image", cond_stage_key="segmentation", channels=3, concat_mode=True,
+                 cond_stage_trainable=True)
 COND_CFGS = {"full": arch.SEMANTIC_SYNTHESIS_COND, "tiny": arch.TINY_SEMANTIC_COND, "tiny_bias": TINY_BIAS_COND}
-
-
-def gen(shape, seed, scale=1.0):
-    return scale * torch.randn(shape, generator=torch.Generator().manual_seed(seed))
 
 
 def case_input(kind, h, w, seed, n_classes):
@@ -56,23 +57,6 @@ def case_input(kind, h, w, seed, n_classes):
         return None, SO.soft_map((1, n_classes, h, w), seed)
     lab = SO.voronoi_labels(h, w, n_classes, seed) if kind == "voronoi" else SO.all_ids_labels(h, w, n_classes, seed)
     return torch.from_numpy(lab)[None], None
-
-
-def build_ss_ld(unet_cfg, vq_cfg, cond_cfg, use_ema=True, image_size=None):
-    """The reference's LatentDiffusion with the semantic_synthesis config's parameters."""
-    CG.install()
-    from ldm.models.diffusion.ddpm import LatentDiffusion
-    with contextlib.redirect_stdout(io.StringIO()):
-        m = LatentDiffusion(
-            first_stage_config={"target": "ldm.models.autoencoder.VQModelInterface",
-                                "params": {"embed_dim": vq_cfg["embed_dim"], "n_embed": vq_cfg["n_embed"],
-                                           "ddconfig": vq_cfg["ddconfig"], "lossconfig": {"target": "torch.nn.Identity"}}},
-            cond_stage_config={"target": "ldm.modules.encoders.modules.SpatialRescaler", "params": dict(cond_cfg)},
-            unet_config={"target": "ldm.modules.diffusionmodules.openaimodel.UNetModel", "params": dict(unet_cfg)},
-            linear_start=LINEAR_START, linear_end=LINEAR_END, log_every_t=100, timesteps=1000, loss_type="l1",
-            first_stage_key="image", cond_stage_key="segmentation", image_size=image_size or unet_cfg["image_size"],
-            channels=3, concat_mode=True, cond_stage_trainable=True, use_ema=use_ema)
-    return m.eval()
 
 
 def ref_cond(ld, labels=None, soft=None):
@@ -93,10 +77,11 @@ def main():
     out = {"unet_seed": UNET_SEED, "vq_seed": VQ_SEED, "cond_seed": COND_SEED, "linear_start": LINEAR_START,
            "linear_end": LINEAR_END, "tiny_bias_cond": TINY_BIAS_COND}
     # the reference's key / shape list of the whole model (both checkpoints share it) and its schedule
-    ld = build_ss_ld(arch.SEMANTIC_SYNTHESIS_UNET, arch.VQ_F4, arch.SEMANTIC_SYNTHESIS_COND)
+    cond = {"target": COND_TARGET, "params": arch.SEMANTIC_SYNTHESIS_COND}
+    ld = R.build_ld(arch.SEMANTIC_SYNTHESIS_UNET, arch.VQ_F4, cond, **LD_PARAMS)
     out["ld_keys"] = [(k, tuple(v.shape)) for k, v in ld.state_dict().items()]
     out["alphas_cumprod"] = ld.alphas_cumprod.clone()
-    ld512 = build_ss_ld(arch.SEMANTIC_SYNTHESIS_UNET, arch.VQ_F4, arch.SEMANTIC_SYNTHESIS_COND, image_size=128)
+    ld512 = R.build_ld(arch.SEMANTIC_SYNTHESIS_UNET, arch.VQ_F4, cond, image_size=128, **LD_PARAMS)
     assert [(k, tuple(v.shape)) for k, v in ld512.state_dict().items()] == out["ld_keys"]
     del ld, ld512
 
@@ -106,7 +91,8 @@ def main():
     for tag, cname, kind, h, w, seed in COND_CASES:
         cfg = COND_CFGS[cname]
         if cname not in cond_lds:
-            ld = build_ss_ld(arch.TINY_SEMANTIC_UNET, arch.TINY_VQ_F4, cfg, use_ema=False)
+            ld = R.build_ld(arch.TINY_SEMANTIC_UNET, arch.TINY_VQ_F4, {"target": COND_TARGET, "params": cfg},
+                            use_ema=False, **LD_PARAMS)
             sd = arch.random_state_dict(arch.spatial_rescaler_param_shapes(cfg), COND_SEED)
             ld.cond_stage_model.load_state_dict(sd, strict=True)
             cond_lds[cname] = (ld, sd)
@@ -136,7 +122,8 @@ def main():
         del net
 
     # log_images' sampling on the tiny model: conditioning from a 64x64 label map, DDIM-10 at eta 0 and 1, decode
-    ld = build_ss_ld(arch.TINY_SEMANTIC_UNET, arch.TINY_VQ_F4, arch.TINY_SEMANTIC_COND, use_ema=False)
+    cond = {"target": COND_TARGET, "params": arch.TINY_SEMANTIC_COND}
+    ld = R.build_ld(arch.TINY_SEMANTIC_UNET, arch.TINY_VQ_F4, cond, use_ema=False, **LD_PARAMS)
     ld.model.diffusion_model.load_state_dict(arch.random_state_dict(arch.unet_param_shapes(arch.TINY_SEMANTIC_UNET),
                                                                     UNET_SEED), strict=True)
     ld.first_stage_model.load_state_dict(arch.random_state_dict(arch.vq_param_shapes(arch.TINY_VQ_F4), VQ_SEED),

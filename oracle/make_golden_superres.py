@@ -3,9 +3,9 @@ CPU fp32 for the LDM super-resolution model (models/ldm/bsr_sr/config.yaml, note
 
 Run in the build container:  python oracle/make_golden_superres.py
 notebook_helpers.py is imported as it is; its notebook-only imports (google.colab, IPython.display, ipywidgets) and the
-bare `display` that get_cond calls are stubbed here. As in make_golden_vq.py, taming's quantizer is oracle/vq_oracle.py's
-restatement. Weights come from stable-diffusion_b200/arch.random_state_dict (seeded); large tables are stored as the
-SHA-256 of their bytes, inputs are regenerated from seeds.
+bare `display` that get_cond calls are stubbed here. taming's quantizer is oracle/vq_oracle.py's restatement (set by
+ref_harness.install()). Weights come from stable-diffusion_b200/arch.random_state_dict (seeded); large tables are stored
+as the SHA-256 of their bytes, inputs are regenerated from seeds.
 """
 from __future__ import annotations
 
@@ -25,8 +25,8 @@ ROOT = os.path.dirname(HERE)
 sys.path.insert(0, ROOT)
 sys.path.insert(0, HERE)
 
-import make_golden_vq as GV  # noqa: E402
 import ref_harness as R  # noqa: E402
+from ref_harness import gen  # noqa: E402
 import superres_oracle as S  # noqa: E402
 import sdb200  # noqa: E402,F401
 from sdb200 import arch  # noqa: E402
@@ -43,15 +43,16 @@ TABLES = [
     ("tiny_tie_uf4", 24, 40, S.notebook_params(16, 8, tie_braker=True), 4),
     ("tiny_stride4_uf1", 20, 28, S.notebook_params(12, 4), 1),
 ]
+# LatentDiffusion with the bsr_sr config's parameters; the cond stage is Identity: the LR image is concatenated as it is
+LD_PARAMS = dict(linear_start=LINEAR_START, linear_end=LINEAR_END, log_every_t=100, timesteps=1000, loss_type="l2",
+                 first_stage_key="image", cond_stage_key="LR_image", channels=3, concat_mode=True,
+                 cond_stage_trainable=False)
+LD_COND = {"target": "torch.nn.Identity"}
 BIG = 64 * 1024            # tables larger than this many bytes are stored as their SHA-256
 
 
 def sha(t):
     return hashlib.sha256(t.contiguous().numpy().tobytes()).hexdigest()
-
-
-def gen(shape, seed, scale=1.0):
-    return scale * torch.randn(shape, generator=torch.Generator().manual_seed(seed))
 
 
 def notebook_module():
@@ -73,24 +74,6 @@ def notebook_module():
     return mod
 
 
-def build_bsr_ld(unet_cfg, vq_cfg, use_ema=True):
-    """The reference's LatentDiffusion with the bsr_sr config's parameters."""
-    GV.install()
-    from ldm.models.diffusion.ddpm import LatentDiffusion
-    with contextlib.redirect_stdout(io.StringIO()):
-        m = LatentDiffusion(
-            first_stage_config={"target": "ldm.models.autoencoder.VQModelInterface",
-                                "params": {"embed_dim": vq_cfg["embed_dim"], "n_embed": vq_cfg["n_embed"],
-                                           "monitor": "val/rec_loss", "ddconfig": vq_cfg["ddconfig"],
-                                           "lossconfig": {"target": "torch.nn.Identity"}}},
-            cond_stage_config={"target": "torch.nn.Identity"},
-            unet_config={"target": "ldm.modules.diffusionmodules.openaimodel.UNetModel", "params": dict(unet_cfg)},
-            linear_start=LINEAR_START, linear_end=LINEAR_END, log_every_t=100, timesteps=1000, loss_type="l2",
-            first_stage_key="image", cond_stage_key="LR_image", image_size=unet_cfg["image_size"], channels=3,
-            concat_mode=True, cond_stage_trainable=False, use_ema=use_ema)
-    return m.eval()
-
-
 def lr_png(h, w, seed):
     g = np.random.default_rng(seed)
     img = g.integers(0, 256, (h, w, 3), dtype=np.uint8)
@@ -102,7 +85,7 @@ def lr_png(h, w, seed):
 def main():
     nb = notebook_module()
     out = {"unet_seed": UNET_SEED, "vq_seed": VQ_SEED, "linear_start": LINEAR_START, "linear_end": LINEAR_END}
-    ld = build_bsr_ld(arch.BSR_SR_UNET, arch.VQ_F4)
+    ld = R.build_ld(arch.BSR_SR_UNET, arch.VQ_F4, LD_COND, **LD_PARAMS)
     out["ld_keys"] = [(k, tuple(v.shape)) for k, v in ld.state_dict().items()]
     assert not [k for k in out["ld_keys"] if k[0].startswith("cond_stage_model.")]
 
@@ -157,7 +140,7 @@ def main():
         del net
 
     # VQ-f4 decode (mid-block attention) of one small latent
-    m = GV.build_vq(arch.VQ_F4)
+    m = R.build_vq(arch.VQ_F4)
     m.load_state_dict(arch.random_state_dict(arch.vq_param_shapes(arch.VQ_F4), VQ_SEED), strict=True)
     h = gen((1, 3, 16, 24), 931)
     out["vq_f4"] = dict(h=h, dec=m.decode(h))
@@ -165,7 +148,7 @@ def main():
     del m
 
     # make_convolutional_sample end to end on the tiny model, split at ks 16 / stride 8 / vqf 4, DDIM-10 at eta 0 and 1
-    ld = build_bsr_ld(arch.TINY_BSR_UNET, arch.TINY_VQ_F4, use_ema=False)
+    ld = R.build_ld(arch.TINY_BSR_UNET, arch.TINY_VQ_F4, LD_COND, use_ema=False, **LD_PARAMS)
     ld.model.diffusion_model.load_state_dict(arch.random_state_dict(arch.unet_param_shapes(arch.TINY_BSR_UNET),
                                                                     UNET_SEED), strict=True)
     ld.first_stage_model.load_state_dict(arch.random_state_dict(arch.vq_param_shapes(arch.TINY_VQ_F4), VQ_SEED),

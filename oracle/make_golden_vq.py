@@ -24,6 +24,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, HERE)
 
 import ref_harness as R  # noqa: E402
+from ref_harness import gen, rel  # noqa: E402
 import uncond_oracle as U  # noqa: E402
 import vq_oracle as V  # noqa: E402
 import sdb200  # noqa: E402,F401
@@ -32,46 +33,9 @@ from sdb200 import arch  # noqa: E402
 OUT = os.path.join(ROOT, "tests", "golden")
 UNET_SEED, VQ_SEED, EMA_SEED = 11, 12, 31
 LINEAR_START, LINEAR_END = 0.0015, 0.0195
-
-
-def rel(a, b):
-    return float((a.double() - b.double()).norm() / b.double().norm())
-
-
-def gen(shape, seed, scale=1.0):
-    return scale * torch.randn(shape, generator=torch.Generator().manual_seed(seed))
-
-
-def install():
-    R.install()
-    import ldm.models.autoencoder as ae
-    ae.VectorQuantizer = V.VectorQuantizer2
-
-
-def build_vq(cfg):
-    install()
-    from ldm.models.autoencoder import VQModelInterface
-    with contextlib.redirect_stdout(io.StringIO()):
-        m = VQModelInterface(embed_dim=cfg["embed_dim"], n_embed=cfg["n_embed"], ddconfig=cfg["ddconfig"],
-                             lossconfig={"target": "torch.nn.Identity"})
-    return m.eval()
-
-
-def build_vq_ld(unet_cfg, vq_cfg, use_ema=True):
-    """The reference's LatentDiffusion with the celebahq-ldm-vq-4.yaml parameters."""
-    install()
-    from ldm.models.diffusion.ddpm import LatentDiffusion
-    with contextlib.redirect_stdout(io.StringIO()):
-        m = LatentDiffusion(
-            first_stage_config={"target": "ldm.models.autoencoder.VQModelInterface",
-                                "params": {"embed_dim": vq_cfg["embed_dim"], "n_embed": vq_cfg["n_embed"],
-                                           "ddconfig": vq_cfg["ddconfig"], "lossconfig": {"target": "torch.nn.Identity"}}},
-            cond_stage_config="__is_unconditional__",
-            unet_config={"target": "ldm.modules.diffusionmodules.openaimodel.UNetModel", "params": dict(unet_cfg)},
-            linear_start=LINEAR_START, linear_end=LINEAR_END, num_timesteps_cond=1, log_every_t=200, timesteps=1000,
-            first_stage_key="image", image_size=unet_cfg["image_size"], channels=unet_cfg["in_channels"],
-            monitor="val/loss_simple_ema", use_ema=use_ema)
-    return m.eval()
+# LatentDiffusion with the celebahq-ldm-vq-4.yaml parameters
+LD_PARAMS = dict(linear_start=LINEAR_START, linear_end=LINEAR_END, num_timesteps_cond=1, log_every_t=200,
+                 timesteps=1000, first_stage_key="image", monitor="val/loss_simple_ema", use_ema=True)
 
 
 @torch.no_grad()
@@ -81,7 +45,7 @@ def main():
     net = R.build_unet(arch.CELEBAHQ_UNET)
     out["celebahq_unet_keys"] = [(k, tuple(v.shape)) for k, v in net.state_dict().items()]
     del net
-    out["vq_f4_keys"] = [(k, tuple(v.shape)) for k, v in build_vq(arch.VQ_F4).state_dict().items()]
+    out["vq_f4_keys"] = [(k, tuple(v.shape)) for k, v in R.build_vq(arch.VQ_F4).state_dict().items()]
 
     out["unet"] = []
     for tag, cfg, shapes in (
@@ -107,7 +71,7 @@ def main():
         ("vq_f4", arch.VQ_F4, (2, 3, 16, 24), [(1, 3, 16, 16), (1, 3, 16, 24)]),
     ):
         sd = arch.random_state_dict(arch.vq_param_shapes(cfg), VQ_SEED)
-        m = build_vq(cfg)
+        m = R.build_vq(cfg)
         m.load_state_dict(sd, strict=True)
         z = gen(zs, 910)
         z_q, _, (_, _, idx) = m.quantize(z)
@@ -131,12 +95,10 @@ def main():
     usd = arch.random_state_dict(arch.unet_param_shapes(arch.TINY_VQ_UNET), UNET_SEED)
     esd = arch.random_state_dict(arch.unet_param_shapes(arch.TINY_VQ_UNET), EMA_SEED)
     vsd = arch.random_state_dict(arch.vq_param_shapes(arch.TINY_VQ), VQ_SEED)
-    ld = build_vq_ld(arch.TINY_VQ_UNET, arch.TINY_VQ, use_ema=True)
+    ld = R.build_ld(arch.TINY_VQ_UNET, arch.TINY_VQ, "__is_unconditional__", **LD_PARAMS)
     ld.model.diffusion_model.load_state_dict(usd, strict=True)
     ld.first_stage_model.load_state_dict(vsd, strict=True)
-    bufs = dict(ld.model_ema.named_buffers())
-    for k, v in esd.items():
-        bufs[("diffusion_model." + k).replace(".", "")].copy_(v)
+    R.load_ema(ld, esd)
     _, ddim = R.build_samplers(ld)
     B, shape = 2, [3, 16, 16]
     x_T = gen((B, *shape), 940)
