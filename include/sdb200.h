@@ -199,7 +199,8 @@ int sdb_im2col3x3(const float* x, int32_t nb, int32_t h, int32_t w, int32_t c, i
 int sdb_im2col3x3_concat(const float* x, int32_t nb, int32_t cx, int32_t h, int32_t w, const float* cond,
                          int32_t cond_nb, int32_t cc, int32_t cond_h, int32_t cond_w, int32_t kpad, void* out_f16,
                          sdb_stream_t stream);
-/* nearest 2x upsample NHWC fp32 -> fp16 (openaimodel.py:116; model.py:54) */
+/* nearest 2x upsample NHWC fp32 -> fp16 (openaimodel.py:116; model.py:54). c % 4 == 0; x 16-byte and out_f16 8-byte
+ * aligned. */
 int sdb_upsample2x(const float* x, int32_t nb, int32_t h, int32_t w, int32_t c, void* out_f16, sdb_stream_t stream);
 /* fp32 -> fp16 cast, optional transpose of [rows, cols] per batch into [cols, ldo] */
 int sdb_cast_f16(const float* x, int64_t n, void* out_f16, sdb_stream_t stream);
@@ -263,7 +264,8 @@ int sdb_vae_sample(const float* moments, const float* noise_nchw, int32_t nb, in
                    float* z_nchw, sdb_stream_t stream);
 int sdb_to_uint8(const float* x_nhwc, int64_t n, uint8_t* out, sdb_stream_t stream);
 /* 2x2 resample of the fp32 residual stream (ResBlock.x_upd, openaimodel.py:209-214,260): NHWC [nb, h, w, c] ->
- * mode 1: 2x2 average pool [nb, h/2, w/2, c] (summed in avg_pool2d's order, then / 4); mode 2: nearest 2x [nb, 2h, 2w, c] */
+ * mode 1: 2x2 average pool [nb, h/2, w/2, c] (summed in avg_pool2d's order, then / 4); mode 2: nearest 2x [nb, 2h, 2w, c].
+ * c % 4 == 0; x and out 16-byte aligned. */
 int sdb_resample_f32(const float* x, int32_t nb, int32_t h, int32_t w, int32_t c, int32_t mode, float* out,
                      sdb_stream_t stream);
 /* Ancestral DDPM step, LatentDiffusion.p_sample with clip_denoised=False (ddpm.py:1047-1108), one timestep per call:

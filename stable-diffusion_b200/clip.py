@@ -109,11 +109,34 @@ class FrozenCLIPEmbedder(PackedStage):
                   "layers": pack_clip_layers(sd, "text_model.encoder.layers", self.cfg["num_hidden_layers"]),
                   "ln_f": (f32("text_model.final_layer_norm.weight"), f32("text_model.final_layer_norm.bias"))}
 
+    def check_ids(self, ids):
+        """Host-side validation before any launch. sdb_embed_tokens reads position row i for token i, so a sequence
+        longer than the position table raises here, as do non-integer and non-2-D ids. It clamps ids to the vocabulary,
+        so ids outside [0, vocab_size) raise here too when they are on the host (tokenizer output, or ids handed to
+        forward / encode_ids from the CPU); ids already on the GPU are not read back, since that would stall the
+        stream once per prompt."""
+        if not torch.is_tensor(ids) or ids.dtype.is_floating_point or ids.dtype.is_complex or ids.dtype == torch.bool \
+                or ids.dim() != 2:
+            raise TypeError(f"{type(self).__name__}: token ids must be a 2-D integer tensor [B, n] (got "
+                            f"{getattr(ids, 'dtype', type(ids))}, shape {tuple(getattr(ids, 'shape', ()))})")
+        B, n = ids.shape
+        n_pos = self.cfg["max_position_embeddings"]
+        if B == 0 or not 1 <= n <= n_pos:
+            raise ValueError(f"{type(self).__name__}: need B >= 1 and 1 <= n <= {n_pos} tokens (got {tuple(ids.shape)})")
+        if not ids.is_cuda:
+            lo, hi = int(ids.min()), int(ids.max())
+            if lo < 0 or hi >= self.cfg["vocab_size"]:
+                raise IndexError(f"{type(self).__name__}: token ids must lie in [0, {self.cfg['vocab_size']}) "
+                                 f"(got {lo} .. {hi})")
+
     @torch.no_grad()
     def encode_ids(self, ids):
-        """ids: int64 [B, n<=77] on the GPU -> fp32 [B, n, hidden]."""
-        assert self.W is not None and ids.is_cuda, "sdb200.FrozenCLIPEmbedder runs on CUDA only (no CPU fallback)"
+        """ids: integer [B, n <= max_position_embeddings] (host ids are checked, then moved) -> fp32 [B, n, hidden] on
+        the GPU."""
+        assert self.W is not None, "weights not loaded (load_state_dict / load_weights, then .cuda())"
+        self.check_ids(ids)
         W = self.W
+        ids = ids.to(W["device"], torch.int64)
         B, n = ids.shape
         h = self.cfg["hidden_size"]
         heads = self.cfg["num_attention_heads"]
@@ -158,7 +181,7 @@ class FrozenCLIPEmbedder(PackedStage):
             ids = text
         else:
             ids = self._tokenize(text)
-        return self.encode_ids(ids.to(self.W["device"]).long())
+        return self.encode_ids(ids)
 
     def encode(self, text):
         return self(text)
@@ -212,9 +235,10 @@ class FrozenCLIPTextEmbedder(FrozenCLIPEmbedder):
 
     @torch.no_grad()
     def encode_ids(self, ids):
-        """ids: int64 [B, n] on the GPU, EOT = the largest id of each row -> fp32 [B, projection_dim], normalised when
-        `normalize` (the reference's forward)."""
-        ids = ids.contiguous()
+        """ids: integer [B, n] (host ids are checked, then moved), EOT = the largest id of each row -> fp32
+        [B, projection_dim] on the GPU, normalised when `normalize` (the reference's forward)."""
+        self.check_ids(ids)
+        ids = ids.to(self.W["device"], torch.int64).contiguous()
         h = super().encode_ids(ids)                                                     # [B, n, hidden], final LN
         pooled = ops.rows_pool(h.view(-1, h.shape[-1]), ids)                           # the EOT rows
         z = ops.linear_small(pooled, self.W["proj"])
@@ -222,7 +246,7 @@ class FrozenCLIPTextEmbedder(FrozenCLIPEmbedder):
 
     def forward(self, text):
         ids = text if torch.is_tensor(text) else self.tokenize(text)
-        return self.encode_ids(ids.to(self.W["device"]).long())
+        return self.encode_ids(ids)
 
     def encode(self, text):
         z = self(text)

@@ -359,6 +359,8 @@ extern "C" int sdb_upsample2x(const float* x, int32_t nb, int32_t h, int32_t w, 
                               sdb_stream_t stream) {
   SDB_REC(sdb_upsample2x(x, nb, h, w, c, out_f16, s_));
   SDB_CHECK(x && out_f16 && c % 4 == 0, "sdb_upsample2x: bad arguments");
+  SDB_CHECK((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(out_f16) & 7) == 0,
+            "sdb_upsample2x: x must be 16-byte and out 8-byte aligned");
   size_t total = static_cast<size_t>(nb) * 4 * h * w * (c / 4);
   upsample2x_kernel<<<grid_for(total), 256, 0, ST>>>(x, nb, h, w, c, static_cast<__half*>(out_f16));
   SDB_LAUNCH_CHECK();
@@ -492,6 +494,8 @@ extern "C" int sdb_resample_f32(const float* x, int32_t nb, int32_t h, int32_t w
   SDB_REC(sdb_resample_f32(x, nb, h, w, c, mode, out, s_));
   SDB_CHECK(x && out && nb > 0 && h > 0 && w > 0 && c > 0 && c % 4 == 0, "sdb_resample_f32: bad arguments");
   SDB_CHECK(mode == 1 || mode == 2, "sdb_resample_f32: mode %d (1 down, 2 up)", mode);
+  SDB_CHECK(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(out)) & 15) == 0,
+            "sdb_resample_f32: x and out must be 16-byte aligned");
   SDB_CHECK(mode != 1 || (h % 2 == 0 && w % 2 == 0), "sdb_resample_f32: 2x2 average pool needs even sides (%dx%d)", h, w);
   const size_t total = static_cast<size_t>(nb) * h * w * (c / 4) * (mode == 1 ? 1 : 4) / (mode == 1 ? 4 : 1);
   resample_f32_kernel<<<grid_for(total), 256, 0, ST>>>(x, nb, h, w, c, mode, out);

@@ -902,10 +902,13 @@ def pointwise_small(x, w, b=None, alpha=1.0):
 
 
 def embed_tokens(ids, tok, pos):
-    """ids int64 [B, n] -> fp32 [B*n, dim]."""
+    """ids int64 [B, n] -> fp32 [B*n, dim]: tok[ids] + pos[:n]. Ids outside [0, vocab) are clamped by the kernel, so
+    callers validate them on the host."""
     assert ids.dtype == torch.int64 and ids.is_cuda and ids.is_contiguous()
     B, n = ids.shape
     dim = tok.shape[1]
+    assert pos.dim() == 2 and pos.shape[0] >= n and pos.shape[1] == dim, (tuple(ids.shape), tuple(tok.shape),
+                                                                         tuple(pos.shape))
     out = torch.empty((B * n, dim), dtype=torch.float32, device=ids.device)
     _l.check(_l.load().sdb_embed_tokens(_ptr(ids), B * n, n, dim, tok.shape[0], _ptr(tok), _ptr(pos), _ptr(out),
                                         _stream()), "sdb_embed_tokens")

@@ -1,6 +1,6 @@
 """One eager forward of each model with random weights: the workloads whose kernel launches the sweeps record
-(test_norm_sweep_gpu.py, test_attention_sweep_gpu.py, test_gemm_plans_gpu.py and the GEMM plan sweeps in the model
-test files). Each table maps a name to a function of the device; a problem's operands are seeded by its index in the
+(test_norm_sweep_gpu.py, test_attention_sweep_gpu.py, test_elementwise_sweep_gpu.py, test_gemm_plans_gpu.py and the
+GEMM plan sweeps in the model test files). Each table maps a name to a function of the device; a problem's operands are seeded by its index in the
 recorded list, so an entry's shapes and call order are part of what a sweep checks."""
 import torch
 
@@ -192,6 +192,42 @@ ATTENTION_WORKLOADS = {
     "vq_f4_128x128_latent": _wl_vq_sr_tile,                                    # 16384 tokens at d = 512
     "vit_l14_b37": lambda dev: _clip_image(arch.CLIP_VISION_PROJ, dev, 37),
     "rdm_one_token_context": lambda dev: _run_unet(arch.RDM_UNET, [(2, 16, 48, 48)], dev, ctx=(1, 768)),
+}
+
+def _wl_cin256_class_embedder(dev):
+    """The ClassEmbedder on all 1001 labels (1000: the unconditional one): embed_tokens with a one-row position table,
+    then the one-token-context projection of every SpatialTransformer (UNetModel.context_kv)."""
+    import sdb200
+    cfg = arch.CIN256_V2_COND
+    emb = sdb200.ClassEmbedder(**cfg).load_weights(_sd(arch.class_embedder_param_shapes, cfg, 15, dev), dev)
+    c = emb({cfg["key"]: torch.arange(cfg["n_classes"], device=dev).flip(0)})
+    _unet(arch.CIN256_V2_UNET, dev).context_kv(c)
+
+
+def _wl_sdv1_vae_sample(dev):
+    """SD-v1 VAE encode with a posterior sample (vae_sample) at 512² and 512x768."""
+    g = torch.Generator(device=dev).manual_seed(7)
+    vae = _vae(arch.SD_V1_VAE, dev)
+    for h, w in ((512, 512), (512, 768)):
+        vae.encode(torch.rand(1, 3, h, w, generator=g, device=dev) * 2 - 1).sample(
+            noise=torch.randn(1, 4, h // 8, w // 8, generator=g, device=dev), scale=0.18215)
+
+
+def _wl_sdv1_decode_uint8(dev):
+    """SD-v1 decodes to uint8 images as the txt2img / img2img pipelines return them: 2 x 512² and 1 x 512x768."""
+    g = torch.Generator(device=dev).manual_seed(8)
+    vae = _vae(arch.SD_V1_VAE, dev)
+    for s in ((2, 4, 64, 64), (1, 4, 64, 96)):
+        ops.to_uint8(vae.decode(torch.randn(*s, generator=g, device=dev), scale=1 / 0.18215, nhwc=True))
+
+
+# the elementwise sweep: what a plain forward of the tables above does not reach
+ELEMENTWISE_WORKLOADS = {
+    **ATTENTION_WORKLOADS,
+    "cin256_class_embedder": _wl_cin256_class_embedder,
+    "sdv1_vae_sample": _wl_sdv1_vae_sample,
+    "vit_l14_b256": lambda dev: _clip_image(arch.CLIP_VISION_PROJ, dev, 256),  # rows_gather stride 257, projection M 256
+    "sdv1_decode_uint8": _wl_sdv1_decode_uint8,
 }
 
 # test_gemm_plans_gpu.py
