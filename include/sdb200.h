@@ -63,10 +63,13 @@ typedef struct sdb_gemm_desc {
   int32_t c0, c1, c2, c3;
   int32_t nb, h, w;      /* rows M = nb*h*w */
   int32_t taps;          /* 1 or 9 */
-  const void* b;         /* fp16 [n, taps*(c0+c1)] */
+  const void* b;         /* fp16 [n, taps*(c0+c1)]. Unless b_dynamic is set, b is streamed ahead of the programmatic-
+                            launch wait (griddepcontrol.wait), while earlier kernels of the stream may still run: it must
+                            not be written by any kernel still in flight (in practice: packed weights) */
   int32_t n;
   float alpha;
-  const float* bias;     /* [n] or NULL */
+  const float* bias;     /* [n] or NULL. Read ahead of the programmatic-launch wait by the split-K second pass: it must not
+                            be written by any kernel still in flight (in practice: packed weights) */
   const float* film;     /* [M / rows_per_sample, ldf] or NULL (timestep FiLM add, openaimodel.py:271-274) */
   int32_t ldf;           /* row stride of film (0 = n) */
   int32_t rows_per_sample;
@@ -88,8 +91,10 @@ typedef struct sdb_gemm_desc {
                             produced, so no separate reduction pass reads it again. T comes from sdb_gemm_plan; the
                             consumer (sdb_groupnorm) folds the T slots */
   int32_t stats_prezeroed; /* unused (kept for layout compatibility) */
-  int32_t b_dynamic;       /* non-zero: b is an activation produced by the preceding kernel (e.g. V^T = W_v . X^T swaps
-                              the operand roles), so it must not be prefetched ahead of the programmatic-launch wait */
+  int32_t b_dynamic;       /* non-zero: b is read only after the programmatic-launch wait. Required whenever b may be
+                              written by a kernel that can still be in flight: not just the preceding one, but any
+                              earlier kernel of an unbroken chain of programmatic launches, since every kernel lets its
+                              successor start before it finishes (e.g. V^T = W_v . X^T, which swaps the operand roles) */
   int32_t conv_stride;     /* taps = 9 only. 0/1: stride 1. 2: stride-2 conv read straight from the NHWC input through
                               strided TMA boxes (no im2col): Downsample, openaimodel.py:149-153; model.py:72-76 */
   int32_t conv_shift;      /* input pixel of output o, tap t (per axis) = stride*o + t - 1 + conv_shift: 0 = zero pad 1
@@ -149,7 +154,10 @@ int sdb_attention(const sdb_attn_desc* d, sdb_stream_t stream);
  * for the following conv and optionally a raw fp16 cast of the (concatenated) input for the 1x1 skip conv.
  */
 int sdb_groupnorm(const float* x0, const float* x1, int32_t c0, int32_t c1, int32_t nb, int32_t hw, int32_t groups,
-                  const float* gamma, const float* beta, float eps, int32_t silu, void* out_f16, void* raw_f16,
+                  const float* gamma /* gamma / beta are read ahead of the programmatic-launch wait, while earlier
+                                        kernels of the stream may still run: they must not be written by any kernel
+                                        still in flight (in practice: packed weights) */,
+                  const float* beta, float eps, int32_t silu, void* out_f16, void* raw_f16,
                   void* out_lo_f16 /* optional low half of the normalised output (hi/lo split) */,
                   void* raw_lo_f16 /* optional low half of the raw cast */,
                   void* stats_ws /* scratch: nb * (128*groups*2 + groups*2 + 1) * 4 bytes */,
@@ -175,7 +183,9 @@ int sdb_groupnorm_mod(const float* x, int32_t c, int32_t nb, int32_t h, int32_t 
                       int32_t resample, void* out_f16, void* stats_ws, const void* chan_stats, int32_t stats_t,
                       int32_t stats_group, sdb_stream_t stream);
 
-/* LayerNorm over the last dim of fp32 [rows, c] -> fp16 (attention.py:203-205, eps 1e-5). */
+/* LayerNorm over the last dim of fp32 [rows, c] -> fp16 (attention.py:203-205, eps 1e-5). gamma / beta are read ahead
+ * of the programmatic-launch wait (c = 320, 512, 640, 768, 1280 with 8-byte aligned operands), while earlier kernels of
+ * the stream may still run: they must not be written by any kernel still in flight (in practice: packed weights). */
 int sdb_layernorm(const float* x, int32_t rows, int32_t c, const float* gamma, const float* beta, float eps,
                   void* out_f16, float* out_f32 /* optional */, sdb_stream_t stream);
 

@@ -1,7 +1,8 @@
 """One eager forward of each model with random weights: the workloads whose kernel launches the sweeps record
 (test_norm_sweep_gpu.py, test_attention_sweep_gpu.py, test_elementwise_sweep_gpu.py, test_gemm_plans_gpu.py and the
 GEMM plan sweeps in the model test files). Each table maps a name to a function of the device; a problem's operands are seeded by its index in the
-recorded list, so an entry's shapes and call order are part of what a sweep checks."""
+recorded list, so an entry's shapes and call order are part of what a sweep checks. Each function returns what it
+computes (tensors, possibly nested in lists and tuples), which test_pdl_order_gpu.py digests bit for bit."""
 import torch
 
 import helpers  # noqa: F401  (puts the repository on sys.path)
@@ -21,15 +22,17 @@ def _run_unet(cfg, shapes, dev, ctx=None, concat=0):
     """One UNet evaluation per shape; concat > 0 passes the last `concat` channels as the concat conditioning."""
     net = _unet(cfg, dev)
     g = torch.Generator(device=dev).manual_seed(0)
+    outs = []
     for s in shapes:
         x = torch.randn(*s, generator=g, device=dev)
         t = torch.linspace(1, 981, s[0], device=dev).round()
         c = None if ctx is None else torch.randn(s[0], *ctx, generator=g, device=dev)
         if concat:
-            net(x[:, :s[1] - concat].contiguous(), t, concat=x[:, s[1] - concat:].contiguous())
+            outs.append(net(x[:, :s[1] - concat].contiguous(), t, concat=x[:, s[1] - concat:].contiguous()))
         else:
-            net(x, t, context=c)
+            outs.append(net(x, t, context=c))
     del net
+    return outs
 
 
 def _vae(cfg, dev):
@@ -47,12 +50,12 @@ def _clip(cfg, dev, ids):
     cls = sdb200.FrozenCLIPTextEmbedder if "projection_dim" in cfg else sdb200.FrozenCLIPEmbedder
     shapes = arch.clip_text_proj_param_shapes if "projection_dim" in cfg else arch.clip_param_shapes
     enc = cls(config=cfg).load_weights(_sd(shapes, cfg, 13, dev), dev)
-    enc.encode_ids(ids)
+    return enc.encode_ids(ids)
 
 
 def _bert(cfg, dev, ids):
     import sdb200
-    sdb200.BERTEmbedder(**cfg, use_tokenizer=False).load_weights(_sd(arch.bert_param_shapes, cfg, 13, dev),
+    return sdb200.BERTEmbedder(**cfg, use_tokenizer=False).load_weights(_sd(arch.bert_param_shapes, cfg, 13, dev),
                                                                  dev).encode_ids(ids)
 
 
@@ -65,7 +68,7 @@ def _clip_image_embedder(cfg, dev):
 def _clip_image(cfg, dev, B):
     e = _clip_image_embedder(cfg, dev)
     g = torch.Generator(device=dev).manual_seed(5)
-    e(torch.rand(B, 3, 224, 224, generator=g, device=dev) * 2 - 1)
+    return e(torch.rand(B, 3, 224, 224, generator=g, device=dev) * 2 - 1)
 
 
 def _ids(vocab, B, dev):
@@ -77,97 +80,96 @@ def _wl_sdv1_first(dev):
     import sdb200
     g = torch.Generator(device=dev).manual_seed(1)
     vae = _vae(arch.SD_V1_VAE, dev)
-    vae.decode(torch.randn(1, 4, 64, 64, generator=g, device=dev))
-    vae.encode(torch.rand(1, 3, 512, 512, generator=g, device=dev) * 2 - 1)
+    img = vae.decode(torch.randn(1, 4, 64, 64, generator=g, device=dev))
+    post = vae.encode(torch.rand(1, 3, 512, 512, generator=g, device=dev) * 2 - 1)
     del vae
-    _clip(arch.SD_V1_CLIP, dev, _ids(49408, 2, dev))
+    c = _clip(arch.SD_V1_CLIP, dev, _ids(49408, 2, dev))
     chk = sdb200.StableDiffusionSafetyChecker(config=arch.SD_V1_SAFETY).load_weights(
         _sd(arch.safety_param_shapes, arch.SD_V1_SAFETY, 14, dev), dev)
-    chk.image_embeds(torch.randn(1, 3, 224, 224, generator=g, device=dev))
+    return img, post, c, chk.image_embeds(torch.randn(1, 3, 224, 224, generator=g, device=dev))
 
 
 def _wl_laion(dev, text_batch, unet_batches):
-    _bert(arch.LAION_BERT, dev, _ids(30522, text_batch, dev))
-    _run_unet(arch.LAION_UNET, [(nb, 4, 64, 64) for nb in unet_batches], dev, ctx=(77, 1280))
+    return (_bert(arch.LAION_BERT, dev, _ids(30522, text_batch, dev)),
+            _run_unet(arch.LAION_UNET, [(nb, 4, 64, 64) for nb in unet_batches], dev, ctx=(77, 1280)))
 
 
 def _wl_rdm_unet_kl(dev, nb):
     g = torch.Generator(device=dev).manual_seed(2)
-    _run_unet(arch.RDM_UNET, [(nb, 16, 48, 48)], dev, ctx=(11, 768))
-    _vae(arch.KL_F16, dev).decode(torch.randn(1, 16, 24, 24, generator=g, device=dev))
+    return (_run_unet(arch.RDM_UNET, [(nb, 16, 48, 48)], dev, ctx=(11, 768)),
+            _vae(arch.KL_F16, dev).decode(torch.randn(1, 16, 24, 24, generator=g, device=dev)))
 
 
 def _wl_rdm(dev):
-    _wl_rdm_unet_kl(dev, 2)
-    _clip(arch.CLIP_TEXT_PROJ, dev, _ids(49408, 2, dev))
-    _clip_image(arch.CLIP_VISION_PROJ, dev, 2)
+    return (_wl_rdm_unet_kl(dev, 2), _clip(arch.CLIP_TEXT_PROJ, dev, _ids(49408, 2, dev)),
+            _clip_image(arch.CLIP_VISION_PROJ, dev, 2))
 
 
 def _wl_celebahq(dev, nb):
     g = torch.Generator(device=dev).manual_seed(2)
-    _run_unet(arch.CELEBAHQ_UNET, [(nb, 3, 64, 64)], dev)
-    _vq(arch.VQ_F4, dev).decode(torch.randn(1, 3, 64, 64, generator=g, device=dev))
+    return (_run_unet(arch.CELEBAHQ_UNET, [(nb, 3, 64, 64)], dev),
+            _vq(arch.VQ_F4, dev).decode(torch.randn(1, 3, 64, 64, generator=g, device=dev)))
 
 
 def _wl_cin_f8(dev, nb):
     g = torch.Generator(device=dev).manual_seed(2)
-    _run_unet(arch.CIN256_F8_UNET, [(nb, 4, 32, 32)], dev, ctx=(1, 512))
-    _vq(arch.VQ_F8, dev).decode(torch.randn(1, 4, 32, 32, generator=g, device=dev))
+    return (_run_unet(arch.CIN256_F8_UNET, [(nb, 4, 32, 32)], dev, ctx=(1, 512)),
+            _vq(arch.VQ_F8, dev).decode(torch.randn(1, 4, 32, 32, generator=g, device=dev)))
 
 
 def _wl_inpaint(dev, batches):
     g = torch.Generator(device=dev).manual_seed(3)
-    _run_unet(arch.INPAINTING_BIG_UNET, [(nb, 7, 128, 128) for nb in batches], dev, concat=4)
+    eps = _run_unet(arch.INPAINTING_BIG_UNET, [(nb, 7, 128, 128) for nb in batches], dev, concat=4)
     m = _vq(arch.VQ_F4_NOATTN, dev)
-    m.encode(torch.rand(1, 3, 512, 512, generator=g, device=dev) * 2 - 1)
-    m.decode(torch.randn(1, 3, 128, 128, generator=g, device=dev))
+    return (eps, m.encode(torch.rand(1, 3, 512, 512, generator=g, device=dev) * 2 - 1),
+            m.decode(torch.randn(1, 3, 128, 128, generator=g, device=dev)))
 
 
 def _wl_bsr(dev):
     g = torch.Generator(device=dev).manual_seed(3)
-    _run_unet(arch.BSR_SR_UNET, [(1, 6, 128, 128)], dev, concat=3)
-    _vq(arch.VQ_F4, dev).decode(torch.randn(1, 3, 64, 96, generator=g, device=dev))
+    return (_run_unet(arch.BSR_SR_UNET, [(1, 6, 128, 128)], dev, concat=3),
+            _vq(arch.VQ_F4, dev).decode(torch.randn(1, 3, 64, 96, generator=g, device=dev)))
 
 
 def _wl_bsr_tiled(dev):
     """The UNet at a tiled sampling batch of 9 and the tiled decode's tile batch: a 192² latent, 2 x 2 tiles of 128²."""
     g = torch.Generator(device=dev).manual_seed(3)
-    _run_unet(arch.BSR_SR_UNET, [(9, 6, 128, 128)], dev, concat=3)
+    eps = _run_unet(arch.BSR_SR_UNET, [(9, 6, 128, 128)], dev, concat=3)
     vq = _vq(arch.VQ_F4, dev)
     q = vq.post_quant(torch.randn(1, 3, 192, 192, generator=g, device=dev))
     tiles, _ = ops.nchw_to_nhwc(ops.patch_unfold(ops.nhwc_to_nchw(q), (128, 128), (64, 64)))
-    vq._decoder(tiles)
+    return eps, vq._decoder(tiles)
 
 
 def _wl_vq_sr_tile(dev):
     g = torch.Generator(device=dev).manual_seed(6)
-    _vq(arch.VQ_F4, dev).decode(torch.randn(1, 3, 128, 128, generator=g, device=dev))
+    return _vq(arch.VQ_F4, dev).decode(torch.randn(1, 3, 128, 128, generator=g, device=dev))
 
 
 def _wl_clip_image_tower(dev):
     """The ViT-L/14 tower from patch rows at B = 1, 64 and 256 images (M = 256 B patch rows, 257 B token rows)."""
     e = _clip_image_embedder(arch.CLIP_VISION_PROJ, dev)
     g = torch.Generator(device=dev).manual_seed(0)
-    for B in (1, 64, 256):
-        e.embed_patches(torch.randn(B * 256, e.W["kpad"], generator=g, device=dev).half(), B)
+    return [e.embed_patches(torch.randn(B * 256, e.W["kpad"], generator=g, device=dev).half(), B) for B in (1, 64, 256)]
 
 
 def _wl_tiny(dev):
     g = torch.Generator(device=dev).manual_seed(4)
-    _run_unet(arch.TINY_UNET, [(2, 4, 16, 16), (1, 4, 16, 24)], dev, ctx=(77, 64))
-    _run_unet(arch.TINY_ATTN_UNET, [(2, 4, 16, 16)], dev)
-    _run_unet(arch.TINY_LAION_UNET, [(2, 4, 16, 16)], dev, ctx=(77, 128))
-    _run_unet(arch.TINY_RDM_UNET, [(2, 16, 16, 16)], dev, ctx=(3, 64))
+    out = [_run_unet(arch.TINY_UNET, [(2, 4, 16, 16), (1, 4, 16, 24)], dev, ctx=(77, 64)),
+           _run_unet(arch.TINY_ATTN_UNET, [(2, 4, 16, 16)], dev),
+           _run_unet(arch.TINY_LAION_UNET, [(2, 4, 16, 16)], dev, ctx=(77, 128)),
+           _run_unet(arch.TINY_RDM_UNET, [(2, 16, 16, 16)], dev, ctx=(3, 64))]
     vae = _vae(arch.TINY_VAE, dev)
-    vae.decode(torch.randn(1, 4, 8, 8, generator=g, device=dev))
-    vae.encode(torch.rand(1, 3, 64, 64, generator=g, device=dev) * 2 - 1)
-    _vae(arch.TINY_KL_F16, dev).decode(torch.randn(1, 16, 4, 4, generator=g, device=dev))
-    _vq(arch.TINY_VQ, dev).decode(torch.randn(1, 3, 8, 8, generator=g, device=dev))
-    _vq(arch.TINY_VQ_F8, dev).decode(torch.randn(1, 4, 8, 8, generator=g, device=dev))
-    _clip(arch.TINY_CLIP, dev, _ids(1000, 2, dev))
-    _clip(arch.TINY_CLIP_TEXT_PROJ, dev, _ids(1000, 2, dev))
-    _bert(arch.TINY_BERT, dev, _ids(1000, 2, dev))
-    _clip_image(arch.TINY_CLIP_VISION_PROJ, dev, 2)
+    out.append(vae.decode(torch.randn(1, 4, 8, 8, generator=g, device=dev)))
+    out.append(vae.encode(torch.rand(1, 3, 64, 64, generator=g, device=dev) * 2 - 1))
+    out.append(_vae(arch.TINY_KL_F16, dev).decode(torch.randn(1, 16, 4, 4, generator=g, device=dev)))
+    out.append(_vq(arch.TINY_VQ, dev).decode(torch.randn(1, 3, 8, 8, generator=g, device=dev)))
+    out.append(_vq(arch.TINY_VQ_F8, dev).decode(torch.randn(1, 4, 8, 8, generator=g, device=dev)))
+    out.append(_clip(arch.TINY_CLIP, dev, _ids(1000, 2, dev)))
+    out.append(_clip(arch.TINY_CLIP_TEXT_PROJ, dev, _ids(1000, 2, dev)))
+    out.append(_bert(arch.TINY_BERT, dev, _ids(1000, 2, dev)))
+    out.append(_clip_image(arch.TINY_CLIP_VISION_PROJ, dev, 2))
+    return out
 
 
 # the norm sweep
@@ -201,24 +203,24 @@ def _wl_cin256_class_embedder(dev):
     cfg = arch.CIN256_V2_COND
     emb = sdb200.ClassEmbedder(**cfg).load_weights(_sd(arch.class_embedder_param_shapes, cfg, 15, dev), dev)
     c = emb({cfg["key"]: torch.arange(cfg["n_classes"], device=dev).flip(0)})
-    _unet(arch.CIN256_V2_UNET, dev).context_kv(c)
+    return c, _unet(arch.CIN256_V2_UNET, dev).context_kv(c)
 
 
 def _wl_sdv1_vae_sample(dev):
     """SD-v1 VAE encode with a posterior sample (vae_sample) at 512² and 512x768."""
     g = torch.Generator(device=dev).manual_seed(7)
     vae = _vae(arch.SD_V1_VAE, dev)
-    for h, w in ((512, 512), (512, 768)):
-        vae.encode(torch.rand(1, 3, h, w, generator=g, device=dev) * 2 - 1).sample(
+    return [vae.encode(torch.rand(1, 3, h, w, generator=g, device=dev) * 2 - 1).sample(
             noise=torch.randn(1, 4, h // 8, w // 8, generator=g, device=dev), scale=0.18215)
+            for h, w in ((512, 512), (512, 768))]
 
 
 def _wl_sdv1_decode_uint8(dev):
     """SD-v1 decodes to uint8 images as the txt2img / img2img pipelines return them: 2 x 512² and 1 x 512x768."""
     g = torch.Generator(device=dev).manual_seed(8)
     vae = _vae(arch.SD_V1_VAE, dev)
-    for s in ((2, 4, 64, 64), (1, 4, 64, 96)):
-        ops.to_uint8(vae.decode(torch.randn(*s, generator=g, device=dev), scale=1 / 0.18215, nhwc=True))
+    return [ops.to_uint8(vae.decode(torch.randn(*s, generator=g, device=dev), scale=1 / 0.18215, nhwc=True))
+            for s in ((2, 4, 64, 64), (1, 4, 64, 96))]
 
 
 # the elementwise sweep: what a plain forward of the tables above does not reach
