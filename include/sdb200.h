@@ -368,8 +368,9 @@ int sdb_axpby(const float* x, float a, float b, int64_t n, float* out, sdb_strea
 /* out = a*x + b*y (DDIMSampler.stochastic_encode, ddim.py:206-220; q_sample, ddpm.py:274-277) */
 int sdb_axpby2(const float* x, const float* y, float a, float b, int64_t n, float* out, sdb_stream_t stream);
 
-/* 1x1 conv with <= 32 channels in fp32 (post_quant_conv 4->4 with the 1/scale_factor folded in as alpha,
- * quant_conv 8->8, KL-f16's 32->32; autoencoder.py:302-303,326,331): out[p, j] = sum_c (alpha x[p, c]) w[j, c] + b[j] */
+/* 1x1 conv with <= 128 channels in and out, fp32 (post_quant_conv 4->4 with the 1/scale_factor folded in as alpha,
+ * quant_conv 8->8, KL-f16's 32->32, KL-f32's 128->128 and 64->64; autoencoder.py:302-303,326,331):
+ * out[p, j] = sum_c (alpha x[p, c]) w[j, c] + b[j] */
 int sdb_pointwise_small(const float* x, int64_t npix, int32_t cin, int32_t cout, const float* w, const float* b,
                         float alpha, float* out, sdb_stream_t stream);
 /* CLIP token + position embedding gather (transformers CLIPTextEmbeddings): ids int64 [rows] -> fp32 [rows, dim] */

@@ -17,7 +17,7 @@ from .safety import StableDiffusionSafetyChecker  # noqa: E402,F401
 from .samplers import DDIMSampler, DPMSolverSampler, PLMSSampler  # noqa: E402,F401
 from .unet import UNetModel  # noqa: E402,F401
 from .vae import AutoencoderKL  # noqa: E402,F401
-from .vq import VQModelInterface  # noqa: E402,F401
+from .vq import VQModel, VQModelInterface  # noqa: E402,F401
 
 
 def _alias_submodules():

@@ -165,6 +165,29 @@ TINY_KL_F16 = dict(embed_dim=16, ddconfig=dict(double_z=True, z_channels=16, res
                                                ch=64, ch_mult=[1, 1, 2, 2, 8], num_res_blocks=1,
                                                attn_resolutions=[16, 4], dropout=0.0))
 TINY_CLIP_TEXT_PROJ = dict(TINY_CLIP, projection_dim=64)
+# the standalone first stages of models/first_stage_models/*/config.yaml that no LDM uses: KL-f4 (3 latent channels),
+# KL-f32 (64 latent channels, six levels, AttnBlocks at 16x16 and 8x8, 1x1 latent heads 128 -> 128 and 64 -> 64),
+# VQ-f8-n256 (VQ-f8 with 256 codes) and VQ-f16 (16384 codes of width 8, five levels, AttnBlocks at 16x16)
+KL_F4 = dict(embed_dim=3, ddconfig=dict(double_z=True, z_channels=3, resolution=256, in_channels=3, out_ch=3, ch=128,
+                                        ch_mult=[1, 2, 4], num_res_blocks=2, attn_resolutions=[], dropout=0.0))
+KL_F32 = dict(embed_dim=64, ddconfig=dict(double_z=True, z_channels=64, resolution=256, in_channels=3, out_ch=3, ch=128,
+                                          ch_mult=[1, 1, 2, 2, 4, 4], num_res_blocks=2, attn_resolutions=[16, 8],
+                                          dropout=0.0))
+VQ_F8_N256 = dict(VQ_F8, n_embed=256)
+VQ_F16 = dict(embed_dim=8, n_embed=16384, ddconfig=dict(double_z=False, z_channels=8, resolution=256, in_channels=3,
+                                                         out_ch=3, ch=128, ch_mult=[1, 1, 2, 2, 4], num_res_blocks=2,
+                                                         attn_resolutions=[16], dropout=0.0))
+# small members for tests with the same level structure: KL-f32's six levels with level attention at 16x16 (128 wide)
+# and 8x8 (256 wide) and the 128 -> 128 quant_conv; VQ-f16's five levels, attention at 16x16 and codes of width 8
+FIRST_STAGES = {"kl-f4": KL_F4, "kl-f8": SD_V1_VAE, "kl-f16": KL_F16, "kl-f32": KL_F32, "vq-f4": VQ_F4,
+                "vq-f4-noattn": VQ_F4_NOATTN, "vq-f8": VQ_F8, "vq-f8-n256": VQ_F8_N256, "vq-f16": VQ_F16}
+TINY_KL_F4 = dict(embed_dim=3, ddconfig={**TINY_VQ_F4["ddconfig"], "double_z": True})
+TINY_KL_F32 = dict(embed_dim=64, ddconfig=dict(double_z=True, z_channels=64, resolution=128, in_channels=3, out_ch=3,
+                                               ch=64, ch_mult=[1, 1, 2, 2, 4, 4], num_res_blocks=1,
+                                               attn_resolutions=[16, 8], dropout=0.0))
+TINY_VQ_F16 = dict(embed_dim=8, n_embed=512, ddconfig=dict(double_z=False, z_channels=8, resolution=64, in_channels=3,
+                                                            out_ch=3, ch=64, ch_mult=[1, 1, 2, 2, 4], num_res_blocks=1,
+                                                            attn_resolutions=[16], dropout=0.0))
 # FrozenClipImageEmbedder (the retriever that embeds RDM databases): the CLIP ViT-L/14 vision tower with the visual
 # projection (transformers CLIPModel's visual_projection); the tiny member's 64-wide embeddings match TINY_RDM_UNET
 CLIP_VISION_PROJ = dict(hidden_size=1024, intermediate_size=4096, num_hidden_layers=24, num_attention_heads=16,

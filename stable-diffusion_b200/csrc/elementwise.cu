@@ -250,7 +250,10 @@ __global__ void axpby_kernel(const float* __restrict__ x, float a, float b, size
   GRID_STRIDE(i, n) out[i] = a * x[i] + b;
 }
 
-// per-pixel small channel mix (1x1 conv with <= 8 channels, fp32): out[p, j] = alpha * sum_c x[p, c] w[j, c] + b[j]
+// per-pixel channel mix (1x1 conv with <= 128 channels in and out, fp32): out[p, j] = alpha * sum_c x[p, c] w[j, c] + b[j]
+// as one fmaf chain over c in order, alpha * x rounded once per term, then + b[j]. Every width takes this one path: the
+// widest head (KL-f32's 128 -> 128 quant_conv) runs on a latent of a few thousand pixels, where one thread per output
+// reading its weight row from L1 costs microseconds.
 __global__ void pointwise_small_kernel(const float* __restrict__ x, size_t npix, int cin, int cout,
                                        const float* __restrict__ w, const float* __restrict__ b, float alpha,
                                        float* __restrict__ out) {
@@ -474,7 +477,7 @@ extern "C" int sdb_axpby(const float* x, float a, float b, int64_t n, float* out
 extern "C" int sdb_pointwise_small(const float* x, int64_t npix, int32_t cin, int32_t cout, const float* w,
                                    const float* b, float alpha, float* out, sdb_stream_t stream) {
   SDB_REC(sdb_pointwise_small(x, npix, cin, cout, w, b, alpha, out, s_));
-  SDB_CHECK(x && w && out && cin > 0 && cin <= 32 && cout > 0 && cout <= 32,"sdb_pointwise_small: bad arguments");
+  SDB_CHECK(x && w && out && cin > 0 && cin <= 128 && cout > 0 && cout <= 128,"sdb_pointwise_small: bad arguments");
   pointwise_small_kernel<<<grid_for(static_cast<size_t>(npix) * cout), 256, 0, ST>>>(
       x, static_cast<size_t>(npix), cin, cout, w, b, alpha, out);
   SDB_LAUNCH_CHECK();

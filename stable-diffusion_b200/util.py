@@ -28,6 +28,7 @@ TARGET_MAP = {
     "ldm.modules.diffusionmodules.openaimodel.UNetModel": "sdb200.unet.UNetModel",
     "ldm.models.autoencoder.AutoencoderKL": "sdb200.vae.AutoencoderKL",
     "ldm.models.autoencoder.VQModelInterface": "sdb200.vq.VQModelInterface",
+    "ldm.models.autoencoder.VQModel": "sdb200.vq.VQModel",
     "ldm.modules.encoders.modules.FrozenCLIPEmbedder": "sdb200.clip.FrozenCLIPEmbedder",
     "ldm.modules.encoders.modules.FrozenCLIPTextEmbedder": "sdb200.clip.FrozenCLIPTextEmbedder",
     "ldm.modules.encoders.modules.FrozenClipImageEmbedder": "sdb200.clip_image.FrozenClipImageEmbedder",

@@ -2,9 +2,10 @@
 (`encode(x) -> posterior`, `decode(z) -> image`; autoencoder.py:285-333) over the VAE Encoder/Decoder of
 ldm/modules/diffusionmodules/model.py:368-568. State-dict keys unchanged (`encoder.*`, `decoder.*`, `quant_conv.*`,
 `post_quant_conv.*`). Same kernels as the UNet: wgmma implicit-GEMM convs, fp32 GroupNorm (eps 1e-6) + SiLU
-producing the fp16 operand, fp32 residual stream. Any latent width the 1x1 quant convs take (<= 16: SD-v1's 4,
-KL-f16's 16) and AttnBlocks inside the levels at ddconfig.attn_resolutions (KL-f16: at 16x16) run; posterior sampling
-is for 4 latent channels. The single-head mid-block attention (c=512, N=h*w;
+producing the fp16 operand, fp32 residual stream. Any latent width the 1x1 quant convs take (<= 64: KL-f4's 3,
+SD-v1's 4, KL-f16's 16, KL-f32's 64) and AttnBlocks inside the levels at ddconfig.attn_resolutions (KL-f16: at 16x16;
+KL-f32: at 16x16 and 8x8) run; posterior sampling is for 4 latent channels (sdb_vae_sample), so forward() of any other
+width needs sample_posterior=False (the posterior mode). The single-head mid-block attention (c=512, N=h*w;
 model.py:178-202) runs in the d = 512 flash kernel (sdb_attention, dpad 512; other widths: QK^T GEMM -> fp32 row softmax -> PV GEMM per image), with the value bias folded through proj_out (softmax rows sum to 1).
 """
 from __future__ import annotations
@@ -55,9 +56,9 @@ class DiagonalGaussianDistribution:
 
 class ConvAutoencoder(PackedStage):
     """The Encoder / Decoder of model.py:368-568 (attention in the mid block, and inside the levels at attn_resolutions)
-    and the weight packing shared by the first stages: AutoencoderKL below and VQModelInterface (vq.py). Both have a
-    quant_conv and a post_quant_conv (1x1, <= 16 channels, fp32), packed here; a subclass sets `shapes` and packs
-    anything else it has (the codebook)."""
+    and the weight packing shared by the first stages: AutoencoderKL below and VQModel / VQModelInterface (vq.py). All
+    have a quant_conv and a post_quant_conv (1x1, <= 128 channels in and out, fp32: sdb_pointwise_small), packed here; a
+    subclass sets `shapes` and packs anything else it has (the codebook)."""
 
     drop_prefixes = ("loss.",)   # the training loss's tensors
 
@@ -212,7 +213,8 @@ class ConvAutoencoder(PackedStage):
     def _decoder(self, h):
         """Decoder.forward (model.py:535-568) on the fp32 NHWC output of post_quant_conv; returns fp32 NHWC."""
         D = self.W["decoder"]
-        h = self._conv3(D["conv_in"], x32=h)
+        # a latent of 64 channels (KL-f32) takes the implicit GEMM, which reads the fp16 operand
+        h = self._conv3(D["conv_in"], x32=h) if D["conv_in"]["col"] else self._conv3(D["conv_in"], x16=ops.cast_f16(h))
         h = self._resnet(D["mid1"], h)
         if D["attn"] is not None:
             h = self._attn(D["attn"], h)
