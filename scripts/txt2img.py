@@ -11,8 +11,22 @@ StableDiffusionSafetyChecker state dict, .safetensors or tensors-only pickle) - 
 
 --laion400m switches to the LAION-400M model as the reference does (configs/latent-diffusion/txt2img-1p4B-eval.yaml,
 models/ldm/text2img-large/model.ckpt, outputs/txt2img-samples-laion400m): BERT-conditioned UNet, same KL-f8 first stage.
-Its prompts are tokenised with the uncased WordPiece vocabulary of --bert_vocab (or the locally cached bert-base-uncased
-files); without one, seeded stand-in ids [CLS] r... [SEP] [PAD]... are used and the empty prompt is [CLS] [SEP] [PAD]...
+
+Any text-conditional LDM config runs through --config, e.g. the LDM-VQ-4 text-to-image model (BERT-640 text encoder,
+VQ-f4 first stage, 64x64x3 latent):
+
+  python scripts/txt2img.py --config models/ldm/text2img256/config.yaml --ckpt models/ldm/text2img256/model.ckpt \
+      --H 256 --W 256 --C 3 --f 4 --scale 5.0 --plms --prompt "a virus monster is playing guitar, oil on canvas"
+
+The tokenizer follows the cond stage's class. A FrozenCLIPEmbedder uses the CLIP BPE (--clip_vocab); without it,
+seeded CLIP stand-in ids are used. A BERTEmbedder uses the uncased WordPiece vocabulary of --bert_vocab (or the locally
+cached bert-base-uncased files); without one, seeded stand-in ids [CLS] r... [SEP] [PAD]... are used and the empty
+prompt is [CLS] [SEP] [PAD].... --random_init builds the model --config names with seeded weights; the built-in SD-v1
+and LAION values are used only when the reference's default path of either config is absent. --C and --f must match
+the model (the UNet's in_channels and the first stage's downsampling factor). The script samples the raw weights, also
+for a config with use_ema: a checkpoint's model_ema.* set is loaded, and model.ema_scope() switches to it, but the
+sampling loop here does not enter that scope (the reference script does, so its samples of such a checkpoint come from
+the EMA weights).
 """
 import argparse
 import os
@@ -25,6 +39,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import sdb200  # noqa: E402
 from sdb200 import pipeline  # noqa: E402
+from sdb200.util import instantiate_from_config, remap_config  # noqa: E402
 from sdb200.safety import StableDiffusionSafetyChecker, WatermarkEncoder, put_watermark  # noqa: E402
 
 DEFAULT_CONFIG = "configs/stable-diffusion/v1-inference.yaml"
@@ -47,7 +62,8 @@ def apply_laion400m(opt):
 def load_model_from_config(config, ckpt, device, verbose=False, random_init=False, unsafe_ckpt=False):
     """scripts/txt2img.py:49-66 via sdb200.checkpoint (pickled .ckpt or .safetensors, reference YAML or built-in values
     of v1-inference.yaml / txt2img-1p4B-eval.yaml when the reference's default path of either is absent). Seeded random
-    weights are used only on request (--random_init): a missing checkpoint or config path is an error."""
+    weights are used only on request (--random_init), for the model the config names: a missing checkpoint or config
+    path is an error."""
     laion = config == LAION_CONFIG
     if config and not os.path.exists(config):
         if config not in (DEFAULT_CONFIG, LAION_CONFIG):
@@ -55,7 +71,10 @@ def load_model_from_config(config, ckpt, device, verbose=False, random_init=Fals
         config = None                         # the reference's default path is absent here: built-in values
     if random_init:
         print("--random_init: seeded random-init weights (images will be noise-like)")
-        model = pipeline.build_laion_model() if laion else pipeline.build_model()
+        if config:
+            model = instantiate_from_config(remap_config(sdb200.checkpoint.load_config(config)))
+        else:
+            model = pipeline.build_laion_model() if laion else pipeline.build_model()
         pipeline.load_random_weights(model, device, gen_device=device)
         return model.eval()
     if not ckpt or not os.path.exists(ckpt):
@@ -73,12 +92,13 @@ def synthetic_ids(n, seed, device):
     return ids.to(device)
 
 
-def synthetic_bert_ids(n, seed, device):
-    """Stand-in bert-base-uncased ids: [CLS], 19 seeded word-piece ids (999 .. 30521), [SEP], [PAD]..."""
+def synthetic_bert_ids(n, seed, device, vocab_size=30522):
+    """Stand-in bert-base-uncased ids: [CLS], 19 seeded word-piece ids (999 .. vocab_size - 1; 103 .. for a vocabulary
+    of at most 2000 rows), [SEP], [PAD]..."""
     g = torch.Generator().manual_seed(seed)
     ids = torch.full((n, 77), BERT_PAD, dtype=torch.long)
     ids[:, 0] = BERT_CLS
-    ids[:, 1:20] = torch.randint(999, 30522, (n, 19), generator=g)
+    ids[:, 1:20] = torch.randint(999 if vocab_size > 2000 else 103, vocab_size, (n, 19), generator=g)
     ids[:, 20] = BERT_SEP
     return ids.to(device)
 
@@ -90,7 +110,36 @@ def bert_uncond_ids(n, device):
     return ids.to(device)
 
 
-def main():
+def text_encoder_kind(model):
+    """"bert" or "clip" from the class of the model's cond stage; a model that is not text-conditional is an error."""
+    enc = model.cond_stage_model
+    if isinstance(enc, sdb200.BERTEmbedder):
+        return "bert"
+    if isinstance(enc, sdb200.FrozenCLIPEmbedder):
+        return "clip"
+    raise SystemExit(f"error: the cond stage {type(enc).__name__} is not a text encoder (BERTEmbedder or "
+                     "FrozenCLIPEmbedder); txt2img samples text-conditional models only")
+
+
+def stand_in_ids(kind, enc, n, seed, device):
+    """Seeded (prompt ids, empty-prompt ids) for the cond stage when no tokenizer vocabulary is available."""
+    if kind == "bert":
+        return synthetic_bert_ids(n, seed, device, enc.cfg["vocab_size"]), bert_uncond_ids(n, device)
+    un = torch.full((n, 77), 49407, dtype=torch.long, device=device)
+    un[:, 0] = 49406
+    return synthetic_ids(n, seed, device), un
+
+
+def check_latent_shape(model, C, f):
+    """--C must be the UNet's in_channels and --f the first stage's downsampling factor 2 ** (len(ch_mult) - 1)."""
+    want_c = model.model.diffusion_model.in_channels
+    want_f = 2 ** (len(model.first_stage_model.cfg["ddconfig"]["ch_mult"]) - 1)
+    if (C, f) != (want_c, want_f):
+        raise SystemExit(f"error: --C {C} --f {f} do not match the model: pass --C {want_c} --f {want_f} (the UNet's "
+                         f"in_channels and the first stage's downsampling factor)")
+
+
+def main(argv=None):
     p = argparse.ArgumentParser()
     p.add_argument("--prompt", type=str, nargs="?", default="a painting of a virus monster playing guitar")
     p.add_argument("--outdir", type=str, nargs="?", default="outputs/txt2img-samples")
@@ -120,15 +169,18 @@ def main():
     p.add_argument("--clip_vocab", type=str, default=None,
                    help="directory with the CLIP vocab.json + merges.txt (host-side BPE); default: transformers' local cache")
     p.add_argument("--bert_vocab", type=str, default=None,
-                   help="directory with the bert-base-uncased vocab.txt (--laion400m); default: the local Hugging Face cache")
+                   help="directory with the bert-base-uncased vocab.txt (any BERTEmbedder cond stage); default: the "
+                        "local Hugging Face cache")
     p.add_argument("--token_seed", type=int, default=1234, help="seed of the stand-in token ids (no tokenizer offline)")
     p.add_argument("--safety_ckpt", type=str, default=None,
                    help="state dict of diffusers' StableDiffusionSafetyChecker: flagged images are blanked (txt2img.py:88-95)")
     p.add_argument("--no_watermark", action="store_true", help="do not embed the invisible watermark (txt2img.py:261-264)")
-    opt = apply_laion400m(p.parse_args())
+    opt = apply_laion400m(p.parse_args(argv))
     torch.manual_seed(opt.seed)           # seed_everything (txt2img.py:243)
     device = torch.device("cuda")
     model = load_model_from_config(opt.config, opt.ckpt, device, random_init=opt.random_init, unsafe_ckpt=opt.unsafe_ckpt)
+    kind = text_encoder_kind(model)
+    check_latent_shape(model, opt.C, opt.f)
     sampler = "dpm_solver" if opt.dpm_solver else ("plms" if opt.plms else "ddim")
     pipe = pipeline.Txt2Img(model, sampler=sampler, steps=opt.ddim_steps, scale=opt.scale,
                             height=opt.H, width=opt.W, eta=opt.ddim_eta, f=opt.f, channels=opt.C)
@@ -153,9 +205,9 @@ def main():
     else:
         prompts = [opt.prompt]
     enc = model.cond_stage_model
-    if opt.clip_vocab and not opt.laion400m:
+    if opt.clip_vocab and kind == "clip":
         enc.version, enc.tokenizer = opt.clip_vocab, None
-    if opt.bert_vocab and opt.laion400m:
+    if opt.bert_vocab and kind == "bert":
         enc.vocab_dir, enc.tokenizer = opt.bert_vocab, None
     start_code = torch.randn([B, opt.C, opt.H // opt.f, opt.W // opt.f], device=device) if opt.fixed_code else None
     base_count = len(os.listdir(sample_path))
@@ -169,12 +221,7 @@ def main():
             except RuntimeError as e:
                 if n == 0 and pi == 0:
                     print(f"tokenizer unavailable ({e}); using seeded token ids")
-                if opt.laion400m:
-                    ids, un = synthetic_bert_ids(B, opt.token_seed + pi, device), bert_uncond_ids(B, device)
-                else:
-                    ids = synthetic_ids(B, opt.token_seed + pi, device)
-                    un = torch.full((B, 77), 49407, dtype=torch.long, device=device)
-                    un[:, 0] = 49406
+                ids, un = stand_in_ids(kind, enc, B, opt.token_seed + pi, device)
             x_T = start_code if start_code is not None else torch.randn(
                 [B, opt.C, opt.H // opt.f, opt.W // opt.f], device=device)      # plms.py:124
             if safety_checker is not None:       # check_safety on the fp32 image, then 255 * x -> uint8 (txt2img.py:317-322)
@@ -196,6 +243,7 @@ def main():
     toc = time.time()
     print(f"Your samples are ready and waiting for you here: \n{opt.outdir} \n"
           f"{n_img} images in {toc - tic:.2f} s ({n_img / (toc - tic):.2f} images/s). Enjoy.")
+    return opt.outdir
 
 
 if __name__ == "__main__":

@@ -144,6 +144,18 @@ LAION_BERT = dict(n_embed=1280, n_layer=32, vocab_size=30522, max_seq_len=77)
 # small members for tests: the attention's inner width stays 8 x 64 = 512
 TINY_BERT = dict(n_embed=128, n_layer=2, vocab_size=1000, max_seq_len=77)
 TINY_LAION_UNET = dict(TINY_UNET, context_dim=128)
+# the text-conditional LDM-VQ-4 (models/ldm/text2img256/config.yaml): a 64x64x3 latent, spatial transformers with heads
+# of num_head_channels 32 (12 / 18 / 30 heads at widths 384 / 576 / 960, 32² / 16² / 8² tokens) cross-attending to a
+# 77-token BERTEmbedder(n_embed=640, n_layer=32) context; the VQ-f4 first stage (VQ_F4)
+TEXT2IMG256_UNET = dict(image_size=64, in_channels=3, out_channels=3, model_channels=192, attention_resolutions=[8, 4, 2],
+                        num_res_blocks=2, channel_mult=[1, 2, 3, 5], num_head_channels=32, use_spatial_transformer=True,
+                        transformer_depth=1, context_dim=640)
+TEXT2IMG256_BERT = dict(n_embed=640, n_layer=32, vocab_size=30522, max_seq_len=77)
+# a small member for tests: 4 / 6 heads of d = 32 at two levels and in the middle block, on TINY_BERT's 128-wide
+# context; first stage TINY_VQ_F4
+TINY_TEXT2IMG256_UNET = dict(image_size=16, in_channels=3, out_channels=3, model_channels=64, attention_resolutions=[2, 4],
+                             num_res_blocks=1, channel_mult=[1, 2, 3], num_head_channels=32, use_spatial_transformer=True,
+                             transformer_depth=1, context_dim=128)
 # the retrieval-augmented diffusion model (configs/retrieval-augmented-diffusion/768x768.yaml, scripts/knn2img.py): a
 # 48x48x16 latent, spatial transformers with heads of num_head_channels 32 (14 / 28 / 42 heads at widths 448 / 896 /
 # 1344, 56 in the middle block) cross-attending to CLIP ViT-L/14's projected text embedding and its retrieved
