@@ -28,7 +28,19 @@ References and bounds (u = 2^-24, the fp32 unit roundoff):
   linear_small  |out - ref| <= LS_REL (|x| |W|^T + |b|) (x 1.2 under SiLU) + ACT_REL |v|: fp32 FMA chains of K
                 terms in 8-wide pieces and a 32-lane shuffle tree stay far below K u, so 1e-5 bounds K <= 6400
                 with margin; __expf / the division inside SiLU are ACT_REL. The fp16 output adds half an fp16 ulp.
-  pointwise     |out - ref| <= LS_REL (|alpha| |x| |W|^T + |b|) (cin <= 32 FMAs after one rounding of alpha x).
+  pointwise     |out - ref| <= LS_REL (|alpha| |x| |W|^T + |b|): one rounding of alpha x per term, a chain of cin <= 128
+                FMAs and the bias add stay below (cin + 2) u = 7.8e-6 relative to that sum.
+  vq_quantize   z_q bit-exact against the fp32 restatement zv = fl(scale z), then fl(zv + fl(e[idx] - zv)). The index:
+                the kernel compares d(j) = fl(fl(zz + q_j) - 2 dot_j) over codes j, where zz sums the D rounded squares
+                fl(zv_k^2) with rounded adds (error <= D u sum zv^2), dot_j is an fma chain of length D (<= D u
+                sum |zv e_j|, doubled exactly), q_j = code_sq is the fp64 sum of e_j^2 rounded once (<= u sum e_j^2),
+                and the add and the subtract round once each (<= u (zz + q_j) and u |d|). With A_j = sum (|zv| +
+                |e_j|)^2 >= sum zv^2 + sum e_j^2 + 2 sum |zv e_j|, every piece fits in (D + 2) u A_j, and (D + 3) u A_j
+                covers the second-order terms. The kernel's choice beats the fp64 argmin j* in its own arithmetic, so
+                d64(idx) - d64(j*) <= VQ_REL(D) (A_idx + A_j*), VQ_REL(D) = (D + 3) u, with d64 the fp64 distance from
+                zv. Bit-identical codes have bit-identical distances, so idx is never a code with an identical twin of
+                lower index (the lowest index wins a tie, as torch.argmin). Without indices, z_q equals that of the
+                same launch with them.
   timestep      the frequency exp(-ln(P) j / half) is formed from three fp32 roundings of an exponent of magnitude
                 e_j = ln(P) j / half and one expf (2 ulp): relative error <= (3 e_j + 3) u; the product t f adds u;
                 cosf / sinf add 2 ulp of a value <= 1. So |out - ref| <= u ((3 e_j + 4) |t f| + TS_ABS) with
@@ -64,6 +76,11 @@ VS_REL = 8 * U
 LS_ROWS = 8                        # linear_small: samples per pass
 LS_SMEM_FLOATS = 200 * 1024 // 4   # linear_small: activations of one pass in shared memory
 FILL_U8 = (0x5A, 0xA5)             # the two fills of a uint8 output: equal results mean every byte was written
+FILL_I64 = (-7, -9)                # the two fills of an int64 output (it has no NaN): code indices are never negative
+FILLS = {torch.uint8: FILL_U8, torch.int64: FILL_I64}
+VQ_CHUNK = 1024                    # vq_quantize: codes per shared-memory chunk
+VQ_THREADS = 256                   # vq_quantize: latent pixels per block
+PW_NARROW = 32                     # pointwise_small: the widest head before KL-f32 (SD-v1's VAE: 8 -> 8, 4 -> 4)
 ACT_SILU = _l.ACT_SILU
 
 
@@ -160,12 +177,19 @@ def _axpby_sig(x, a, b=0.0, out=None):
     return dict(op="axpby", n=x.numel(), a=float(a), b=float(b), ax=eoff(x), ao=_ao(out))
 
 
+def _vq_quantize_sig(z, codebook, code_sq, scale=1.0, want_indices=False):
+    n_e, e_dim = codebook.shape
+    # z_q and the indices are allocated by ops.vq_quantize: offset 0
+    return dict(op="vq_quantize", m=z.numel() // e_dim, e_dim=e_dim, n_e=n_e, scale=float(scale),
+                idx=bool(want_indices), az=eoff(z), aq=0, ae=eoff(codebook), asq=eoff(code_sq))
+
+
 SIGS = {"nchw_to_nhwc": _nchw_to_nhwc_sig, "nhwc_to_nchw": _nhwc_to_nchw_sig, "transpose_f16": _transpose_f16_sig,
         "im2col3x3": _im2col3x3_sig, "upsample2x": _upsample2x_sig, "resample_f32": _resample_f32_sig,
         "cast_f16": _cast_f16_sig, "timestep_embedding_f32": _timestep_embedding_f32_sig,
         "embed_tokens": _embed_tokens_sig, "vit_embed": _vit_embed_sig, "rows_gather": _rows_gather_sig,
         "rows_pool": _rows_pool_sig, "linear_small": _linear_small_sig, "pointwise_small": _pointwise_small_sig,
-        "vae_sample": _vae_sample_sig, "to_uint8": _to_uint8_sig, "axpby": _axpby_sig}
+        "vae_sample": _vae_sample_sig, "to_uint8": _to_uint8_sig, "axpby": _axpby_sig, "vq_quantize": _vq_quantize_sig}
 
 
 def label(p):
@@ -227,6 +251,18 @@ def classes(p, sms):
         cls |= {k for k, on in (("pool:ids", p["ids"]), ("pool:normalize", p["normalize"])) if on}
     elif op == "nchw_to_nhwc":
         cls.add("nhwc:" + ("both" if p["f32"] and p["f16"] else "f32" if p["f32"] else "f16"))
+    elif op == "pointwise_small":
+        cls |= {k for k, on in (("pw:wide_in", p["cin"] > PW_NARROW), ("pw:wide_out", p["cout"] > PW_NARROW)) if on}
+    elif op == "vq_quantize":
+        cls.add(f"vq:e{p['e_dim']}")
+        if p["n_e"] > VQ_CHUNK:
+            cls.add("vq:multi_chunk")
+            if p["n_e"] % VQ_CHUNK:
+                cls.add("vq:partial_chunk")      # a last chunk shorter than the full ones before it
+        if p["m"] % VQ_THREADS:
+            cls.add("vq:tail_block")             # a block with threads past the last pixel
+        if not p["idx"]:
+            cls.add("vq:no_indices")
     return cls
 
 
@@ -236,8 +272,9 @@ GRID_STRIDE_OPS = ("im2col3x3", "upsample2x", "resample_f32", "cast_f16", "silu_
 REQUIRED = ({"ls:one_pass", "ls:passes", "ls:partial_u", "ls:n_tail", "ls:bias", "ls:silu", "ls:f16",
              "im2col:s1p1", "im2col:s2p0", "im2col:s2p1", "resample:1", "resample:2", "pool:ids", "pool:normalize",
              "nhwc:f32", "nhwc:f16", "nhwc:both", "nhwc_to_nchw", "transpose_f16", "timestep_embedding_f32",
-             "rows_pool", "to_uint8", "silu_f16", "timestep_embedding"}
-            | {f"wrap:{op}" for op in GRID_STRIDE_OPS})
+             "rows_pool", "to_uint8", "silu_f16", "timestep_embedding", "pw:wide_in", "pw:wide_out",
+             "vq:multi_chunk", "vq:partial_chunk", "vq:tail_block", "vq:no_indices"}
+            | {f"vq:e{d}" for d in range(1, 9)} | {f"wrap:{op}" for op in GRID_STRIDE_OPS})
 COVER = defaultdict(int)
 
 
@@ -252,7 +289,7 @@ def _inp(values, off, fill=NAN):
 
 
 class Out:
-    """An output view at element offset `off` inside GUARD fill elements on both sides (NaN; uint8: FILL_U8)."""
+    """An output view at element offset `off` inside GUARD fill elements on both sides (NaN; uint8 and int64: FILLS)."""
 
     def __init__(self, shape, dtype, dev, off=0):
         n = math.prod(shape)
@@ -261,11 +298,11 @@ class Out:
         self.lo, self.n = GUARD + off, n
 
     def fill(self, k):
-        self.buf.fill_(FILL_U8[k] if self.buf.dtype == torch.uint8 else NAN)
+        self.buf.fill_(FILLS[self.buf.dtype][k] if self.buf.dtype in FILLS else NAN)
 
     def guards_ok(self, k):
         out = torch.cat([self.buf[:self.lo], self.buf[self.lo + self.n:]])
-        return bool((out == FILL_U8[k]).all()) if out.dtype == torch.uint8 else bool(out.isnan().all())
+        return bool((out == FILLS[out.dtype][k]).all()) if out.dtype in FILLS else bool(out.isnan().all())
 
 
 def _bits(t):
@@ -777,7 +814,70 @@ def run_mask_blend(p, g, dev):
     return {"exact": _eq(res["img"].cpu(), ref), "exact_dup": _eq(res["img2"].cpu(), ref)}, same, guards
 
 
-RUN = {k[4:]: v for k, v in globals().items() if k.startswith("run_")}
+def vq_operands(p, g):
+    """(z, codebook, zv = fl(scale z)) of a vq_quantize problem on g's device: zv and the codes N(0, 1), with two
+    planted decisions. Code n_e - 1 equals zv of row 0 (distance 0; when n_e % 1024 == 1 it is the only code of the
+    last chunk). When n_e > 1025 and m > 1, codes 1023 and 1024 both equal zv of row m - 1: an exact tie across a chunk
+    boundary, which the lower index must win."""
+    m, n_e = p["m"], p["n_e"]
+    s = f32(p["scale"]).to(g.device)
+    z = _randn((m, p["e_dim"]), g) / s
+    zv = z * s
+    cb = _randn((n_e, p["e_dim"]), g)
+    cb[n_e - 1] = zv[0]
+    if n_e > VQ_CHUNK + 1 and m > 1:
+        cb[VQ_CHUNK - 1] = zv[m - 1]
+        cb[VQ_CHUNK] = zv[m - 1]
+    return z, cb, zv
+
+
+def vq_check(zv, cb, idx, zq):
+    """The vq_quantize checks of the module docstring for the indices idx and the output zq of zv = fl(scale z)."""
+    m, D = zv.shape
+    n_e = cb.shape[0]
+    r = {"idx_range": bool(((idx >= 0) & (idx < n_e)).all())}
+    if not r["idx_range"]:
+        return r
+    r["exact_zq"] = _eq(zq, zv + (cb[idx] - zv))
+    zd, ed = zv.double(), cb.double()
+    e2 = (ed * ed).sum(1)
+    best = torch.empty(m, dtype=torch.int64, device=zv.device)     # the fp64 argmin, in chunks of <= 2^25 distances
+    step = max(1, (1 << 25) // n_e)
+    for r0 in range(0, m, step):
+        zc = zd[r0:r0 + step]
+        best[r0:r0 + step] = ((zc * zc).sum(1, keepdim=True) + e2[None] - 2 * zc @ ed.t()).argmin(1)
+    dist = lambda j: ((zd - ed[j]) ** 2).sum(1)
+    amag = lambda j: ((zd.abs() + ed[j].abs()) ** 2).sum(1)
+    r["vq_decision"] = _share((dist(idx) - dist(best)).clamp_min(0), (D + 3) * U * (amag(idx) + amag(best)))
+    _, inv = torch.unique(cb, dim=0, return_inverse=True)
+    first = torch.full((int(inv.max()) + 1,), n_e, device=cb.device).scatter_reduce(
+        0, inv, torch.arange(n_e, device=cb.device), "amin")                 # lowest index of each distinct code
+    r["lowest_of_equal"] = bool((first[inv[idx]] == idx).all())
+    return r
+
+
+def run_vq_quantize(p, g, dev):
+    m, D, n_e = p["m"], p["e_dim"], p["n_e"]
+    z, cb, zv = vq_operands(p, g)
+    z, cb = _inp(z, p["az"]), _inp(cb, p["ae"])
+    code_sq = _inp((cb.double() ** 2).sum(1).float(), p["asq"])                # as VQModel.pack_weights
+    outs = {"zq": Out((m, D), torch.float32, dev, p["aq"])}
+    if p["idx"]:
+        outs["idx"] = Out((m,), torch.int64, dev)
+    launch = lambda zq, idx: L().sdb_vq_quantize(P(z), m, D, p["scale"], P(cb), P(code_sq), n_e, P(zq), P(idx), S())
+    res, same, guards = launch2(outs, lambda: launch(outs["zq"].v, outs["idx"].v if p["idx"] else None),
+                                "sdb_vq_quantize")
+    if p["idx"]:
+        return vq_check(zv, cb, res["idx"], res["zq"]), same, guards
+    zq, idx = torch.empty_like(zv), torch.empty(m, dtype=torch.int64, device=dev)   # the same launch with indices
+    _l.check(launch(zq, idx), "sdb_vq_quantize")
+    torch.cuda.synchronize()
+    r = vq_check(zv, cb, idx, zq)
+    r["same_as_indexed"] = _eq(res["zq"], zq)
+    return r, same, guards
+
+
+RUN ={k[4:]: v for k, v in globals().items() if k.startswith("run_")}
 
 
 # ------------------------------------------------------------------------------------------------ the sweep
@@ -845,7 +945,8 @@ def _p(op, **kw):
             "embed_tokens": dict(ai=0, at=0, ap=0), "vit_embed": dict(ax=0, ac=0, ap=0), "rows_gather": dict(ax=0),
             "rows_pool": dict(ax=0), "linear_small": dict(bias=True, act=0, f16=False, ax=0, aw=0, ab=0, ao=0),
             "pointwise_small": dict(alpha=1.0, bias=True, ax=0, aw=0, ab=0), "vae_sample": dict(ax=0, an=0),
-            "to_uint8": dict(ax=0), "axpby": dict(ax=0, ao=0)}.get(op, {})
+            "to_uint8": dict(ax=0), "axpby": dict(ax=0, ao=0),
+            "vq_quantize": dict(scale=1.0, idx=True, az=0, aq=0, ae=0, asq=0)}.get(op, {})
     return dict(dict(op=op, **base), **kw)
 
 
@@ -910,6 +1011,28 @@ def edge_grid():
     ps += [_p("rows_pool", b=3, n_ctx=1, dim=64, ids=True, normalize=False)]
     ps += [_p("rows_gather", rows=5, stride=257, dim=1024, xrows=4 * 257 + 1), _p("vit_embed", nb=3, np=7, dim=12)]
     ps += [_p("to_uint8", n=3 * 17 * 13), _p("axpby", n=1000, a=1.0, b=0.0, ax=1, ao=3)]
+    # the wide 1x1 heads (KL-f32: 128 -> 128, 64 -> 64): past 32 channels in, out or both, with and without bias
+    for cin in (33, 64, 127, 128):
+        for cout in (33, 64, 127, 128):
+            for bias in (True, False):
+                ps.append(_p("pointwise_small", npix=257, cin=cin, cout=cout, bias=bias,
+                             alpha=1 / 0.18215 if bias else -0.5, ax=cin % 4, aw=cout % 4, ab=1))
+    ps += [_p("pointwise_small", npix=300, cin=4, cout=128), _p("pointwise_small", npix=300, cin=128, cout=3,
+                                                                bias=False, alpha=1.3)]
+    return ps
+
+
+def vq_grid():
+    """vq_quantize at every compiled e_dim; codebooks of one code, of one chunk, one code short of and past a chunk
+    (1025: a last chunk of one code), two chunks and one code (2049) and VQ-f16's 16384; 1 pixel, one short of a block,
+    one block (VQ-f16's 16² latent) and one past it; indices on and off; scale 1 and not; operands off 16-byte
+    boundaries. vq_operands plants a code at distance 0 and, past 1025 codes, an exact tie across a chunk boundary."""
+    ps = []
+    for D in range(1, 9):
+        for n_e in (1, 256, 1023, 1024, 1025, 2049, 16384):
+            for m, idx in ((1, True), (255, True), (256, True), (257, True), (257, False)):
+                ps.append(_p("vq_quantize", m=m, e_dim=D, n_e=n_e, scale=1.0 if (m + D) % 2 else 1.3, idx=idx,
+                             az=D % 4, aq=m % 4, ae=n_e % 4, asq=(m + D) % 4))
     return ps
 
 
@@ -917,7 +1040,7 @@ def edge_grid():
 @pytest.mark.timeout(600)
 def test_elementwise_synthetic_grid(cuda_dev):
     sms = _l.load().sdb_sm_count()
-    run_sweep(wrap_grid(sms) + edge_grid(), "synthetic")
+    run_sweep(wrap_grid(sms) + edge_grid() + vq_grid(), "synthetic")
 
 
 @pytest.mark.gpu
@@ -1014,7 +1137,7 @@ ENTRY_POINT_TESTS = {
     "sdb_softmax_rows": ("test_norm_sweep_gpu.py",),
     "sdb_resample_f32": (HERE, "test_uncond_ldm_gpu.py"),
     "sdb_ddpm_step": (HERE, "test_uncond_ldm_gpu.py"),
-    "sdb_vq_quantize": ("test_vq_ldm_gpu.py",),
+    "sdb_vq_quantize": (HERE, "test_vq_ldm_gpu.py"),
     "sdb_nchw_to_nhwc": (HERE,),
     "sdb_nhwc_to_nchw": (HERE,),
     "sdb_im2col3x3": (HERE,),
@@ -1154,6 +1277,50 @@ def test_signatures_and_classes_cpu():
         assert work_items(q) > cap, q
     assert {f"wrap:{q['op']}" for q in wrap_grid(132)} == {f"wrap:{op}" for op in GRID_STRIDE_OPS}
     assert set(RUN) >= {q["op"] for q in wrap_grid(132) + edge_grid()} and set(RUN) >= set(SIGS)
+
+
+def test_vq_and_pointwise_signatures_and_classes_cpu():
+    book = torch.zeros(16384, 8)
+    p = _vq_quantize_sig(torch.zeros(1, 16, 16, 8), book, torch.zeros(16384), scale=1.3, want_indices=True)
+    assert (p["m"], p["e_dim"], p["n_e"], p["scale"], p["idx"]) == (256, 8, 16384, 1.3, True)
+    assert classes(p, 132) == {"vq_quantize", "vq:e8", "vq:multi_chunk"}               # VQ-f16 at 256²
+    assert signature(p) != signature(_vq_quantize_sig(torch.zeros(1, 16, 16, 8), book, torch.zeros(16384), 1.3))
+    q = _vq_quantize_sig(torch.zeros(2, 8, 12, 4), torch.zeros(256, 4), torch.zeros(256))
+    assert classes(q, 132) == {"vq_quantize", "vq:e4", "vq:tail_block", "vq:no_indices"}  # VQ-f8-n256, 64x96, batch 2
+    assert "vq:partial_chunk" in classes(_p("vq_quantize", m=1, e_dim=1, n_e=1025), 132)
+    assert not classes(_p("vq_quantize", m=256, e_dim=3, n_e=1023), 132) & {"vq:partial_chunk", "vq:multi_chunk"}
+    w = _pointwise_small_sig(torch.zeros(2, 4, 4, 128), torch.zeros(128, 128), torch.zeros(128), alpha=1.3)
+    assert (w["npix"], w["cin"], w["cout"], w["alpha"]) == (32, 128, 128, 1.3)
+    assert classes(w, 132) >= {"pw:wide_in", "pw:wide_out"}
+    assert classes(_pointwise_small_sig(torch.zeros(10, 32), torch.zeros(32, 32)), 132) == {"pointwise_small"}
+    assert classes(_p("pointwise_small", npix=9, cin=4, cout=64), 132) == {"pointwise_small", "pw:wide_out"}
+    grid = {c for q in edge_grid() + vq_grid() for c in classes(q, 132)}
+    assert {c for c in REQUIRED if c.startswith(("vq:", "pw:"))} <= grid
+    assert {c for c in REQUIRED if c.startswith(("vq:", "pw:"))} == {f"vq:e{d}" for d in range(1, 9)} | {
+        "vq:multi_chunk", "vq:partial_chunk", "vq:tail_block", "vq:no_indices", "pw:wide_in", "pw:wide_out"}
+
+
+@pytest.mark.parametrize("n_e", [1025, 2049])
+def test_vq_checks_cpu(n_e):
+    """vq_check passes the fp64 nearest codes (lowest index first) and fails each value mutant of the kernel: the
+    highest index of a tie, the last partial chunk skipped, z_q = e without the straight-through rounding, and
+    distances from the unscaled z."""
+    z, cb, zv = vq_operands(_p("vq_quantize", m=257, e_dim=3, n_e=n_e, scale=1.3), torch.Generator().manual_seed(5))
+    nearest = lambda x, codes: torch.cdist(x.double(), codes.double()).argmin(1)       # the first of equal minima
+    st = lambda i: zv + (cb[i] - zv)
+    idx = nearest(zv, cb)
+    assert int(idx[0]) == n_e - 1 and (n_e < 2049 or int(idx[-1]) == VQ_CHUNK - 1)
+    ok = vq_check(zv, cb, idx, st(idx))
+    assert ok["idx_range"] and ok["exact_zq"] and ok["lowest_of_equal"] and ok["vq_decision"] == 0.0
+    if n_e == 2049:
+        tie = torch.where(idx == VQ_CHUNK - 1, VQ_CHUNK, idx)
+        assert not vq_check(zv, cb, tie, st(tie))["lowest_of_equal"]
+    skip = nearest(zv, cb[:(n_e - 1) // VQ_CHUNK * VQ_CHUNK])
+    assert vq_check(zv, cb, skip, st(skip))["vq_decision"] > 1
+    assert not vq_check(zv, cb, idx, cb[idx])["exact_zq"]
+    unscaled = nearest(z, cb)
+    assert vq_check(zv, cb, unscaled, st(unscaled))["vq_decision"] > 1
+    assert not vq_check(zv, cb, torch.full_like(idx, FILL_I64[0]), zv)["idx_range"]
 
 
 def test_clip_check_ids_cpu():

@@ -17,7 +17,7 @@ import test_gemm_plans_gpu as GP
 from helpers import golden, rel_l2
 from sweeps import record
 from test_text2img256_cpu import _script, tiny_node, tiny_state_dict
-from workloads import _bert, _ids, _run_unet
+from workloads import _run_unet, text2img256
 from sdb200 import arch
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(1800)]
@@ -194,19 +194,13 @@ def test_txt2img_script_full_size_random_init(cuda_dev, tmp_path):
 
 
 # ------------------------------------------------------------------------------------------------ kernel sweeps
-def _gemm_workload(dev):
-    """BERT-640 on the cond + uncond ids of a batch of 3 (6 x 77 tokens), then the UNet at the guidance batches 2 and 8.
-    Kept here rather than in workloads.py's shared tables, whose sweeps run every model they list."""
-    return (_bert(arch.TEXT2IMG256_BERT, dev, _ids(30522, 6, dev)),
-            _run_unet(arch.TEXT2IMG256_UNET, [(2, 3, 64, 64), (8, 3, 64, 64)], dev, ctx=(77, 640)))
-
-
 def test_every_plan_of_every_text2img256_gemm_problem(cuda_dev):
-    """BERT-640 on the cond + uncond ids of a batch of 3 (6 x 77 tokens: the K / V projections of K = 640 and the
-    8 x 64 attention's 512-wide inner dimension), then the UNet at the guidance batches 2 and 8."""
-    problems = GP.catalogue(_gemm_workload, cuda_dev)
-    print(f"\ntext2img256 BERT (6 x 77 tokens) + UNet (2 and 8, 3, 64²), context (77, 640): {len(problems)} distinct GEMM "
-          "problems")
+    """workloads.text2img256: BERT-640 on the cond + uncond ids of a batch of 3 (6 x 77 tokens: the K / V projections
+    of K = 640 and the 8 x 64 attention's 512-wide inner dimension), the UNet at the guidance batches 2 and 8, and the
+    VQ-f4 decode of a 64² latent. Its norm and elementwise launches are swept in test_first_stage_sweep_gpu.py."""
+    problems = GP.catalogue(text2img256, cuda_dev)
+    print(f"\ntext2img256 BERT (6 x 77 tokens) + UNet (2 and 8, 3, 64²), context (77, 640) + VQ-f4 decode (64²): "
+          f"{len(problems)} distinct GEMM problems")
     assert any(p["chans"] == (640,) for p in problems)
     GP.run_sweep(problems, cuda_dev, "text2img256")
     torch.cuda.empty_cache()

@@ -1,8 +1,9 @@
 """One eager forward of each model with random weights: the workloads whose kernel launches the sweeps record
-(test_norm_sweep_gpu.py, test_attention_sweep_gpu.py, test_elementwise_sweep_gpu.py, test_gemm_plans_gpu.py and the
-GEMM plan sweeps in the model test files). Each table maps a name to a function of the device; a problem's operands are seeded by its index in the
-recorded list, so an entry's shapes and call order are part of what a sweep checks. Each function returns what it
-computes (tensors, possibly nested in lists and tuples), which test_pdl_order_gpu.py digests bit for bit."""
+(test_norm_sweep_gpu.py, test_attention_sweep_gpu.py, test_elementwise_sweep_gpu.py, test_gemm_plans_gpu.py, all four
+over the first stages in test_first_stage_sweep_gpu.py, and the GEMM plan sweeps in the model test files). Each table
+maps a name to a function of the device; a problem's operands are seeded by its index in the recorded list, so an
+entry's shapes and call order are part of what a sweep checks. Each function returns what it computes (tensors,
+possibly nested in lists and tuples), which test_pdl_order_gpu.py digests bit for bit."""
 import torch
 
 import helpers  # noqa: F401  (puts the repository on sys.path)
@@ -146,6 +147,15 @@ def _wl_vq_sr_tile(dev):
     return _vq(arch.VQ_F4, dev).decode(torch.randn(1, 3, 128, 128, generator=g, device=dev))
 
 
+def text2img256(dev):
+    """text2img256: BERT-640 on the cond + uncond ids of a batch of 3 (6 x 77 tokens), the UNet at the guidance batches
+    2 and 8, and one VQ-f4 decode of a 64² latent (the model's scale_factor is 1)."""
+    g = torch.Generator(device=dev).manual_seed(2)
+    return (_bert(arch.TEXT2IMG256_BERT, dev, _ids(30522, 6, dev)),
+            _run_unet(arch.TEXT2IMG256_UNET, [(2, 3, 64, 64), (8, 3, 64, 64)], dev, ctx=(77, 640)),
+            _vq(arch.VQ_F4, dev).decode(torch.randn(1, 3, 64, 64, generator=g, device=dev)))
+
+
 def _wl_clip_image_tower(dev):
     """The ViT-L/14 tower from patch rows at B = 1, 64 and 256 images (M = 256 B patch rows, 257 B token rows)."""
     e = _clip_image_embedder(arch.CLIP_VISION_PROJ, dev)
@@ -253,3 +263,43 @@ GEMM_MODEL_WORKLOADS = {
     "bsr_sr": _wl_bsr_tiled,
     "semantic": lambda dev: _run_unet(arch.SEMANTIC_SYNTHESIS_UNET, [(8, 6, 64, 64), (1, 6, 128, 128)], dev, concat=3),
 }
+
+# test_first_stage_sweep_gpu.py: every first stage of arch.FIRST_STAGES, kept out of the tables above so that their
+# sweeps and the PDL digest child (pdl_child.ALL) do not grow
+DECODE_SCALE = 1.3     # decode(z, scale): not 1, so the quantizer and the 1x1 head see a scale
+
+
+def first_stage_geometries(f):
+    """(batch, height, width) of the images a first stage of factor f runs: 256² (the configs' training size); 256x384
+    at batch 2 (non-square, batch strides; every level attention of the nine configs has a token count divisible by 8
+    there, e.g. KL-f32 at 16x24 and 8x12); and the thin f x 8f, whose 1 x 8 latent makes the last stride-2 conv run
+    2 x 16 -> 1 x 8 with pad (0, 1, 0, 1), the mid attention run at 8 tokens and the last GroupNorms at 8 pixels."""
+    return ((1, 256, 256), (2, 256, 384), (1, f, 8 * f))
+
+
+def _wl_first_stage(cfg, dev):
+    """At each geometry: encode (the posterior's mode for KL, VQModel.encode with indices for VQ), decode of a seeded
+    latent at DECODE_SCALE (VQModelInterface.decode, which re-quantizes at that scale) and, for VQ, decode_code of the
+    indices the encode chose."""
+    import sdb200
+    f = 2 ** (len(cfg["ddconfig"]["ch_mult"]) - 1)
+    g = torch.Generator(device=dev).manual_seed(9)
+    if "n_embed" in cfg:
+        sd = _sd(arch.vq_param_shapes, cfg, 12, dev)
+        vq, vqi = sdb200.VQModel(**cfg).load_weights(sd, dev), sdb200.VQModelInterface(**cfg).load_weights(sd, dev)
+    else:
+        kl = _vae(cfg, dev)
+    outs = []
+    for nb, h, w in first_stage_geometries(f):
+        x = torch.rand(nb, 3, h, w, generator=g, device=dev) * 2 - 1
+        z = torch.randn(nb, cfg["embed_dim"], h // f, w // f, generator=g, device=dev)
+        if "n_embed" in cfg:
+            quant, loss, (_, _, idx) = vq.encode(x)
+            outs += [quant, loss, idx, vqi.decode(z, scale=DECODE_SCALE), vq.decode_code(idx.view(nb, h // f, w // f))]
+        else:
+            outs += [kl.encode(x).mode(), kl.decode(z, scale=DECODE_SCALE)]
+    return outs
+
+
+FIRST_STAGE_WORKLOADS = {name: (lambda cfg: lambda dev: _wl_first_stage(cfg, dev))(cfg)
+                         for name, cfg in arch.FIRST_STAGES.items()}
