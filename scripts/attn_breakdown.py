@@ -6,7 +6,6 @@ plus the QK and V^T projection GEMMs (the two GEMMs right before each self-atten
 usage: python scripts/attn_breakdown.py [reps]"""
 import collections
 import statistics
-import subprocess
 import sys
 
 import torch
@@ -14,13 +13,13 @@ import torch
 sys.path.insert(0, ".")
 import sdb200
 from sdb200 import arch, ops
+from measure import card
 
 dev = torch.device("cuda:0")
 REPS = int(sys.argv[1]) if len(sys.argv) > 1 else 7
-q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                   capture_output=True, text=True).stdout.strip().splitlines()[0]
-print("GPU:", q)
-clk = float(q.split(",")[-1].split()[0]) * 1e6
+gpu = card()
+print("GPU:", ", ".join(gpu.values()))
+clk = float(gpu["max_sm_clock"].split()[0]) * 1e6
 sms = torch.cuda.get_device_properties(dev).multi_processor_count
 net = sdb200.UNetModel(**arch.SD_V1_UNET).load_weights(
     arch.random_state_dict(arch.unet_param_shapes(arch.SD_V1_UNET), 11, device=dev), dev)

@@ -9,10 +9,8 @@ network and first stage.
   python scripts/bench_celebahq.py --batches 3 --out outputs/celebahq.json
 """
 import argparse
-import json
 import os
 import sys
-import time
 
 import torch
 
@@ -21,7 +19,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from sdb200 import arch, ops  # noqa: E402
 from sdb200.samplers import DDIMSampler  # noqa: E402
 from sdb200.util import instantiate_from_config, remap_config  # noqa: E402
-from bench_lsun import gpu_info  # noqa: E402
+from measure import card, emit, event_ms, wall_s  # noqa: E402
 
 
 def padded_gemm_share(u, x, t):
@@ -70,47 +68,22 @@ def main():
     torch.manual_seed(0)
     one_batch()                       # warm-up: autotune, graph capture, first stage
     torch.cuda.synchronize()
-    times = []
-    for _ in range(a.batches):
-        t0 = time.perf_counter()
-        img = one_batch()
-        torch.cuda.synchronize()
-        times.append(time.perf_counter() - t0)
+    times, img = wall_s(one_batch, a.batches)
     assert img.shape == (a.batch_size, 3, 256, 256) and bool(torch.isfinite(img).all())
     x = torch.randn(shape, device=dev)
     t = torch.full((a.batch_size,), 501.0, device=dev)
-    for _ in range(5):
-        u(x, t)
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    n = 50
-    e0.record()
-    for _ in range(n):
-        u(x, t)
-    e1.record()
-    e1.synchronize()
-    unet_ms = e0.elapsed_time(e1) / n
+    unet_ms = event_ms(lambda: u(x, t), 50, warmup=5)
     # first stage alone: decode of one batch of latents
     z = torch.randn(shape, device=dev)
-    m.decode_first_stage(z)
-    e0.record()
-    for _ in range(3):
-        m.decode_first_stage(z)
-    e1.record()
-    e1.synchronize()
-    dec_ms = e0.elapsed_time(e1) / 3
+    dec_ms = event_ms(lambda: m.decode_first_stage(z), 3, warmup=1)
     u.use_cuda_graph = False
     padded_ms, gemm_ms = padded_gemm_share(u, x, t)
     res = dict(workload=f"CelebA-HQ VQ-f4 LDM 256x256 DDIM-{a.steps} eta={a.eta} batch {a.batch_size} (random weights), "
                         "sampling + decode_first_stage",
                images_per_s=a.batch_size / min(times), batch_s=times, unet_eval_ms=unet_ms, decode_ms=dec_ms,
                eager_gemm_ms=gemm_ms, eager_padded_k_gemm_ms=padded_ms, padded_k_share_of_unet_eval=padded_ms / unet_ms,
-               **gpu_info())
-    line = json.dumps(res)
-    print(line)
-    if a.out:
-        os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
-        with open(a.out, "w") as f:
-            f.write(line + "\n")
+               **card())
+    emit(res, a.out)
 
 
 if __name__ == "__main__":

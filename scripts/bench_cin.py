@@ -12,18 +12,16 @@ name and power limit read in the same run.
   python scripts/bench_cin.py --model cin256 --repeats 3 --out outputs/cin256.json
 """
 import argparse
-import json
 import os
 import statistics
 import sys
-import time
 
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from sdb200 import ops  # noqa: E402
-from bench_lsun import gpu_info  # noqa: E402
+from measure import card, emit, event_ms, wall_s  # noqa: E402
 
 
 def attention_launches(u, x, t, c, reps=5):
@@ -31,13 +29,8 @@ def attention_launches(u, x, t, c, reps=5):
     runs, totals = [], []
     for _ in range(reps):
         ops.PROFILE = []
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        u(x, t, context=c)
-        e1.record()
-        torch.cuda.synchronize()
+        totals.append(event_ms(lambda: u(x, t, context=c), 1))
         runs.append(ops.PROFILE)
-        totals.append(e0.elapsed_time(e1))
     ops.PROFILE = None
     out = []
     for i, (kind, fl, _, _, shp) in enumerate(runs[0]):
@@ -63,28 +56,14 @@ def main():
     torch.manual_seed(0)
     S.sample_classes(m, classes, n, ddim_steps=a.steps, scale=scale)   # warm-up: autotune, graph capture, first stage
     torch.cuda.synchronize()
-    times = []
-    for _ in range(a.repeats):
-        t0 = time.perf_counter()
-        img = S.sample_classes(m, classes, n, ddim_steps=a.steps, scale=scale)
-        torch.cuda.synchronize()
-        times.append(time.perf_counter() - t0)
+    times, img = wall_s(lambda: S.sample_classes(m, classes, n, ddim_steps=a.steps, scale=scale), a.repeats)
     assert img.shape == (len(classes) * n, 3, 256, 256) and bool(torch.isfinite(img).all())
     labels = n * [1000] + n * [25] if scale != 1.0 else n * [25]
     nb = len(labels)
     x = torch.randn(nb, u.in_channels, u.image_size, u.image_size, device=dev)
     t = torch.full((nb,), 501.0, device=dev)
     c = m.get_learned_conditioning({"class_label": torch.tensor(labels, device=dev)})
-    for _ in range(5):
-        u(x, t, context=c)
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    reps = 50
-    e0.record()
-    for _ in range(reps):
-        u(x, t, context=c)
-    e1.record()
-    e1.synchronize()
-    unet_ms = e0.elapsed_time(e1) / reps
+    unet_ms = event_ms(lambda: u(x, t, context=c), 50, warmup=5)
     u.use_cuda_graph = False
     launches, eager_ms = attention_launches(u, x, t, c)
     attn_us = sum(r[5] for r in launches)
@@ -98,13 +77,8 @@ def main():
                         f"{shp}), decode_first_stage, random weights",
                images_per_s=len(classes) * n / min(times), run_s=times, unet_eval_ms_graph=unet_ms,
                unet_eval_ms_eager_profiled=eager_ms, attention_us_eager=attn_us,
-               attention_share_of_eager_eval=attn_us / 1e3 / eager_ms, attention_launches=rows, **gpu_info())
-    line = json.dumps(res)
-    print(line)
-    if a.out:
-        os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
-        with open(a.out, "w") as f:
-            f.write(line + "\n")
+               attention_share_of_eager_eval=attn_us / 1e3 / eager_ms, attention_launches=rows, **card())
+    emit(res, a.out)
 
 
 if __name__ == "__main__":

@@ -11,7 +11,6 @@ Prints one JSON line with the card name and power limit read in the same run; --
   python scripts/bench_clip_image.py --out outputs/clip_image.json
 """
 import argparse
-import json
 import os
 import sys
 
@@ -22,7 +21,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import sdb200  # noqa: E402
 from sdb200 import arch  # noqa: E402
 from sdb200.clip_image import _table  # noqa: E402
-from bench_lsun import gpu_info  # noqa: E402
+from measure import card, emit, event_ms  # noqa: E402
 
 
 def tower_flops(cfg):
@@ -33,16 +32,6 @@ def tower_flops(cfg):
     n = g2 + 1
     per_layer = 2 * n * h * (2 * h) + 2 * n * h * h + 4 * n * n * h + 2 * n * h * h + 2 * n * h * inter * 2
     return 2 * g2 * (3 * P * P) * h + L * per_layer + 2 * h * cfg["projection_dim"]
-
-
-def timed(fn, reps):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    e1.synchronize()
-    return e0.elapsed_time(e1) / reps
 
 
 def main():
@@ -58,19 +47,14 @@ def main():
     emb.load_weights(arch.random_state_dict(emb.shapes, 16, device=dev), dev)
     flops = tower_flops(cfg)
     S, P, kpad = cfg["image_size"], cfg["patch_size"], emb.W["kpad"]
-    res = dict(bench="clip_image", **gpu_info(), side=opt.side, gflop_per_image=round(flops / 1e9, 2), runs=[])
+    res = dict(bench="clip_image", **card(), side=opt.side, gflop_per_image=round(flops / 1e9, 2), runs=[])
     g = torch.Generator(device=dev).manual_seed(0)
     for B in opt.batches:
         flat = torch.randint(0, 256, (B * opt.side * opt.side * 3,), dtype=torch.uint8, device=dev, generator=g)
         hw = [(opt.side, opt.side)] * B
         table = _table(hw, 3, flat.numel()).to(dev)
-        for _ in range(2):
-            emb.encode_packed(flat, hw)
-        torch.cuda.synchronize()
-        ms = timed(lambda: emb.encode_packed(flat, hw), opt.reps)
-        pre = lambda: emb.preprocess_patches(flat, table)
-        pre()
-        pre_ms = timed(pre, 5 * opt.reps)
+        ms = event_ms(lambda: emb.encode_packed(flat, hw), opt.reps, warmup=2)
+        pre_ms = event_ms(lambda: emb.preprocess_patches(flat, table), 5 * opt.reps, warmup=1)
         bytes_img = opt.side * opt.side * 3 + (S // P) ** 2 * kpad * 2
         run = dict(batch=B, ms_per_batch=round(ms, 2), images_per_s=round(B / (ms * 1e-3), 1),
                    tflop_per_s=round(B * flops / (ms * 1e-3) / 1e12, 1),
@@ -84,12 +68,7 @@ def main():
               file=sys.stderr)
         del flat
         torch.cuda.empty_cache()
-    line = json.dumps(res)
-    print(line)
-    if opt.out:
-        os.makedirs(os.path.dirname(os.path.abspath(opt.out)), exist_ok=True)
-        with open(opt.out, "w") as f:
-            f.write(line + "\n")
+    emit(res, opt.out)
 
 
 if __name__ == "__main__":

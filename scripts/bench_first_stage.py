@@ -11,7 +11,6 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import torch
@@ -19,27 +18,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import sdb200  # noqa: E402
 from sdb200 import arch  # noqa: E402
-
-
-def card():
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                              capture_output=True, text=True, check=True).stdout.strip().splitlines()[0]
-    except (OSError, subprocess.CalledProcessError, IndexError):
-        return torch.cuda.get_device_name() + ", power limit unknown"
-
-
-def timed(fn, iters, warmup):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(iters):
-        fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) / 1e3 / iters
+from measure import card, event_ms  # noqa: E402
 
 
 def main(argv=None):
@@ -52,7 +31,8 @@ def main(argv=None):
     opt = p.parse_args(argv)
     assert torch.cuda.is_available(), "bench_first_stage needs a CUDA device"
     dev = torch.device("cuda")
-    print(f"# {card()}", flush=True)
+    c = card()
+    print(f"# {c['gpu']}, {c['power_limit']}", flush=True)
     x = torch.randn(opt.batch, 3, opt.size, opt.size, generator=torch.Generator().manual_seed(0)).clamp(-1, 1).to(dev)
     for name in opt.only or sorted(arch.FIRST_STAGES):
         cfg = arch.FIRST_STAGES[name]
@@ -66,7 +46,7 @@ def main(argv=None):
             model.load_weights(arch.random_state_dict(model.shapes, 7, device=dev), dev)
             mean = model.encode(x).mean
             enc, dec = (lambda: model.encode(x).parameters), (lambda: model.decode(mean))
-        te, td = timed(enc, opt.iters, opt.warmup), timed(dec, opt.iters, opt.warmup)
+        te, td = (event_ms(fn, opt.iters, opt.warmup) / 1e3 for fn in (enc, dec))
         print(json.dumps({"config": name, "batch": opt.batch, "size": opt.size, "encode_img_s": round(opt.batch / te, 1),
                           "decode_img_s": round(opt.batch / td, 1), "encode_ms": round(te * 1e3, 2),
                           "decode_ms": round(td * 1e3, 2)}), flush=True)

@@ -9,28 +9,16 @@ same run.
   python scripts/bench_laion.py --repeats 3 --out outputs/laion.json
 """
 import argparse
-import json
 import os
 import sys
-import time
 
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from sdb200 import pipeline  # noqa: E402
-from bench_lsun import gpu_info  # noqa: E402
+from measure import card, emit, event_ms, wall_s  # noqa: E402
 from txt2img import bert_uncond_ids, synthetic_bert_ids  # noqa: E402
-
-
-def event_ms(fn, reps):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    e1.synchronize()
-    return e0.elapsed_time(e1) / reps
 
 
 def main():
@@ -54,34 +42,20 @@ def main():
         x_T = torch.randn(B, 4, 64, 64, generator=g, device=dev)
         img = pipe(ids, un, x_T=x_T)                            # warm-up: autotune, graph capture, first stage
         torch.cuda.synchronize()
-        times = []
-        for _ in range(a.repeats):
-            t0 = time.perf_counter()
-            img = pipe(ids, un, x_T=x_T)
-            torch.cuda.synchronize()
-            times.append(time.perf_counter() - t0)
+        times, img = wall_s(lambda: pipe(ids, un, x_T=x_T), a.repeats)
         assert img.shape == (B, 512, 512, 3)
         both = torch.cat([un, ids])
         c = model.get_learned_conditioning(both)
         x = torch.randn(2 * B, 4, 64, 64, generator=g, device=dev)
         t = torch.full((2 * B,), 501.0, device=dev)
-        for _ in range(5):
-            u(x, t, context=c)
-        unet_ms = event_ms(lambda: u(x, t, context=c), 50)
-        for _ in range(3):
-            enc.encode(both)
-        bert_ms = event_ms(lambda: enc.encode(both), 20)
+        unet_ms = event_ms(lambda: u(x, t, context=c), 50, warmup=5)
+        bert_ms = event_ms(lambda: enc.encode(both), 20, warmup=3)
         res[f"b{B}"] = dict(images_per_s=B / min(times), run_s=times, unet_eval_ms_graph=unet_ms,
                             unet_batch=2 * B, bert_encode_ms=bert_ms, bert_tokens=tuple(both.shape))
         print(f"batch {B}: {B / min(times):.3f} images/s, UNet eval (batch {2 * B}) {unet_ms:.2f} ms, "
               f"BERT encode {tuple(both.shape)} {bert_ms:.2f} ms", file=sys.stderr)
-    res.update(gpu_info())
-    line = json.dumps(res)
-    print(line)
-    if a.out:
-        os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
-        with open(a.out, "w") as f:
-            f.write(line + "\n")
+    res.update(card())
+    emit(res, a.out)
 
 
 if __name__ == "__main__":

@@ -6,11 +6,8 @@ Prints one JSON line with the card name and power limit read in the same run.
   python scripts/bench_lsun.py --batches 3 --out outputs/lsun.json
 """
 import argparse
-import json
 import os
-import subprocess
 import sys
-import time
 
 import torch
 
@@ -18,16 +15,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from sdb200 import arch  # noqa: E402
 from sdb200.samplers import DDIMSampler  # noqa: E402
 from sdb200.util import instantiate_from_config, remap_config  # noqa: E402
-
-
-def gpu_info():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power, clk = [v.strip() for v in q.split(",")]
-        return dict(gpu=name, power_limit=power, max_sm_clock=clk)
-    except Exception as e:  # noqa: BLE001
-        return dict(gpu=torch.cuda.get_device_name(), power_limit=f"unknown ({e})")
+from measure import card, emit, event_ms, wall_s  # noqa: E402
 
 
 def main():
@@ -59,35 +47,16 @@ def main():
     torch.manual_seed(0)
     one_batch()                       # warm-up: autotune, graph capture, VAE
     torch.cuda.synchronize()
-    times = []
-    for _ in range(a.batches):
-        t0 = time.perf_counter()
-        img = one_batch()
-        torch.cuda.synchronize()
-        times.append(time.perf_counter() - t0)
+    times, img = wall_s(one_batch, a.batches)
     assert img.shape == (a.batch_size, 3, 256, 256) and bool(torch.isfinite(img).all())
     # one UNet evaluation (graph replay) by CUDA events over many launches
     x = torch.randn(shape, device=dev)
     t = torch.full((a.batch_size,), 501.0, device=dev)
-    for _ in range(5):
-        u(x, t)
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    n = 50
-    e0.record()
-    for _ in range(n):
-        u(x, t)
-    e1.record()
-    e1.synchronize()
+    unet_ms = event_ms(lambda: u(x, t), 50, warmup=5)
     res = dict(workload=f"LSUN-Churches 256x256 DDIM-{a.steps} eta={a.eta} batch {a.batch_size} (random weights), "
                         "sampling + decode_first_stage",
-               images_per_s=a.batch_size / min(times), batch_s=times, unet_eval_ms=e0.elapsed_time(e1) / n,
-               **gpu_info())
-    line = json.dumps(res)
-    print(line)
-    if a.out:
-        os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
-        with open(a.out, "w") as f:
-            f.write(line + "\n")
+               images_per_s=a.batch_size / min(times), batch_s=times, unet_eval_ms=unet_ms, **card())
+    emit(res, a.out)
 
 
 if __name__ == "__main__":

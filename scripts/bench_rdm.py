@@ -2,26 +2,23 @@
 """Retrieval-augmented diffusion sampling speed on the H100 engine: the reference workload of scripts/knn2img.py (768²,
 DDIM-50, eta 0, scale 5.0, batch 3, CLIP text encode, decode_first_stage included) on seeded random weights, text-only
 and with --knn 10 neighbours from a seeded synthetic database (search included). Also reports one graph-replayed UNet
-evaluation at the guided batch (CUDA events) with its FLOPs summed from the GEMM and attention launches of one eager
-evaluation (ops.PROFILE), and the k-NN search kernel alone at N = 1 M, 4 M and 16 M rows of 768 (fp16): time and the
-database bytes streamed per second against the H100 SXM data-sheet HBM3 bandwidth (3.35 TB/s). Prints one JSON line with
-the card name and power limit read in the same run.
+evaluation at the guided batch with the 11-token context (CUDA events) with its FLOPs from the layer shapes, and the
+k-NN search kernel alone at N = 1 M, 4 M and 16 M rows of 768 (fp16): time and the database bytes streamed per second
+against the H100 SXM data-sheet HBM3 bandwidth (3.35 TB/s). Prints one JSON line with the card name and power limit read
+in the same run.
 
   python scripts/bench_rdm.py --out outputs/rdm.json
 """
 import argparse
-import json
 import os
-import statistics
 import sys
-import time
 
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from sdb200 import ops, retrieval  # noqa: E402
-from bench_lsun import gpu_info  # noqa: E402
+from sdb200 import arch, ops, retrieval  # noqa: E402
+from measure import card, emit, event_ms, unet_flops, wall_s  # noqa: E402
 
 HBM_BYTES_PER_S = 3.35e12
 
@@ -45,15 +42,7 @@ def time_search(n, dim, b, k, dev, reps=20):
         db[i:i + x.shape[0]] = (x / x.norm(dim=1, keepdim=True)).half()
     q = torch.randn((b, dim), device=dev, generator=g)
     q = (q / q.norm(dim=1, keepdim=True)).half()
-    for _ in range(3):
-        ops.knn_topk(db, q, k)
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        ops.knn_topk(db, q, k)
-    e1.record()
-    e1.synchronize()
-    ms = e0.elapsed_time(e1) / reps
+    ms = event_ms(lambda: ops.knn_topk(db, q, k), reps, warmup=3)
     del db
     torch.cuda.empty_cache()
     gbs = n * dim * 2 / (ms * 1e-3) / 1e9
@@ -84,17 +73,12 @@ def main():
 
     searcher = synthetic_searcher(a.db_rows, 768, dev)
     res = dict(workload=f"knn2img 768², DDIM-{a.steps} eta 0, scale 5.0, batch 3 (UNet batch 6 at 48x48x16), CLIP text "
-                        f"encode, decode_first_stage, random weights", **gpu_info())
+                        f"encode, decode_first_stage, random weights", **card())
     for tag, s, k in (("text_only", None, 0), ("knn10", searcher, 10)):
         torch.manual_seed(0)
         K.sample(m, Ids(), ["p"] * 3, s, max(k, 1), ddim_steps=a.steps)   # warm-up: autotune, graph capture
         torch.cuda.synchronize()
-        times = []
-        for _ in range(a.repeats):
-            t0 = time.perf_counter()
-            img, c = K.sample(m, Ids(), ["p"] * 3, s, max(k, 1), ddim_steps=a.steps)
-            torch.cuda.synchronize()
-            times.append(time.perf_counter() - t0)
+        times, (img, c) = wall_s(lambda: K.sample(m, Ids(), ["p"] * 3, s, max(k, 1), ddim_steps=a.steps), a.repeats)
         assert img.shape == (3, 3, 768, 768) and bool(torch.isfinite(img).all()) and c.shape[1] == 1 + k
         res[f"images_per_s_{tag}"] = 3 / min(times)
         res[f"run_s_{tag}"] = times
@@ -102,22 +86,8 @@ def main():
     x = torch.randn(6, 16, 48, 48, device=dev)
     t = torch.full((6,), 501.0, device=dev)
     c = torch.randn(6, 11, 768, device=dev)
-    for _ in range(5):
-        u(x, t, context=c)
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    reps = 30
-    e0.record()
-    for _ in range(reps):
-        u(x, t, context=c)
-    e1.record()
-    e1.synchronize()
-    unet_ms = e0.elapsed_time(e1) / reps
-    u.use_cuda_graph = False
-    ops.PROFILE = []
-    u(x, t, context=c)
-    torch.cuda.synchronize()
-    flops = sum(r[1] for r in ops.PROFILE)
-    ops.PROFILE = None
+    unet_ms = event_ms(lambda: u(x, t, context=c), 30, warmup=5)
+    flops = unet_flops(arch.RDM_UNET, 6, 48, 48, c.shape[1])
     res.update(unet_eval_ms_graph=unet_ms, unet_eval_gflop=flops / 1e9, unet_tflop_per_s=flops / (unet_ms * 1e-3) / 1e12)
     del m, u, clip, searcher, x, c
     import gc
@@ -125,12 +95,7 @@ def main():
     torch.cuda.empty_cache()
     res["search_kernel"] = [time_search(n, 768, 3, 10, dev) for n in (1 << 20, 4 << 20, 16 << 20)]
     res["search_kernel"].append(time_search(16 << 20, 768, 64, 64, dev))
-    line = json.dumps(res)
-    print(line)
-    if a.out:
-        os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
-        with open(a.out, "w") as f:
-            f.write(line + "\n")
+    emit(res, a.out)
 
 
 if __name__ == "__main__":

@@ -10,10 +10,8 @@ power limit read in the same run.
   python scripts/bench_semantic.py --repeats 2 --out outputs/semantic.json
 """
 import argparse
-import json
 import os
 import sys
-import time
 
 import torch
 import torch.nn.functional as F
@@ -23,9 +21,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle"))
 from sdb200 import arch, ops  # noqa: E402
 from sdb200.samplers import DDIMSampler  # noqa: E402
-from bench_inpaint import unet_flops  # noqa: E402
-from bench_lsun import gpu_info  # noqa: E402
-from bench_superres import timed  # noqa: E402
+from measure import card, emit, event_ms, unet_flops, wall_s  # noqa: E402
 import semantic_oracle as SO  # noqa: E402
 
 
@@ -35,12 +31,8 @@ def run_workload(S, m, maps, steps, repeats):
     with m.ema_scope():
         S.synthesize(m, sampler, maps, steps=2)        # warm-up: autotune, graph capture, decoder
         torch.cuda.synchronize()
-        times = []
-        for _ in range(repeats):
-            t0 = time.perf_counter()
-            x, c, s = S.synthesize(m, sampler, maps, steps=steps, eta=1.0, return_latents=True)
-            torch.cuda.synchronize()
-            times.append(time.perf_counter() - t0)
+        times, (x, c, s) = wall_s(lambda: S.synthesize(m, sampler, maps, steps=steps, eta=1.0, return_latents=True),
+                                  repeats)
     assert bool(torch.isfinite(x).all())
     return times, c, s
 
@@ -51,8 +43,8 @@ def unet_eval(m, c, dev):
     g = torch.Generator(device=dev).manual_seed(1)
     xt = torch.randn(nb, 3, h, w, generator=g, device=dev)
     t = torch.linspace(1, 981, nb, device=dev).round()
-    ms = timed(lambda: u(xt, t, concat=c), 10)
-    fl = unet_flops(arch.SEMANTIC_SYNTHESIS_UNET, h, w, nb=nb)
+    ms = event_ms(lambda: u(xt, t, concat=c), 10, warmup=2)
+    fl = unet_flops(arch.SEMANTIC_SYNTHESIS_UNET, nb, h, w)
     return ms, fl
 
 
@@ -69,7 +61,7 @@ def label_kernels(m, h, w, dev):
         for _ in range(n):
             x = F.interpolate(x, scale_factor=0.5, mode="bilinear")
         return F.conv2d(x, w4)
-    t_f, t_t = timed(fused, 20), timed(torch_path, 5)
+    t_f, t_t = event_ms(fused, 20, warmup=2), event_ms(torch_path, 5, warmup=2)
     err = float((fused() - torch_path()).abs().max())
     return t_f, t_t, err
 
@@ -89,7 +81,7 @@ def main():
     maps = torch.stack([torch.from_numpy(SO.voronoi_labels(256, 256, 182, 100 + i)) for i in range(8)])
     times, c, s = run_workload(S, m, maps, a.steps, a.repeats)
     ms, fl = unet_eval(m, c, dev)
-    dec = timed(lambda: m.decode_first_stage(s), 3)
+    dec = event_ms(lambda: m.decode_first_stage(s), 3, warmup=2)
     res["ss256"] = dict(workload=f"semantic_synthesis256, 8 maps of 256x256, DDIM-{a.steps} eta 1, cond + sampling + "
                                  "decode, random weights", images_per_s=8 / min(times), run_s=times,
                         unet_eval_ms_graph=ms, unet_tflop=fl / 1e12, unet_tflops=fl / (ms * 1e-3) / 1e12,
@@ -106,18 +98,13 @@ def main():
     maps = torch.from_numpy(SO.voronoi_labels(512, 1024, 182, 200))[None]
     times, c, s = run_workload(S, m, maps, a.steps, a.repeats)
     ms, fl = unet_eval(m, c, dev)
-    dec = timed(lambda: m.decode_first_stage(s), 3)
+    dec = event_ms(lambda: m.decode_first_stage(s), 3, warmup=2)
     res["landscape512x1024"] = dict(workload=f"semantic_synthesis512, one 512x1024 map (latent 128x256), DDIM-{a.steps} "
                                              "eta 1, cond + sampling + decode, random weights",
                                     images_per_s=1 / min(times), run_s=times, unet_eval_ms_graph=ms,
                                     unet_tflop=fl / 1e12, unet_tflops=fl / (ms * 1e-3) / 1e12, decode_ms=dec)
-    res.update(gpu_info())
-    line = json.dumps(res)
-    print(line)
-    if a.out:
-        os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
-        with open(a.out, "w") as f:
-            f.write(line + "\n")
+    res.update(card())
+    emit(res, a.out)
 
 
 if __name__ == "__main__":

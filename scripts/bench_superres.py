@@ -10,10 +10,8 @@ Prints one JSON line with the card name and power limit read in the same run.
   python scripts/bench_superres.py --repeats 2 --out outputs/superres.json
 """
 import argparse
-import json
 import os
 import sys
-import time
 
 import numpy as np
 import torch
@@ -22,21 +20,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from sdb200 import arch, ops  # noqa: E402
 from sdb200.samplers import DDIMSampler  # noqa: E402
-from bench_inpaint import unet_flops  # noqa: E402
-from bench_lsun import gpu_info  # noqa: E402
-
-
-def timed(fn, reps):
-    """Mean milliseconds per call of fn over reps calls, after two warm-up calls (CUDA events)."""
-    for _ in range(2):
-        fn()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    e1.synchronize()
-    return e0.elapsed_time(e1) / reps
+from measure import card, emit, event_ms, unet_flops, wall_s  # noqa: E402
 
 
 def main():
@@ -59,17 +43,17 @@ def main():
     with m.ema_scope():
         S.superresolve(m, sampler, lrs[0], steps=2)          # warm-up: autotune, graph capture, tables, decoder
         torch.cuda.synchronize()
-        times, split = [], []
-        for lr in lrs[1:]:
-            ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
-            t0 = time.perf_counter()
+        runs, events = iter(lrs[1:]), []
+
+        def one_image():
+            ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+            events.append(ev)
             ev[0].record()
-            x, c, s, path = S.superresolve(m, sampler, lr, steps=a.steps, eta=1.0, return_latents=True)
+            out = S.superresolve(m, sampler, next(runs), steps=a.steps, eta=1.0, return_latents=True)
             ev[1].record()
-            torch.cuda.synchronize()
-            times.append(time.perf_counter() - t0)
-            ev[1].synchronize()
-            split.append(ev[0].elapsed_time(ev[1]))
+            return out
+        times, (x, c, s, path) = wall_s(one_image, a.repeats)
+        split = [e0.elapsed_time(e1) for e0, e1 in events]
     assert path == "split" and tuple(x.shape) == (1, 3, 4 * a.size, 4 * a.size) and bool(torch.isfinite(x).all())
 
     plan = m._split_plan((1, 3, a.size, a.size), 1, dev)
@@ -79,19 +63,21 @@ def main():
     xt = torch.randn(n, 3, *ks, generator=gt, device=dev)
     ct = torch.randn(n, 3, *ks, generator=gt, device=dev)
     t = torch.full((n,), 501.0, device=dev)
-    tiled = timed(lambda: u(xt, t, concat=ct), 20)
+    tiled = event_ms(lambda: u(xt, t, concat=ct), 20, warmup=2)
     one = [(xt[i:i + 1].contiguous(), t[i:i + 1].contiguous(), ct[i:i + 1].contiguous()) for i in range(n)]
-    nine_calls = timed(lambda: [u(x1, t1, concat=c1) for x1, t1, c1 in one], 10)
-    fl = unet_flops(arch.BSR_SR_UNET, *ks, nb=n)
-    decode = timed(lambda: m.decode_first_stage(s), 3)
+    nine_calls = event_ms(lambda: [u(x1, t1, concat=c1) for x1, t1, c1 in one], 10, warmup=2)
+    fl = unet_flops(arch.BSR_SR_UNET, n, *ks)
+    decode = event_ms(lambda: m.decode_first_stage(s), 3, warmup=2)
     eps_tiles = u(xt, t, concat=ct)
-    fold_eps = timed(lambda: ops.patch_fold(eps_tiles, plan["weight"], plan["norm"], plan["grid"], plan["stride"]), 50)
+    fold_eps = event_ms(lambda: ops.patch_fold(eps_tiles, plan["weight"], plan["norm"], plan["grid"], plan["stride"]), 50,
+                        warmup=2)
     xl = torch.randn(1, 3, a.size, a.size, generator=gt, device=dev)
-    unfold = timed(lambda: ops.patch_unfold(xl, ks, plan["stride"]), 50)
+    unfold = event_ms(lambda: ops.patch_unfold(xl, ks, plan["stride"]), 50, warmup=2)
     kd = dplan["ks"][0] * 4
     dec_tiles = torch.randn(dplan["n"], kd, kd, 3, generator=gt, device=dev)
     sd = (dplan["stride"][0] * 4, dplan["stride"][1] * 4)
-    fold_dec = timed(lambda: ops.patch_fold(dec_tiles, dplan["weight"], dplan["norm"], dplan["grid"], sd, nhwc=True), 20)
+    fold_dec = event_ms(lambda: ops.patch_fold(dec_tiles, dplan["weight"], dplan["norm"], dplan["grid"], sd, nhwc=True),
+                        20, warmup=2)
     res = dict(workload=f"bsr_sr LDM, {a.size}x{a.size} -> {4 * a.size}x{4 * a.size}, {plan['grid'][0]}x{plan['grid'][1]} "
                         f"tiles of {ks[0]}x{ks[1]} at stride {plan['stride'][0]}, DDIM-{a.steps} eta 1, batch 1, LR "
                         "conversion + tiled sampling + tiled VQ-f4 decode, random weights",
@@ -99,13 +85,8 @@ def main():
                unet_tiled_eval_ms_graph=tiled, unet_tiled_tflop=fl / 1e12, unet_tiled_tflops=fl / (tiled * 1e-3) / 1e12,
                unet_nine_single_tile_calls_ms_graph=nine_calls, tiled_decode_ms=decode,
                stitch_eps_fold_ms=fold_eps, stitch_decode_fold_ms=fold_dec, unfold_xt_ms=unfold,
-               unet_chunk=plan["chunk"], decode_chunk=dplan["chunk"], **gpu_info())
-    line = json.dumps(res)
-    print(line)
-    if a.out:
-        os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
-        with open(a.out, "w") as f:
-            f.write(line + "\n")
+               unet_chunk=plan["chunk"], decode_chunk=dplan["chunk"], **card())
+    emit(res, a.out)
 
 
 if __name__ == "__main__":
