@@ -52,9 +52,9 @@ def wall_s(fn, repeats):
 def unet_flops(cfg, nb, h, w, n_ctx=0):
     """Algorithmic FLOPs (2 per multiply-add) of one UNet evaluation at batch nb on an h x w latent, walking
     arch.unet_plan: 3x3 convolutions, 1x1 skips, attention projections, Q K^T and P V over the tokens and the n_ctx
-    context tokens, and the spatial transformers' GEGLU feed-forward. Norms, FiLM and pointwise work are not counted,
-    nor are the cross-attention K / V projections of the context, which the engine computes once per context, not per
-    evaluation. A layer kind without a count here raises."""
+    context tokens, and the spatial transformers' GEGLU feed-forward, the last three once per transformer block. Norms,
+    FiLM and pointwise work are not counted, nor are the cross-attention K / V projections of the context, which the
+    engine computes once per context, not per evaluation. A layer kind without a count here raises."""
     plan = arch.unet_plan(cfg)
     px, total = h * w, 0
 
@@ -74,8 +74,8 @@ def unet_flops(cfg, nb, h, w, n_ctx=0):
             total += conv(a["cin"], a["cout"], 1) if a["cin"] != a["cout"] else 0
         elif kind == "attn":            # qkv and proj_out
             total += conv(a["ch"], 4 * a["ch"], 1) + 4 * nb * px * px * a["ch"]
-        elif kind == "st":              # proj in / out 2, attn1 q k v out 4, attn2 q out 2, ff c -> 8c and 4c -> c 12
-            total += conv(a["ch"], 20 * a["ch"], 1) + 4 * nb * px * (px + n_ctx) * a["ch"]
+        elif kind == "st":              # proj in / out 2; per block attn1 q k v out 4, attn2 q out 2, ff c -> 8c, 4c -> c 12
+            total += conv(a["ch"], (2 + 18 * a["depth"]) * a["ch"], 1) + a["depth"] * 4 * nb * px * (px + n_ctx) * a["ch"]
         elif kind in ("down", "up"):
             total += conv(a["ch"], a["ch"])
         else:

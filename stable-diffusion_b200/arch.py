@@ -156,6 +156,18 @@ TEXT2IMG256_BERT = dict(n_embed=640, n_layer=32, vocab_size=30522, max_seq_len=7
 TINY_TEXT2IMG256_UNET = dict(image_size=16, in_channels=3, out_channels=3, model_channels=64, attention_resolutions=[2, 4],
                              num_res_blocks=1, channel_mult=[1, 2, 3], num_head_channels=32, use_spatial_transformer=True,
                              transformer_depth=1, context_dim=128)
+# the layout-to-image LDM (models/ldm/layout2img-openimages256/config.yaml): a 64x64x3 latent, spatial transformers of
+# three BasicTransformerBlocks each, with heads of num_head_channels 32 (8 / 12 / 16 heads at widths 256 / 384 / 512,
+# 32² / 16² / 8² tokens), cross-attending to a 92-token BERTEmbedder(n_embed=512, n_layer=16, vocab_size=8192) context
+# fed token ids directly (cond_stage_key coordinates_bbox, use_tokenizer False); the VQ-f4 first stage (VQ_F4)
+LAYOUT2IMG_UNET = dict(image_size=64, in_channels=3, out_channels=3, model_channels=128, attention_resolutions=[8, 4, 2],
+                       num_res_blocks=2, channel_mult=[1, 2, 3, 4], num_head_channels=32, use_spatial_transformer=True,
+                       transformer_depth=3, context_dim=512)
+LAYOUT2IMG_BERT = dict(n_embed=512, n_layer=16, vocab_size=8192, max_seq_len=92)
+# small members for tests: TINY_TEXT2IMG256_UNET with three blocks per spatial transformer, and a two-layer BERT with the
+# model's 92 positions and 8192-id vocabulary; first stage TINY_VQ_F4
+TINY_LAYOUT2IMG_UNET = dict(TINY_TEXT2IMG256_UNET, transformer_depth=3)
+TINY_LAYOUT2IMG_BERT = dict(n_embed=128, n_layer=2, vocab_size=8192, max_seq_len=92)
 # the retrieval-augmented diffusion model (configs/retrieval-augmented-diffusion/768x768.yaml, scripts/knn2img.py): a
 # 48x48x16 latent, spatial transformers with heads of num_head_channels 32 (14 / 28 / 42 heads at widths 448 / 896 /
 # 1344, 56 in the middle block) cross-attending to CLIP ViT-L/14's projected text embedding and its retrieved
@@ -212,7 +224,8 @@ TINY_CLIP_VISION_PROJ = dict(hidden_size=128, intermediate_size=256, num_hidden_
 def unet_plan(cfg):
     """Block list of UNetModel as (kind, prefix, params) tuples, in execution order.
 
-    kinds: conv_in, res(cin, cout, ss, updown), st(ch, heads, dhead), attn(ch, heads, dhead), down(ch), up(ch), out.
+    kinds: conv_in, res(cin, cout, ss, updown), st(ch, heads, dhead, depth), attn(ch, heads, dhead), down(ch), up(ch),
+    out.
     Mirrors the constructor loops at openaimodel.py:512-686. Without a spatial transformer the attention layers are
     AttentionBlocks with `num_heads` heads of ch / num_heads channels (legacy=True passes num_head_channels=-1,
     openaimodel.py:547-549), or, when num_head_channels is set, ch / num_head_channels heads of num_head_channels
@@ -229,13 +242,14 @@ def unet_plan(cfg):
     ss = bool(cfg.get("use_scale_shift_norm", False))
     updown = bool(cfg.get("resblock_updown", False))
     akind = "st" if st else "attn"
+    depth = {"depth": cfg.get("transformer_depth", 1)} if st else {}     # BasicTransformerBlocks per SpatialTransformer
 
     def res(pre, cin, cout, ud=None, **kw):
         return ("res", pre, dict(cin=cin, cout=cout, ss=ss, updown=ud, **kw))
 
     def att(pre, ch):
         heads = nh if nhc == -1 else ch // nhc
-        return (akind, pre, dict(ch=ch, heads=heads, dhead=ch // heads))
+        return (akind, pre, dict(ch=ch, heads=heads, dhead=ch // heads, **depth))
 
     plan = {"input": [], "middle": [], "output": []}
     plan["input"].append([("conv_in", "input_blocks.0.0", dict(cin=cfg["in_channels"], cout=mc))])
@@ -296,25 +310,26 @@ def _res_shapes(p, pre, cin, cout, temb, ss=False):
         p[f"{pre}.skip_connection.bias"] = (cout,)
 
 
-def _st_shapes(p, pre, ch, ctx):
+def _st_shapes(p, pre, ch, ctx, depth=1):
     p[f"{pre}.norm.weight"] = (ch,)
     p[f"{pre}.norm.bias"] = (ch,)
     p[f"{pre}.proj_in.weight"] = (ch, ch, 1, 1)
     p[f"{pre}.proj_in.bias"] = (ch,)
-    tb = f"{pre}.transformer_blocks.0"
-    for a, kdim in (("attn1", ch), ("attn2", ctx)):
-        p[f"{tb}.{a}.to_q.weight"] = (ch, ch)
-        p[f"{tb}.{a}.to_k.weight"] = (ch, kdim)
-        p[f"{tb}.{a}.to_v.weight"] = (ch, kdim)
-        p[f"{tb}.{a}.to_out.0.weight"] = (ch, ch)
-        p[f"{tb}.{a}.to_out.0.bias"] = (ch,)
-    p[f"{tb}.ff.net.0.proj.weight"] = (8 * ch, ch)
-    p[f"{tb}.ff.net.0.proj.bias"] = (8 * ch,)
-    p[f"{tb}.ff.net.2.weight"] = (ch, 4 * ch)
-    p[f"{tb}.ff.net.2.bias"] = (ch,)
-    for n in ("norm1", "norm2", "norm3"):
-        p[f"{tb}.{n}.weight"] = (ch,)
-        p[f"{tb}.{n}.bias"] = (ch,)
+    for i in range(depth):
+        tb = f"{pre}.transformer_blocks.{i}"
+        for a, kdim in (("attn1", ch), ("attn2", ctx)):
+            p[f"{tb}.{a}.to_q.weight"] = (ch, ch)
+            p[f"{tb}.{a}.to_k.weight"] = (ch, kdim)
+            p[f"{tb}.{a}.to_v.weight"] = (ch, kdim)
+            p[f"{tb}.{a}.to_out.0.weight"] = (ch, ch)
+            p[f"{tb}.{a}.to_out.0.bias"] = (ch,)
+        p[f"{tb}.ff.net.0.proj.weight"] = (8 * ch, ch)
+        p[f"{tb}.ff.net.0.proj.bias"] = (8 * ch,)
+        p[f"{tb}.ff.net.2.weight"] = (ch, 4 * ch)
+        p[f"{tb}.ff.net.2.bias"] = (ch,)
+        for n in ("norm1", "norm2", "norm3"):
+            p[f"{tb}.{n}.weight"] = (ch,)
+            p[f"{tb}.{n}.bias"] = (ch,)
     p[f"{pre}.proj_out.weight"] = (ch, ch, 1, 1)
     p[f"{pre}.proj_out.bias"] = (ch,)
 
@@ -331,7 +346,7 @@ def _attn_block_shapes(p, pre, ch):
 
 def unet_param_shapes(cfg):
     """OrderedDict key -> shape, keys exactly as UNetModel.state_dict() (686 tensors for SD v1)."""
-    assert cfg.get("transformer_depth", 1) == 1, "SD v1 uses transformer_depth 1"
+    assert cfg.get("transformer_depth", 1) in (1, 3), "the published LDMs use transformer_depth 1 or 3"
     mc = cfg["model_channels"]
     temb = 4 * mc
     ctx = cfg.get("context_dim")
@@ -350,7 +365,7 @@ def unet_param_shapes(cfg):
             elif kind == "res":
                 _res_shapes(p, pre, a["cin"], a["cout"], temb, a["ss"])
             elif kind == "st":
-                _st_shapes(p, pre, a["ch"], ctx)
+                _st_shapes(p, pre, a["ch"], ctx, a["depth"])
             elif kind == "attn":
                 _attn_block_shapes(p, pre, a["ch"])
             elif kind == "down":

@@ -3,7 +3,8 @@ reference's `ldm.modules.diffusionmodules.openaimodel.UNetModel` (constructor kw
 `forward(x, timesteps, context)` openaimodel.py:710-742, state-dict keys unchanged).
 
 Two members of the reference's UNet family run: the SD-v1 spatial-transformer UNet (cross-attention on a context, with
-num_heads heads, or heads of num_head_channels as in the cin256 LDM-VQ-8), and
+num_heads heads, or heads of num_head_channels as in the cin256 LDM-VQ-8; one BasicTransformerBlock per
+SpatialTransformer, or three as in layout2img-openimages256), and
 the unconditional AttentionBlock UNet (use_spatial_transformer=False, e.g. LSUN-Churches) with any combination of
 use_scale_shift_norm and resblock_updown, or with plain ResBlocks and heads of num_head_channels (the VQ-f4 models).
 
@@ -121,8 +122,9 @@ class UNetModel(PackedStage):
                            conv_resample=not conv_resample, use_new_attention_order=bool(use_new_attention_order),
                            num_heads_upsample=num_heads_upsample not in (-1, num_heads))
         if use_spatial_transformer:
+            # depth 1 (every other spatial-transformer LDM) and 3 (layout2img-openimages256) are the published ones
             unsupported.update(resblock_updown=resblock_updown, use_scale_shift_norm=use_scale_shift_norm,
-                               transformer_depth=transformer_depth != 1)
+                               transformer_depth=transformer_depth not in (1, 3))
         bad = [k for k, v in unsupported.items() if v]
         if bad:
             raise NotImplementedError("sdb200.UNetModel supports the SD-v1 UNet and the unconditional AttentionBlock UNet "
@@ -131,7 +133,8 @@ class UNetModel(PackedStage):
                         out_channels=out_channels, num_res_blocks=num_res_blocks,
                         attention_resolutions=list(attention_resolutions), channel_mult=list(channel_mult),
                         num_heads=num_heads, num_head_channels=num_head_channels,
-                        use_spatial_transformer=bool(use_spatial_transformer), transformer_depth=1,
+                        use_spatial_transformer=bool(use_spatial_transformer),
+                        transformer_depth=int(transformer_depth) if use_spatial_transformer else 1,
                         context_dim=context_dim, legacy=legacy, use_scale_shift_norm=bool(use_scale_shift_norm),
                         resblock_updown=bool(resblock_updown))
         self.conditional = bool(use_spatial_transformer)   # cross-attention on a context; otherwise forward(x, t)
@@ -245,26 +248,32 @@ class UNetModel(PackedStage):
             s["b_proj"] = (sd[pre + ".proj_out.bias"].double() + wp.double() @ b[:, 2].reshape(-1).double()).float().contiguous()
             return s
 
+        def pack_block(tb):
+            """One BasicTransformerBlock (attention.py:196-215)."""
+            b = {"tb": tb}
+            for i in (1, 2, 3):
+                b[f"ln{i}"] = (f32(f"{tb}.norm{i}.weight"), f32(f"{tb}.norm{i}.bias"))
+            b["w_qk1"] = torch.cat([sd[tb + ".attn1.to_q.weight"], sd[tb + ".attn1.to_k.weight"]], 0).half().contiguous()
+            b["w_v1"] = f16(tb + ".attn1.to_v.weight")
+            b["w_o1"], b["b_o1"] = f16(tb + ".attn1.to_out.0.weight"), f32(tb + ".attn1.to_out.0.bias")
+            b["w_q2"] = f16(tb + ".attn2.to_q.weight")
+            b["w_k2"] = f16(tb + ".attn2.to_k.weight")
+            b["w_v2"] = f16(tb + ".attn2.to_v.weight")
+            b["w_o2"], b["b_o2"] = f16(tb + ".attn2.to_out.0.weight"), f32(tb + ".attn2.to_out.0.bias")
+            b["w_ff1"], b["b_ff1"] = _pack_geglu(sd[tb + ".ff.net.0.proj.weight"], sd[tb + ".ff.net.0.proj.bias"])
+            b["w_ff2"], b["b_ff2"] = f16(tb + ".ff.net.2.weight"), f32(tb + ".ff.net.2.bias")
+            return b
+
         def pack_st(pre, a):
-            """SpatialTransformer with the plan's heads of dhead channels (num_heads, or ch / num_head_channels)."""
+            """SpatialTransformer with the plan's heads of dhead channels (num_heads, or ch / num_head_channels) and its
+            `depth` BasicTransformerBlocks in order."""
             ch, d = a["ch"], a["dhead"]
             dp = _dpad(d)
-            tb = pre + ".transformer_blocks.0"
-            s = {"ch": ch, "d": d, "dpad": dp, "heads": a["heads"], "tb": tb}
+            s = {"ch": ch, "d": d, "dpad": dp, "heads": a["heads"]}
             s["gn"] = (f32(pre + ".norm.weight"), f32(pre + ".norm.bias"))
             s["w_in"], s["b_in"] = one(sd[pre + ".proj_in.weight"].reshape(ch, ch)), f32(pre + ".proj_in.bias")
             s["w_out"], s["b_out"] = one(sd[pre + ".proj_out.weight"].reshape(ch, ch)), f32(pre + ".proj_out.bias")
-            for i in (1, 2, 3):
-                s[f"ln{i}"] = (f32(f"{tb}.norm{i}.weight"), f32(f"{tb}.norm{i}.bias"))
-            s["w_qk1"] = torch.cat([sd[tb + ".attn1.to_q.weight"], sd[tb + ".attn1.to_k.weight"]], 0).half().contiguous()
-            s["w_v1"] = f16(tb + ".attn1.to_v.weight")
-            s["w_o1"], s["b_o1"] = f16(tb + ".attn1.to_out.0.weight"), f32(tb + ".attn1.to_out.0.bias")
-            s["w_q2"] = f16(tb + ".attn2.to_q.weight")
-            s["w_k2"] = f16(tb + ".attn2.to_k.weight")
-            s["w_v2"] = f16(tb + ".attn2.to_v.weight")
-            s["w_o2"], s["b_o2"] = f16(tb + ".attn2.to_out.0.weight"), f32(tb + ".attn2.to_out.0.bias")
-            s["w_ff1"], s["b_ff1"] = _pack_geglu(sd[tb + ".ff.net.0.proj.weight"], sd[tb + ".ff.net.0.proj.bias"])
-            s["w_ff2"], s["b_ff2"] = f16(tb + ".ff.net.2.weight"), f32(tb + ".ff.net.2.bias")
+            s["blocks"] = [pack_block(f"{pre}.transformer_blocks.{i}") for i in range(a["depth"])]
             return s
 
         def pack_layers(layers):
@@ -351,30 +360,58 @@ class UNetModel(PackedStage):
             out._sdb_f16 = o16.view(nb, H, Wd, r["cout"])
         return out
 
-    def _st(self, s, x, kv, emit_f16=False):
-        """SpatialTransformer.forward (attention.py:250-261) with one BasicTransformerBlock (:211-215)."""
+    def _st(self, s, x, kvs, emit_f16=False):
+        """SpatialTransformer.forward (attention.py:250-261): GroupNorm and proj_in, the BasicTransformerBlocks in order
+        (one cross-attention K / V^T of `kvs` each) on the fp32 token stream, then proj_out and the residual. A block
+        before the last writes its feed-forward output in fp32 for the next block's LayerNorm; the last one's goes to
+        proj_out as fp16 (hi / lo in fp16x3)."""
         nb, H, Wd, ch = x.shape
         ntok = H * Wd
-        heads, d, dp = s["heads"], s["d"], s["dpad"]
-        hd = heads * d                                                                     # heads packed at stride d
-        scale = d ** -0.5
         x3 = self.W["x3"]
         if x3:
             xn, _, xn_lo, _ = ops.groupnorm(x, *s["gn"], eps=1e-6, silu=False, want_lo=True)
-            _, t0 = ops.gemm(xn, s["w_in"], a1=xn_lo, a2=xn, bias=s["b_in"], want_f32=True, splits=-1)
+            _, t = ops.gemm(xn, s["w_in"], a1=xn_lo, a2=xn, bias=s["b_in"], want_f32=True, splits=-1)
         else:
             xn, _ = ops.groupnorm(x, *s["gn"], eps=1e-6, silu=False)
-            _, t0 = ops.gemm(xn, s["w_in"], bias=s["b_in"], want_f32=True, splits=-1)      # tokens [M, ch] fp32
+            _, t = ops.gemm(xn, s["w_in"], bias=s["b_in"], want_f32=True, splits=-1)       # tokens [M, ch] fp32
+        blocks = s["blocks"]
+        assert len(kvs) == len(blocks)
+        for b, kv in zip(blocks[:-1], kvs[:-1]):
+            t2, g = self._block(s, b, t, kv, nb, ntok)
+            _, t = ops.gemm(g, b["w_ff2"], bias=b["b_ff2"], residual=t2, want_f32=True, splits=-1)
+        b = blocks[-1]
+        t2, g = self._block(s, b, t, kvs[-1], nb, ntok)
+        if x3:
+            t3, _, t3_lo = ops.gemm(g, b["w_ff2"], bias=b["b_ff2"], residual=t2, want_lo=True, splits=-1)
+            o16, out = ops.gemm(t3, s["w_out"], a1=t3_lo, a2=t3, bias=s["b_out"], residual=x.view(-1, ch), want_f32=True,
+                                want_f16=emit_f16, splits=-1, rows_per_sample=ntok, want_stats=True, stats_group=self._sg)
+        else:
+            t3, _ = ops.gemm(g, b["w_ff2"], bias=b["b_ff2"], residual=t2, want_f16=True, splits=-1)
+            o16, out = ops.gemm(t3, s["w_out"], bias=s["b_out"], residual=x.view(-1, ch), want_f32=True,
+                                want_f16=emit_f16, splits=-1, rows_per_sample=ntok, want_stats=True, stats_group=self._sg)
+        out = out.view(nb, H, Wd, ch)
+        if emit_f16:
+            out._sdb_f16 = o16.view(nb, H, Wd, ch)
+        return out
+
+    def _block(self, s, b, t0, kv, nb, ntok):
+        """BasicTransformerBlock._forward (attention.py:211-215) on the fp32 tokens t0 up to the feed-forward's GEGLU:
+        returns the residual stream after both attentions (fp32) and the GEGLU output (fp16), whose second linear layer
+        the caller runs with the output form it needs."""
+        ch = s["ch"]
+        heads, d, dp = s["heads"], s["d"], s["dpad"]
+        hd = heads * d                                                                     # heads packed at stride d
+        scale = d ** -0.5
         # --- self attention
-        y = ops.layernorm(t0, *s["ln1"])
-        qk, _ = ops.gemm(y, s["w_qk1"], want_f16=True)                                     # [M, 2*hd]
+        y = ops.layernorm(t0, *b["ln1"])
+        qk, _ = ops.gemm(y, b["w_qk1"], want_f16=True)                                     # [M, 2*hd]
         qk3 = qk.view(nb, ntok, 2 * hd)
         if ntok % 8 == 0:
             # V^T straight out of the tensor cores by swapping the operand roles: [hd, M] = Wv . y^T
-            vt, _ = ops.gemm(s["w_v1"], y, want_f16=True, b_dynamic=True)
+            vt, _ = ops.gemm(b["w_v1"], y, want_f16=True, b_dynamic=True)
             vt3 = vt.view(hd, nb, ntok).permute(1, 0, 2)                                   # [nb, hd, ntok] (strided view)
         else:  # TMA needs 16-byte aligned strides: tiny token counts go through an explicit transpose
-            v, _ = ops.gemm(y, s["w_v1"], want_f16=True)
+            v, _ = ops.gemm(y, b["w_v1"], want_f16=True)
             vt3 = ops.transpose_f16(v.view(nb, ntok, hd))
         o = ops.attention(qk3[:, :, :hd], qk3[:, :, hd:], vt3, heads=heads, d=d, dpad=dp, nq=ntok, nkv=ntok, scale=scale,
                           head_stride=d)
@@ -382,32 +419,21 @@ class UNetModel(PackedStage):
         if k2 is None:
             # one-token context (context_kv): attn2(LN2(t1), c) = u per sample, added as the FiLM operand of the attn1
             # out-projection, which then yields t2 = t0 + attn1 + u directly
-            _, t2 = ops.gemm(o.view(-1, ch), s["w_o1"], bias=s["b_o1"], film=vt2, rows_per_sample=ntok, residual=t0,
+            _, t2 = ops.gemm(o.view(-1, ch), b["w_o1"], bias=b["b_o1"], film=vt2, rows_per_sample=ntok, residual=t0,
                              want_f32=True, splits=-1)
         else:
-            _, t1 = ops.gemm(o.view(-1, ch), s["w_o1"], bias=s["b_o1"], residual=t0, want_f32=True, splits=-1)
+            _, t1 = ops.gemm(o.view(-1, ch), b["w_o1"], bias=b["b_o1"], residual=t0, want_f32=True, splits=-1)
             # --- cross attention (K / V^T of the context are precomputed per prompt)
-            y = ops.layernorm(t1, *s["ln2"])
-            q, _ = ops.gemm(y, s["w_q2"], want_f16=True)
+            y = ops.layernorm(t1, *b["ln2"])
+            q, _ = ops.gemm(y, b["w_q2"], want_f16=True)
             o = ops.attention(q.view(nb, ntok, hd), k2, vt2, heads=heads, d=d, dpad=dp, nq=ntok, nkv=nkv, scale=scale,
                               head_stride=d)
-            _, t2 = ops.gemm(o.view(-1, ch), s["w_o2"], bias=s["b_o2"], residual=t1, want_f32=True, splits=-1)
+            _, t2 = ops.gemm(o.view(-1, ch), b["w_o2"], bias=b["b_o2"], residual=t1, want_f32=True, splits=-1)
         # --- GEGLU feed-forward
-        y = ops.layernorm(t2, *s["ln3"])
-        g, _ = ops.gemm(y, s["w_ff1"], bias=s["b_ff1"], act=ACT_GEGLU, want_f16=True,
-                        block_n=_geglu_tile(s["w_ff1"].shape[0] // 2))
-        if x3:
-            t3, _, t3_lo = ops.gemm(g, s["w_ff2"], bias=s["b_ff2"], residual=t2, want_lo=True, splits=-1)
-            o16, out = ops.gemm(t3, s["w_out"], a1=t3_lo, a2=t3, bias=s["b_out"], residual=x.view(-1, ch), want_f32=True,
-                                want_f16=emit_f16, splits=-1, rows_per_sample=ntok, want_stats=True, stats_group=self._sg)
-        else:
-            t3, _ = ops.gemm(g, s["w_ff2"], bias=s["b_ff2"], residual=t2, want_f16=True, splits=-1)
-            o16, out = ops.gemm(t3, s["w_out"], bias=s["b_out"], residual=x.view(-1, ch), want_f32=True,
-                                want_f16=emit_f16, splits=-1, rows_per_sample=ntok, want_stats=True, stats_group=self._sg)
-        out = out.view(nb, H, Wd, ch)
-        if emit_f16:
-            out._sdb_f16 = o16.view(nb, H, Wd, ch)
-        return out
+        y = ops.layernorm(t2, *b["ln3"])
+        g, _ = ops.gemm(y, b["w_ff1"], bias=b["b_ff1"], act=ACT_GEGLU, want_f16=True,
+                        block_n=_geglu_tile(b["w_ff1"].shape[0] // 2))
+        return t2, g
 
     def _attn(self, s, x, emit_f16=False):
         """AttentionBlock._forward (openaimodel.py:318-324) with QKVAttentionLegacy (:347-372) on the flash kernel.
@@ -442,20 +468,26 @@ class UNetModel(PackedStage):
         if "u_w" not in W:      # from the fp32 weights of the set in use: one fp16 rounding of the product
             src = self._host_sd if self._active == "raw" else self._alt_sd[self._active]
             f64 = lambda k: src[k].to(device=W["device"], dtype=torch.float64)
-            W["u_w"] = torch.cat([(f64(s["tb"] + ".attn2.to_out.0.weight") @ f64(s["tb"] + ".attn2.to_v.weight")).half()
-                                  for s in W["st_list"]], 0).contiguous()
-            W["u_b"] = torch.cat([s["b_o2"] for s in W["st_list"]], 0).contiguous()
+            tbs = [s["blocks"][0] for s in W["st_list"]]
+            W["u_w"] = torch.cat([(f64(b["tb"] + ".attn2.to_out.0.weight") @ f64(b["tb"] + ".attn2.to_v.weight")).half()
+                                  for b in tbs], 0).contiguous()
+            W["u_b"] = torch.cat([b["b_o2"] for b in tbs], 0).contiguous()
         return W["u_w"], W["u_b"]
 
     def context_kv(self, context, static=False):
-        """Cross-attention K and V^T for all SpatialTransformers (x/t independent: once per prompt).
-        static=True writes into persistent per-shape buffers so captured CUDA graphs stay valid across prompts.
+        """Cross-attention K and V^T for every BasicTransformerBlock of every SpatialTransformer, in execution order
+        (x/t independent: once per prompt). static=True writes into persistent per-shape buffers, one per block, so
+        captured CUDA graphs stay valid across prompts.
         A one-token context (the ClassEmbedder's) makes the softmax over one key exactly 1, so attn2(x, c) =
         to_out(to_v(c)) does not depend on x: each SpatialTransformer gets (None, u [nb, ch], 1) with
-        u = W_o2 W_v2 c + b_o2 instead of K / V^T."""
+        u = W_o2 W_v2 c + b_o2 instead of K / V^T. That fold is made for single-block transformers only: no published
+        model pairs a one-token context with deeper ones."""
         nb, nkv, cd = context.shape
         bufs = self._kv_static.setdefault((nb, nkv), {}) if static else {}
         if nkv == 1:
+            if self.cfg["transformer_depth"] != 1:
+                raise NotImplementedError("a one-token context (ClassEmbedder) with transformer_depth "
+                                          f"{self.cfg['transformer_depth']}: only depth 1 is supported")
             w, b = self._one_token_weights()
             u = ops.linear_small(context.contiguous().float().view(nb, cd), w, b, out=bufs.get("u"))
             bufs["u"] = u
@@ -467,15 +499,15 @@ class UNetModel(PackedStage):
         ctx16 = ops.cast_f16(context.contiguous().float().view(nb * nkv, cd))
         ld = (nkv + 7) // 8 * 8
         out = []
-        for i, s in enumerate(self.W["st_list"]):
+        for i, (s, b) in enumerate((s, b) for s in self.W["st_list"] for b in s["blocks"]):
             hd = s["heads"] * s["d"]
             if i not in bufs:
                 bufs[i] = (torch.empty((nb * nkv, hd), dtype=torch.float16, device=context.device),
                            torch.empty((nb * nkv, hd), dtype=torch.float16, device=context.device),
                            torch.empty((nb, hd, ld), dtype=torch.float16, device=context.device))
             kb, vb, vtb = bufs[i]
-            ops.gemm(ctx16, s["w_k2"], out_f16=kb)
-            ops.gemm(ctx16, s["w_v2"], out_f16=vb)
+            ops.gemm(ctx16, b["w_k2"], out_f16=kb)
+            ops.gemm(ctx16, b["w_v2"], out_f16=vb)
             ops.transpose_f16(vb.view(nb, nkv, hd), out=vtb)
             out.append((kb.view(nb, nkv, hd), vtb, nkv))
         return out
@@ -507,8 +539,9 @@ class UNetModel(PackedStage):
                 h = self._res(p, h, skip, film, emit_f16=last)
                 skip = None
             elif kind == "st":
-                h = self._st(p, h, kvs[st_idx[0]], emit_f16=last)
-                st_idx[0] += 1
+                n = len(p["blocks"])
+                h = self._st(p, h, kvs[st_idx[0]: st_idx[0] + n], emit_f16=last)
+                st_idx[0] += n
             elif kind == "attn":
                 h = self._attn(p, h, emit_f16=last)
             elif kind == "down":
