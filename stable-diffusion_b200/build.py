@@ -32,7 +32,7 @@ def _newer(target: Path, deps) -> bool:
 
 def build(verbose: bool = False, force: bool = False) -> Path:
     sources = sorted(CSRC.glob("*.cu"))
-    headers = sorted(CSRC.glob("*.cuh")) + sorted(CSRC.glob("*.h")) + [CSRC.parent.parent / "include" / "sdb200.h"]
+    headers = sorted(CSRC.glob("*.cuh")) + sorted(CSRC.glob("*.h")) + sorted((CSRC.parent.parent / "include").glob("*.h"))
     objs = []
     jobs = []
     for src in sources:

@@ -7,7 +7,10 @@ Sub-modules keep the reference attribute names so checkpoint prefixes resolve:
 Unconditional models (cond_stage_config "__is_unconditional__", e.g. LSUN-Churches) sample through DDIM with no
 conditioning, or through the ancestral sampler (p_sample_loop / progressive_denoising, ddpm.py:1047-1213) whose update
 is one fused kernel per step (sdb_ddpm_step).
-Training (p_losses, training_step, optimizers, logging) is out of scope.
+The denoising objective is evaluated forward-only: p_losses / get_loss (:1012-1045, :279-293), forward (:870-879),
+get_input (:654-705), shared_step (:865-868) and validation_step (:358-364), with the noising at one timestep per sample
+(sdb_q_sample_t) and the per-sample reduction (sdb_diffusion_loss) as kernels. Training itself (gradients, optimizers,
+EMA updates, logging) is out of scope.
 """
 from __future__ import annotations
 
@@ -135,9 +138,19 @@ class LatentDiffusion(nn.Module):
                  cond_stage_trainable=False, concat_mode=True, cond_stage_forward=None, conditioning_key=None,
                  scale_factor=1.0, scale_by_std=False, parameterization="eps", use_ema=True, image_size=256,
                  channels=3, first_stage_key="image", log_every_t=100, monitor=None, v_posterior=0.,
-                 scheduler_config=None, **ignored):
+                 scheduler_config=None, loss_type="l2", l_simple_weight=1., original_elbo_weight=0.,
+                 learn_logvar=False, logvar_init=0., **ignored):
         super().__init__()
         assert parameterization == "eps" and beta_schedule == "linear"
+        if learn_logvar:
+            raise NotImplementedError("learn_logvar: a learned per-timestep logvar is a training parameter; no "
+                                      "published config sets it")
+        if loss_type not in ops.LOSS_KINDS:
+            raise NotImplementedError(f"unknown loss type '{loss_type}'")
+        self.loss_type = loss_type
+        self.l_simple_weight, self.original_elbo_weight = float(l_simple_weight), float(original_elbo_weight)
+        self.learn_logvar, self.logvar_init = False, float(logvar_init)
+        self.cond_stage_trainable = bool(cond_stage_trainable)
         if conditioning_key is None:
             conditioning_key = "concat" if concat_mode else "crossattn"
         if cond_stage_config == "__is_unconditional__":      # ddpm.py:447-448, 501-504
@@ -189,6 +202,13 @@ class LatentDiffusion(nn.Module):
                              to_torch(betas * np.sqrt(alphas_cumprod_prev) / (1. - alphas_cumprod)), **nonp)
         self.register_buffer("posterior_mean_coef2",
                              to_torch((1. - alphas_cumprod_prev) * np.sqrt(alphas) / (1. - alphas_cumprod)), **nonp)
+        # the loss weights of p_losses (ddpm.py:158-169, 87-89), formed in fp32 from the fp32 buffers as the reference
+        # does; neither is in a checkpoint
+        lvlb_weights = self.betas ** 2 / (2 * self.posterior_variance * to_torch(alphas) * (1 - self.alphas_cumprod))
+        lvlb_weights[0] = lvlb_weights[1]
+        self.register_buffer("lvlb_weights", lvlb_weights, **nonp)
+        self.register_buffer("logvar", torch.full(fill_value=self.logvar_init, size=(self.num_timesteps,)),
+                             **nonp)
 
     @property
     def device(self):
@@ -364,6 +384,139 @@ class LatentDiffusion(nn.Module):
         a = float(self.sqrt_alphas_cumprod[int(t_host[0])])
         s = float(self.sqrt_one_minus_alphas_cumprod[int(t_host[0])])
         return ops.axpby2(x_start.contiguous().float(), noise.contiguous().float(), a, s)
+
+    def _q_sample_per_sample(self, x_start, t, noise):
+        """q_sample at one timestep per sample: the uniform-t route of q_sample when every t is equal (so the result
+        does not depend on which route ran), sdb_q_sample_t otherwise."""
+        t = t.to(self.device, torch.long).reshape(-1).contiguous()
+        t_host = t.cpu()
+        if bool((t_host == t_host[0]).all()):
+            if not 0 <= int(t_host[0]) < self.num_timesteps:
+                raise IndexError(f"timesteps must lie in [0, {self.num_timesteps}), got {int(t_host[0])}")
+            return self.q_sample(x_start, t_host, noise)
+        return ops.q_sample_t(x_start.contiguous().float(), noise.contiguous().float(), t,
+                              self.sqrt_alphas_cumprod, self.sqrt_one_minus_alphas_cumprod)
+
+    # -- denoising objective, forward only (ddpm.py:279-293, 654-705, 865-880, 1012-1045, 358-364)
+    def get_loss(self, pred, target, mean=True):
+        """get_loss (ddpm.py:279-293) with mean=True: the l1 / l2 mean over every element, from the per-sample means
+        of sdb_diffusion_loss (every sample has the same size, so their mean is the overall mean). The elementwise form
+        (mean=False) is not materialized: p_losses reduces per sample inside the kernel."""
+        if not mean:
+            raise NotImplementedError("get_loss(mean=False): elementwise losses are not materialized; p_losses reduces "
+                                      "them per sample with sdb_diffusion_loss")
+        t = torch.zeros(pred.shape[0], dtype=torch.long, device=pred.device)
+        per = ops.diffusion_loss(pred.contiguous().float(), target.contiguous().float(), self.loss_type, t,
+                                 self.logvar, self.lvlb_weights)
+        return per[0].cpu().double().mean().float()
+
+    def p_losses(self, x_start, cond, t, noise=None):
+        """ddpm.py:1012-1045: noise x_start to t (one timestep per sample), predict eps with apply_model, and reduce.
+        Returns (loss, loss_dict) with the reference's keys under train/ or val/ (from self.training); the values are
+        0-d fp32 CPU tensors, the batch means formed on the host in the reference's order."""
+        x_start = x_start.to(self.device).contiguous().float()
+        if noise is None:
+            noise = torch.randn_like(x_start)
+        noise = noise.to(self.device).contiguous().float()
+        t = t.to(self.device, torch.long).reshape(-1).contiguous()
+        x_noisy = self._q_sample_per_sample(x_start, t, noise)
+        model_output = self.apply_model(x_noisy, t, cond)
+        per = ops.diffusion_loss(model_output.contiguous().float(), noise, self.loss_type, t, self.logvar,
+                                 self.lvlb_weights).cpu()
+        prefix = "train" if self.training else "val"
+        loss_simple, loss, loss_vlb = per[0], per[1], per[2]
+        loss_dict = {f"{prefix}/loss_simple": loss_simple.mean()}
+        loss = self.l_simple_weight * loss.mean()
+        loss_vlb = loss_vlb.mean()
+        loss_dict[f"{prefix}/loss_vlb"] = loss_vlb
+        loss = loss + self.original_elbo_weight * loss_vlb
+        loss_dict[f"{prefix}/loss"] = loss
+        return loss, loss_dict
+
+    def forward(self, x, c, *args, **kwargs):
+        """ddpm.py:870-879: a uniformly drawn timestep per sample, then p_losses."""
+        t = torch.randint(0, self.num_timesteps, (x.shape[0],), device=self.device).long()
+        if self.model.conditioning_key is not None:
+            assert c is not None
+            if self.cond_stage_trainable:
+                c = self.get_learned_conditioning(c)
+        return self.p_losses(x, c, t, *args, **kwargs)
+
+    @staticmethod
+    def _batch_image(batch, k):
+        """DDPM.get_input (ddpm.py:329-335): a [B, H, W(, C)] tensor to NCHW fp32."""
+        x = batch[k]
+        if not torch.is_tensor(x):
+            raise TypeError(f"get_input: batch[{k!r}] must be a [B, H, W, C] tensor, got {type(x).__name__}")
+        if x.dim() == 3:
+            x = x[..., None]
+        return x.permute(0, 3, 1, 2).contiguous().float()
+
+    @torch.no_grad()
+    def get_input(self, batch, k, return_first_stage_outputs=False, force_c_encode=False, cond_key=None,
+                  return_original_cond=False, bs=None):
+        """ddpm.py:654-705: encode batch[k] ([B, H, W, C] in [-1, 1]) with the first stage (a KL posterior is sampled
+        with noise drawn on the CPU generator, as the reference does) and build the conditioning from the batch:
+        `caption` (a list of strings, tokenized by the cond stage), `class_label` (the whole batch goes to
+        ClassEmbedder) or an image-like key such as `segmentation` or `LR_image`. Returns [z, c] (+ [x, xrec] + [xc])."""
+        conditional = self.model.conditioning_key is not None
+        cond_key = self.cond_stage_key if cond_key is None else cond_key
+        if conditional and cond_key in ("txt", "coordinates_bbox", "nix"):
+            raise NotImplementedError(f"get_input: cond_stage_key {cond_key!r} has no conditioning path in the "
+                                      "reference's get_input (ddpm.py:664-672)")
+        if conditional and cond_key == "masked_image":
+            raise NotImplementedError(
+                "get_input: 'masked_image' conditioning is built by scripts/inpaint.py (masked image encoded by the "
+                "first stage, concatenated with the downsampled mask); pass that conditioning to p_losses instead")
+        x = self._batch_image(batch, k)
+        if bs is not None:
+            x = x[:bs]
+        x = x.to(self.device)
+        z = self.get_first_stage_encoding(self.encode_first_stage(x))
+        xc = c = None
+        if conditional:
+            if cond_key != self.first_stage_key:
+                if cond_key == "caption":
+                    xc = batch[cond_key]
+                elif cond_key == "class_label":
+                    xc = batch
+                else:
+                    xc = self._batch_image(batch, cond_key).to(self.device)
+            else:
+                xc = x
+            if not self.cond_stage_trainable or force_c_encode:
+                c = self.get_learned_conditioning(xc)
+            else:
+                c = xc
+            if bs is not None:
+                c = c[:bs]
+        out = [z, c]
+        if return_first_stage_outputs:
+            out.extend([x, self.decode_first_stage(z)])
+        if return_original_cond:
+            out.append(xc)
+        return out
+
+    @torch.no_grad()
+    def shared_step(self, batch, **kwargs):
+        x, c = self.get_input(batch, self.first_stage_key)
+        return self(x, c)
+
+    @torch.no_grad()
+    def validation_step(self, batch, batch_idx):
+        """ddpm.py:358-364 without the logger: the raw weights' loss_dict merged with the EMA weights' (keys + '_ema'),
+        each from its own shared_step (its own t, noise and posterior sample). Runs in eval mode, so the keys carry
+        the val/ prefix as under Lightning's validation loop."""
+        was_training = self.training
+        self.eval()
+        try:
+            _, loss_dict_no_ema = self.shared_step(batch)
+            with self.ema_scope():
+                _, loss_dict_ema = self.shared_step(batch)
+                loss_dict_ema = {key + "_ema": loss_dict_ema[key] for key in loss_dict_ema}
+        finally:
+            self.train(was_training)
+        return {**loss_dict_no_ema, **loss_dict_ema}
 
     # -- ancestral sampler (ddpm.py:1047-1213), unconditional models
     def _p_step(self, img, t, noise):

@@ -145,6 +145,12 @@ SIGNATURES = {
     "sdb_sample_plms": ([C.POINTER(PlmsDesc), _P], C.c_int),
 }
 
+# name -> argtypes of the evaluation entry points declared in include/sdb200_eval.h (tests check both ways).
+EVAL_SIGNATURES = {
+    "sdb_q_sample_t": ([_P, _P, _P, _P, _P, _I, _L, _P, _P], C.c_int),
+    "sdb_diffusion_loss": ([_P, _P, _I, _P, _P, _P, _I, _L, _P, _P], C.c_int),
+}
+
 _lib = None
 
 
@@ -157,7 +163,7 @@ def load() -> C.CDLL:
                 f"{_LIB_PATH} is missing: build it with `python stable-diffusion_b200/build.py` "
                 "(there is no CPU or PyTorch fallback for the sdb200 kernels)")
         lib = C.CDLL(str(_LIB_PATH))
-        for name, (argtypes, restype) in SIGNATURES.items():
+        for name, (argtypes, restype) in {**SIGNATURES, **EVAL_SIGNATURES}.items():
             fn = getattr(lib, name)
             fn.argtypes = argtypes
             fn.restype = restype

@@ -850,6 +850,54 @@ def mask_blend(img_orig, mask, img, b, dup=False):
     return img
 
 
+LOSS_KINDS = {"l1": 1, "l2": 2}
+
+
+def _check_t(t, nb, num_timesteps):
+    assert t.dtype == torch.int64 and t.is_cuda and t.is_contiguous() and t.shape == (nb,), \
+        f"t: need contiguous cuda int64 [{nb}], got {t.dtype} {tuple(t.shape)} on {t.device}"
+    lo, hi = (int(v) for v in torch.stack([t.min(), t.max()]).cpu())
+    if lo < 0 or hi >= num_timesteps:
+        raise IndexError(f"timesteps must lie in [0, {num_timesteps}), got min {lo} and max {hi}")
+
+
+def q_sample_t(x0, noise, t, sqrt_ac, sqrt_1m_ac):
+    """sqrt_ac[t_b] * x0 + sqrt_1m_ac[t_b] * noise with one int64 timestep per sample (sdb_q_sample_t). Raises
+    IndexError, before any launch, when a t lies outside the schedule."""
+    _chk32(x0, "x0")
+    _chk32(noise, "noise")
+    _chk32(sqrt_ac, "sqrt_ac")
+    _chk32(sqrt_1m_ac, "sqrt_1m_ac")
+    assert noise.shape == x0.shape and sqrt_ac.shape == sqrt_1m_ac.shape and sqrt_ac.dim() == 1
+    nb = x0.shape[0]
+    _check_t(t, nb, sqrt_ac.numel())
+    out = torch.empty_like(x0)
+    _l.check(_l.load().sdb_q_sample_t(_ptr(x0), _ptr(noise), _ptr(t), _ptr(sqrt_ac), _ptr(sqrt_1m_ac), nb,
+                                      x0[0].numel(), _ptr(out), _stream()), "sdb_q_sample_t")
+    _count()
+    return out
+
+
+def diffusion_loss(pred, target, kind, t, logvar, lvlb_weights):
+    """Per-sample (loss_simple, loss, loss_vlb) of p_losses before the batch means (sdb_diffusion_loss): fp32 [3, nb].
+    kind is "l1" or "l2". Raises IndexError, before any launch, when a t lies outside the tables."""
+    _chk32(pred, "pred")
+    _chk32(target, "target")
+    _chk32(logvar, "logvar")
+    _chk32(lvlb_weights, "lvlb_weights")
+    assert pred.shape == target.shape and logvar.shape == lvlb_weights.shape and logvar.dim() == 1
+    if kind not in LOSS_KINDS:
+        raise NotImplementedError(f"unknown loss type '{kind}'")
+    nb = pred.shape[0]
+    _check_t(t, nb, logvar.numel())
+    out = torch.empty((3, nb), dtype=torch.float32, device=pred.device)
+    _l.check(_l.load().sdb_diffusion_loss(_ptr(pred), _ptr(target), LOSS_KINDS[kind], _ptr(t), _ptr(logvar),
+                                          _ptr(lvlb_weights), nb, pred[0].numel(), _ptr(out), _stream()),
+             "sdb_diffusion_loss")
+    _count()
+    return out
+
+
 def axpby2(x, y, a, b):
     _chk32(x, "x")
     _chk32(y, "y")
