@@ -7,7 +7,8 @@ __version__ = "0.1.0"
 
 import sys as _sys
 
-from . import arch, bert, checkpoint, clip, clip_image, diffusion, dist, encoders, lib, ops, pipeline, retrieval, safety, samplers, tokenizer, unet, util, vae, vq  # noqa: E402,F401
+from . import ae_loss, arch, bert, checkpoint, clip, clip_image, diffusion, dist, encoders, lib, ops, pipeline, retrieval, safety, samplers, tokenizer, unet, util, vae, vq  # noqa: E402,F401
+from .ae_loss import LPIPS, LPIPSWithDiscriminator, NLayerDiscriminator  # noqa: E402,F401
 from .bert import BERTEmbedder  # noqa: E402,F401
 from .clip import FrozenCLIPEmbedder, FrozenCLIPTextEmbedder  # noqa: E402,F401
 from .clip_image import FrozenClipImageEmbedder  # noqa: E402,F401

@@ -145,4 +145,29 @@ def load_model_from_config(config, ckpt, device="cuda", verbose=False, allow_pic
         model = model.to(device)
     model.eval()
     model.load_info = {"missing": list(m), "unexpected": list(u), **info}
+    if "global_step" in info and hasattr(model, "global_step"):
+        model.global_step = int(info["global_step"])
     return model
+
+
+def load_first_stage_loss(model, config, ckpt, device="cuda", allow_pickle=False):
+    """Build the training loss of a KL first stage from its YAML's `lossconfig` (ldm.modules.losses.
+    LPIPSWithDiscriminator -> sdb200.ae_loss.LPIPSWithDiscriminator), load it from the checkpoint's `loss.*` tensors and
+    attach it to `model` (an AutoencoderKL from load_model_from_config) for validation_step. A checkpoint without those
+    tensors leaves the loss unloaded (`load_info["missing"]`), and validation_step then raises naming them. Returns the
+    loss stage, in eval mode on `device`."""
+    node = load_config(config)
+    lc = node.get("params", {}).get("lossconfig")
+    if not lc or "target" not in lc:
+        raise KeyError(f"{node.get('target')}: the config has no lossconfig")
+    loss = instantiate_from_config(remap_config(lc))
+    sd, info = read_state_dict(ckpt, allow_pickle=allow_pickle)
+    m, u = loss.load_state_dict({k[len("loss."):]: v for k, v in sd.items() if k.startswith("loss.")}, strict=False)
+    if device is not None:
+        loss = loss.to(device)
+    loss.eval()
+    loss.load_info = {"missing": ["loss." + k for k in m], "unexpected": ["loss." + k for k in u]}
+    object.__setattr__(model, "loss", loss)    # not a submodule: the autoencoder's state dict is unchanged
+    if "global_step" in info:
+        model.global_step = int(info["global_step"])
+    return loss

@@ -120,6 +120,13 @@ __device__ __forceinline__ float apply_act(float x, int act) {
   if (act == SDB_ACT_GELU) return gelu_erf(x);
   return x;
 }
+// The activation of an epilogue of kind KIND: kind 4 carries only the ReLU family (SDB_ACT_RELU, SDB_ACT_LEAKY_RELU),
+// so the other kinds compile exactly the code they had before it existed.
+template <int KIND>
+__device__ __forceinline__ float epi_act(float x, int act) {
+  if (KIND == 4) return act == SDB_ACT_RELU ? fmaxf(x, 0.0f) : (x > 0.0f ? x : 0.2f * x);
+  return apply_act(x, act);
+}
 
 // Output row of accumulator row r of tile m_tile. 3x3 geometry: a tile is TW x TH x TN output pixels (powers of two, so
 // the row decomposes with shifts); its origin (TileGeo) costs three integer divisions and is computed once per tile.
@@ -156,11 +163,12 @@ __device__ __forceinline__ bool map_row(const GemmArgs& p, int m_tile, int r, in
 }
 
 // One element of the fused epilogue (after alpha/bias which are column-only).
+template <int KIND = 2>
 __device__ __forceinline__ void store_elem(const GemmArgs& p, float x, int orow, int sample, int col, bool finish) {
   if (finish) {
     if (p.film) x += p.film[static_cast<size_t>(sample) * p.ldf + col];
     if (p.residual) x += p.residual[static_cast<size_t>(orow) * p.ldr + col];
-    x = apply_act(x, p.act);
+    x = epi_act<KIND>(x, p.act);
   }
   size_t o = static_cast<size_t>(orow) * p.ldo + col;
   if (p.out_f32) p.out_f32[o] = x;
@@ -175,6 +183,7 @@ __device__ __forceinline__ void store_elem(const GemmArgs& p, float x, int orow,
 // global memory with row-contiguous accesses: 16 lanes x 2 columns per row, two rows per instruction.
 //   mode 0: fused epilogue (alpha, bias, FiLM, residual, activation)   mode 1: raw split-K partial   mode 2: values
 //   already final (GEGLU computed in row layout)
+template <int KIND = 2>
 __device__ __forceinline__ void drain_chunk(const GemmArgs& p, const float* stage, int lane, int my_row, int my_sample,
                                             bool my_valid, int ocol0, int ncols, int mode, int split) {
   const int l16 = lane & 15, rsel = lane >> 4;
@@ -210,8 +219,8 @@ __device__ __forceinline__ void drain_chunk(const GemmArgs& p, const float* stag
       x1 = x1 * p.alpha + b1;
     }
     if (!vec) {
-      store_elem(p, x0, orow, sample, col, mode == 0);
-      if (c1) store_elem(p, x1, orow, sample, col + 1, mode == 0);
+      store_elem<KIND>(p, x0, orow, sample, col, mode == 0);
+      if (c1) store_elem<KIND>(p, x1, orow, sample, col + 1, mode == 0);
       continue;
     }
     if (mode == 0) {
@@ -225,8 +234,8 @@ __device__ __forceinline__ void drain_chunk(const GemmArgs& p, const float* stag
         x0 += rv.x;
         x1 += rv.y;
       }
-      x0 = apply_act(x0, p.act);
-      x1 = apply_act(x1, p.act);
+      x0 = epi_act<KIND>(x0, p.act);
+      x1 = epi_act<KIND>(x1, p.act);
     }
     const size_t o = static_cast<size_t>(orow) * p.ldo + col;
     if (p.out_f32) *reinterpret_cast<float2*>(p.out_f32 + o) = make_float2(x0, x1);
@@ -285,16 +294,19 @@ struct EpiRows {   // the output rows one epilogue warp handles: row per lane + 
 //   1 geglu  : GEGLU with fp16 output only (the feed-forward up-projection)
 //   2 general: everything (activations, scalar-store epilogue for odd widths, per-row FiLM, fp32 + fp16 hi/lo outputs)
 //   3 lean + cluster split-K (kind 0 is compiled without the cluster exchange, kind 3 without the single-CTA epilogue)
+//   4 general with the ReLU family instead of the other activations (SDB_ACT_RELU / SDB_ACT_LEAKY_RELU; never split:
+//     the split-K second pass applies kind 2's activations only)
 template <int BN, int CG, int KIND>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_constant__ TmapPack tm, const GemmArgs p) {
   // compile-time specialisation of the descriptor fields the KIND fixes (dead branches fold away)
   const int act = (KIND == 0 || KIND == 3) ? SDB_ACT_NONE : (KIND == 1 ? SDB_ACT_GEGLU : p.act);
-  const bool fast = KIND == 2 ? (p.fast != 0) : true;
-  const bool film_row = KIND == 2 && p.film && !p.film_table;
+  const bool fast = (KIND == 2 || KIND == 4) ? (p.fast != 0) : true;
+  const bool film_row = (KIND == 2 || KIND == 4) && p.film && !p.film_table;
   // debug hooks (phase stamps, SDB_DBG switches) exist only in a -DSDB_TRACE build (SDB_BUILD_TRACE=1 python build.py)
   const int dbg = SDB_TRACE_ENABLED ? p.dbg : 0;
   unsigned long long* const trace = SDB_TRACE_ENABLED ? p.trace : nullptr;
-  const int csk = KIND == 0 ? 0 : (KIND == 3 ? 1 : p.csk);   // lean kinds: 0 = no cluster split-K, 3 = cluster split-K
+  // lean kinds: 0 = no cluster split-K, 3 = cluster split-K; kind 4 never splits
+  const int csk = (KIND == 0 || KIND == 4) ? 0 : (KIND == 3 ? 1 : p.csk);
   using Cfg = GemmCfg<BN, CG>;
   constexpr int STAGES = Cfg::STAGES;
   constexpr int B_ROWS = Cfg::B_ROWS;
@@ -381,7 +393,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
   const int par = warp & 1;      // the two warps of a lane group alternate chunks
   const int et = threadIdx.x;
   uint8_t* stg = staging + ew * STG_WARP_BYTES;
-  const bool geglu = (KIND == 0 || KIND == 3) ? false : (KIND == 1 ? true : ((p.act == SDB_ACT_GEGLU) && !p.ws));
+  const bool geglu = (KIND == 0 || KIND == 3 || KIND == 4) ? false : (KIND == 1 ? true : ((p.act == SDB_ACT_GEGLU) && !p.ws));
   constexpr int HALF = BN / 2;
   const int n_chunks = geglu ? HALF / 32 : BN / 32;
   const int n_lim = geglu ? p.N / 2 : p.N;   // output columns that exist
@@ -492,7 +504,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
       }
       if (act != SDB_ACT_NONE) {
 #pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = apply_act(v[j], act);
+        for (int j = 0; j < 32; ++j) v[j] = epi_act<KIND>(v[j], act);
       }
     }
     if (tr_chunk) SDB_TR(4, clock64() - clk0);
@@ -932,7 +944,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
 #pragma unroll
             for (int j = 0; j < 32; ++j) stage[lane * 33 + j] = v[j];
             __syncwarp();
-            drain_chunk(p, stage, lane, rw.row, rw.sample, rw.valid, ocol0, geglu ? p.N / 2 : p.N,
+            drain_chunk<KIND>(p, stage, lane, rw.row, rw.sample, rw.valid, ocol0, geglu ? p.N / 2 : p.N,
                         geglu ? 2 : (p.ws ? 1 : 0), split);
             __syncwarp();
             continue;
@@ -1128,7 +1140,7 @@ static int launch_gemm(const TmapPack& tm, const GemmArgs& p, cudaStream_t st) {
   return 0;
 }
 
-// all tile shapes of one KIND (one translation unit per KIND: gemm_k0.cu, gemm_k1.cu, gemm_k2.cu)
+// all tile shapes of one KIND (one translation unit per KIND: gemm_k0.cu .. gemm_k4.cu)
 template <int KIND>
 static int launch_gemm_kind(int bn, int cg, const TmapPack& tm, const GemmArgs& p, cudaStream_t st) {
   if (cg == 2) {
@@ -1162,5 +1174,6 @@ int launch_gemm_kind0(int bn, int cg, const TmapPack& tm, const GemmArgs& p, cud
 int launch_gemm_kind1(int bn, int cg, const TmapPack& tm, const GemmArgs& p, cudaStream_t st);
 int launch_gemm_kind2(int bn, int cg, const TmapPack& tm, const GemmArgs& p, cudaStream_t st);
 int launch_gemm_kind3(int bn, int cg, const TmapPack& tm, const GemmArgs& p, cudaStream_t st);
+int launch_gemm_kind4(int bn, int cg, const TmapPack& tm, const GemmArgs& p, cudaStream_t st);
 
 }  // namespace sdb

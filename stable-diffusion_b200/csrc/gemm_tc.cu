@@ -100,8 +100,11 @@ static double choice_cost(const sdb_gemm_desc* d, const Geometry& g, const Choic
   return t;
 }
 
+static bool relu_family(int act) { return act == SDB_ACT_RELU || act == SDB_ACT_LEAKY_RELU; }
+
 static int make_geometry(const sdb_gemm_desc* d, Geometry* g) {
-  SDB_CHECK(d->act >= SDB_ACT_NONE && d->act <= SDB_ACT_GELU, "sdb_gemm: unknown activation %d", d->act);
+  SDB_CHECK((d->act >= SDB_ACT_NONE && d->act <= SDB_ACT_GELU) || relu_family(d->act), "sdb_gemm: unknown activation %d",
+            d->act);
   const void* srcs[MAX_SRC] = {d->a0, d->a1, d->a2, d->a3};
   const int chans[MAX_SRC] = {d->c0, d->c1, d->c2, d->c3};
   int nsrc = 0, chunks = 0;
@@ -158,6 +161,7 @@ static int resolve_choice(const sdb_gemm_desc* d, const Geometry& g, Choice* out
   const int bns[] = {256, 160, 128, 64, 32};
   const int sps[] = {1, 2, 3, 4, 6, 8, 12, 16, 24, 32};
   int want_splits = d->splits;                      // >1 explicit, 0/1 none, -1 auto
+  if (relu_family(d->act)) want_splits = 1;         // kind 4 runs unsplit (the split-K second pass has no ReLU)
   if (want_splits > g.k_iters) want_splits = g.k_iters;
   Choice best{0, 1, 1, 0};
   double best_t = 1e300;
@@ -420,13 +424,14 @@ extern "C" int sdb_gemm(const sdb_gemm_desc* d, sdb_stream_t stream) {
   }
 
   // epilogue kind: the lean and GEGLU instantiations carry only the code their launches execute
-  int kind = 2;
+  int kind = relu_family(d->act) ? 4 : 2;
   if (p.fast && d->act == SDB_ACT_GEGLU && !p.out_f32 && !p.out_f16_lo && !p.ws) kind = 1;
   else if (p.fast && d->act == SDB_ACT_NONE && (!p.film || p.film_table) && !(p.out_f32 && p.out_f16 && p.out_f16_lo)) kind = 0;
   if (kind == 0 && p.csk) kind = 3;
   int rc = kind == 0   ? launch_gemm_kind0(bn, ch.cg, tm, p, st)
            : kind == 1 ? launch_gemm_kind1(bn, ch.cg, tm, p, st)
            : kind == 3 ? launch_gemm_kind3(bn, ch.cg, tm, p, st)
+           : kind == 4 ? launch_gemm_kind4(bn, ch.cg, tm, p, st)
                        : launch_gemm_kind2(bn, ch.cg, tm, p, st);
   if (rc) return rc;
   if (splits > 1 && !p.csk) {

@@ -11,6 +11,7 @@ from pathlib import Path
 _LIB_PATH = Path(__file__).resolve().parent / "csrc" / "libsdb200.so"
 
 ACT_NONE, ACT_GEGLU, ACT_QUICK_GELU, ACT_SILU, ACT_GELU = 0, 1, 2, 3, 4
+ACT_RELU, ACT_LEAKY_RELU = 6, 7   # 5 is not an activation (sdb_gemm rejects it)
 
 
 class GemmDesc(C.Structure):
@@ -151,6 +152,16 @@ EVAL_SIGNATURES = {
     "sdb_diffusion_loss": ([_P, _P, _I, _P, _P, _P, _I, _L, _P, _P], C.c_int),
 }
 
+# name -> argtypes of the first-stage loss entry points declared in include/sdb200_ae_loss.h (tests check both ways).
+AE_LOSS_SIGNATURES = {
+    "sdb_lpips_scale": ([_P, _P, _I, _I, _I, _P, _P, _P, _P], C.c_int),
+    "sdb_maxpool2x2": ([_P, _I, _I, _I, _I, _P, _P], C.c_int),
+    "sdb_lpips_head_work": ([_I, _I], C.c_int64),
+    "sdb_lpips_head": ([_P, _I, _I, _I, _P, _I, _P, _P, _P, _P], C.c_int),
+    "sdb_im2col": ([_P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P], C.c_int),
+    "sdb_ae_loss_terms": ([_P, _P, _I, _I, _L, _I, _P, _P], C.c_int),
+}
+
 _lib = None
 
 
@@ -163,7 +174,7 @@ def load() -> C.CDLL:
                 f"{_LIB_PATH} is missing: build it with `python stable-diffusion_b200/build.py` "
                 "(there is no CPU or PyTorch fallback for the sdb200 kernels)")
         lib = C.CDLL(str(_LIB_PATH))
-        for name, (argtypes, restype) in {**SIGNATURES, **EVAL_SIGNATURES}.items():
+        for name, (argtypes, restype) in {**SIGNATURES, **EVAL_SIGNATURES, **AE_LOSS_SIGNATURES}.items():
             fn = getattr(lib, name)
             fn.argtypes = argtypes
             fn.restype = restype

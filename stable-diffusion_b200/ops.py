@@ -11,7 +11,7 @@ import ctypes as C
 import torch
 
 from . import lib as _l
-from .lib import ACT_GEGLU, ACT_GELU, ACT_NONE, ACT_QUICK_GELU, ACT_SILU, AttnDesc, GemmDesc  # noqa: F401
+from .lib import ACT_GEGLU, ACT_GELU, ACT_LEAKY_RELU, ACT_NONE, ACT_QUICK_GELU, ACT_RELU, ACT_SILU, AttnDesc, GemmDesc  # noqa: F401
 
 LAUNCHES = 0        # op calls made through this module
 _GRAPH_LAUNCHES = 0  # kernels replayed from CUDA graphs (counted at capture time, added per replay)
@@ -960,5 +960,89 @@ def embed_tokens(ids, tok, pos):
     out = torch.empty((B * n, dim), dtype=torch.float32, device=ids.device)
     _l.check(_l.load().sdb_embed_tokens(_ptr(ids), B * n, n, dim, tok.shape[0], _ptr(tok), _ptr(pos), _ptr(out),
                                         _stream()), "sdb_embed_tokens")
+    _count()
+    return out
+
+
+# ---- first-stage loss (include/sdb200_ae_loss.h) ----
+def lpips_scale(in0, in1, shift, scale):
+    """LPIPS ScalingLayer of both NCHW fp32 [nb, 3, h, w] inputs -> NHWC fp32 [2 * nb, h, w, 3] (in0's images first)."""
+    _chk32(in0, "in0")
+    _chk32(in1, "in1")
+    _chk32(shift, "shift")
+    _chk32(scale, "scale")
+    assert in0.dim() == 4 and in0.shape[1] == 3 and in1.shape == in0.shape, (tuple(in0.shape), tuple(in1.shape))
+    assert shift.numel() == 3 and scale.numel() == 3
+    nb, _, h, w = in0.shape
+    out = torch.empty((2 * nb, h, w, 3), dtype=torch.float32, device=in0.device)
+    _l.check(_l.load().sdb_lpips_scale(_ptr(in0), _ptr(in1), nb, h, w, _ptr(shift), _ptr(scale), _ptr(out), _stream()),
+             "sdb_lpips_scale")
+    _count()
+    return out
+
+
+def maxpool2x2(x):
+    """MaxPool2d(2, 2) of NHWC fp16 [nb, h, w, c] -> [nb, h // 2, w // 2, c]."""
+    _chk16(x, "x")
+    nb, h, w, c = x.shape
+    out = torch.empty((nb, h // 2, w // 2, c), dtype=torch.float16, device=x.device)
+    _l.check(_l.load().sdb_maxpool2x2(_ptr(x), nb, h, w, c, _ptr(out), _stream()), "sdb_maxpool2x2")
+    _count()
+    return out
+
+
+def lpips_head(f, lin_w, acc, first, out=None):
+    """One LPIPS layer of the feature pair f fp16 [2 * nb, h, w, c] (in0's samples first), accumulated into the fp64
+    per-sample acc [nb] (overwritten when first); out fp32 [nb], when given, receives acc rounded to fp32."""
+    _chk16(f, "f")
+    _chk32(lin_w, "lin_w")
+    n2, h, w, c = f.shape
+    nb = n2 // 2
+    assert n2 == 2 * nb and lin_w.numel() == c and acc.dtype == torch.float64 and acc.shape == (nb,) and acc.is_cuda
+    if out is not None:
+        _chk32(out, "out")
+        assert out.numel() == nb
+    lib = _l.load()
+    work = torch.empty(int(lib.sdb_lpips_head_work(nb, h * w)), dtype=torch.float64, device=f.device)
+    _l.check(lib.sdb_lpips_head(_ptr(f), nb, h * w, c, _ptr(lin_w), 1 if first else 0, _ptr(work), _ptr(acc),
+                                _ptr(out), _stream()), "sdb_lpips_head")
+    _count(2)
+    return acc
+
+
+def im2col(x, k, stride, pad, kpad):
+    """k x k patches of NHWC fp16 [nb, h, w, c] -> fp16 [nb * ho * wo, kpad], column (ky * k + kx) * c + ch."""
+    _chk16(x, "x")
+    nb, h, w, c = x.shape
+    ho, wo = (h + 2 * pad - k) // stride + 1, (w + 2 * pad - k) // stride + 1
+    assert ho > 0 and wo > 0, f"im2col: a {k}x{k} / stride {stride} / pad {pad} conv leaves no pixel of {h}x{w}"
+    out = torch.empty((nb * ho * wo, kpad), dtype=torch.float16, device=x.device)
+    _l.check(_l.load().sdb_im2col(_ptr(x), nb, h, w, c, k, stride, pad, ho, wo, kpad, _ptr(out), _stream()),
+             "sdb_im2col")
+    _count()
+    return out, ho, wo
+
+
+AE_TERM_KINDS = {"abs": 1, "kl": 2, "logits": 3}
+
+
+def ae_loss_terms(a, kind, b=None, n=None, cc=1):
+    """Per-sample fp64 sums of sdb_ae_loss_terms: "abs" sum |a - b| of fp32 [nb, ...] pairs -> [1, nb]; "kl" the
+    posterior KL of NHWC moments a fp32 [nb, h, w, 2 * cc] -> [1, nb]; "logits" the five logit sums of column 0 of a
+    fp32 [nb * n, cc] -> [5, nb]."""
+    _chk32(a, "a")
+    k = AE_TERM_KINDS[kind]
+    if k == 1:
+        _chk32(b, "b")
+        assert b.shape == a.shape
+        nb, n = a.shape[0], a[0].numel()
+    elif k == 2:
+        nb, n = a.shape[0], a[0].numel() // 2
+        assert a.shape[-1] == 2 * cc
+    else:
+        nb = a.shape[0] // n
+        assert a.dim() == 2 and a.shape == (nb * n, cc)
+    out = torch.empty((5 if k == 3 else 1, nb), dtype=torch.float64, device=a.device)
+    _l.check(_l.load().sdb_ae_loss_terms(_ptr(a), _ptr(b), k, nb, n, cc, _ptr(out), _stream()), "sdb_ae_loss_terms")
     _count()
     return out

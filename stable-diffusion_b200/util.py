@@ -35,6 +35,8 @@ TARGET_MAP = {
     "ldm.modules.encoders.modules.ClassEmbedder": "sdb200.encoders.ClassEmbedder",
     "ldm.modules.encoders.modules.BERTEmbedder": "sdb200.bert.BERTEmbedder",
     "ldm.modules.encoders.modules.SpatialRescaler": "sdb200.encoders.SpatialRescaler",
+    "ldm.modules.losses.LPIPSWithDiscriminator": "sdb200.ae_loss.LPIPSWithDiscriminator",
+    "ldm.modules.losses.contperceptual.LPIPSWithDiscriminator": "sdb200.ae_loss.LPIPSWithDiscriminator",
 }
 
 

@@ -53,6 +53,15 @@ class DiagonalGaussianDistribution:
     def mode(self):
         return self.mean
 
+    def kl_sums(self):
+        """Per-sample KL against N(0, I), fp64 [nb] on the device (sdb_ae_loss_terms, fixed summation order)."""
+        return ops.ae_loss_terms(self._m.view(self.nb, self.h, self.w, 2 * self.zc), "kl", cc=self.zc)[0]
+
+    def kl(self):
+        """distributions.py:38-45 with other=None: 0.5 * sum(mean^2 + var - 1 - logvar) over [C, H, W], fp32 [nb]; any
+        latent width."""
+        return self.kl_sums().float()
+
 
 class ConvAutoencoder(PackedStage):
     """The Encoder / Decoder of model.py:368-568 (attention in the mid block, and inside the levels at attn_resolutions)
@@ -249,6 +258,12 @@ class ConvAutoencoder(PackedStage):
 
 
 class AutoencoderKL(ConvAutoencoder):
+    # training step of the checkpoint (checkpoint.load_model_from_config sets it); decides the loss's disc_factor
+    global_step = 0
+    # the training loss (ae_loss.LPIPSWithDiscriminator), attached by checkpoint.load_first_stage_loss as a stage of its
+    # own: it is not a submodule, so the autoencoder's state dict and key reporting stay as they are
+    loss = None
+
     def __init__(self, ddconfig, lossconfig=None, embed_dim=4, ckpt_path=None, ignore_keys=(), image_key="image",
                  colorize_nlabels=None, monitor=None):
         assert ddconfig["double_z"], "AutoencoderKL needs double_z"
@@ -261,6 +276,7 @@ class AutoencoderKL(ConvAutoencoder):
         super().__init__(vae_param_shapes(cfg))
         self.cfg = cfg
         self.embed_dim = embed_dim
+        self.image_key = image_key
 
     # ------------------------------------------------------------------ public API
     @torch.no_grad()
@@ -292,3 +308,37 @@ class AutoencoderKL(ConvAutoencoder):
         posterior = self.encode(input)
         z = posterior.sample() if sample_posterior else posterior.mode()
         return self.decode(z), posterior
+
+    # ------------------------------------------------------------------ validation (autoencoder.py:364-395)
+    def get_input(self, batch, k):
+        """autoencoder.py:364-369: batch[k] NHWC (or NHW) -> NCHW fp32 on the stage's device."""
+        x = batch[k]
+        if len(x.shape) == 3:
+            x = x[..., None]
+        return x.permute(0, 3, 1, 2).to(device=self.W["device"], memory_format=torch.contiguous_format).float()
+
+    def get_last_layer(self):
+        return self._host_sd["decoder.conv_out.weight"]
+
+    @torch.no_grad()
+    def validation_step(self, batch, batch_idx):
+        """autoencoder.py:372-383: reconstruct through forward() (posterior sampled, 4-channel latents only), then both
+        loss calls; returns the merged val/* dict. The discriminator's logits on the reconstructions are computed once
+        and serve both calls."""
+        loss = self.loss
+        if loss is None:
+            raise RuntimeError("AutoencoderKL.validation_step needs the loss stage: load it with "
+                               "sdb200.checkpoint.load_first_stage_loss(model, config, ckpt)")
+        missing = loss.missing_keys()
+        if missing:
+            raise RuntimeError(f"the checkpoint carries no loss.* tensors for {len(missing)} keys of the loss stage, "
+                               f"e.g. {['loss.' + k for k in missing[:4]]}")
+        inputs = self.get_input(batch, self.image_key)
+        loss._check(inputs, inputs, None, 1, None, None)
+        if loss.perceptual_weight > 0:
+            loss.perceptual_loss.check_inputs(inputs, inputs)
+        reconstructions, posterior = self(inputs)
+        t, x = loss.terms(inputs, reconstructions, posterior, ("abs", "fake", "real"))
+        _, log_ae = loss.combine(t, x, 0, self.global_step, split="val")
+        _, log_disc = loss.combine(t, x, 1, self.global_step, split="val")
+        return {**log_ae, **log_disc}
