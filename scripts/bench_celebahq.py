@@ -16,7 +16,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from sdb200 import arch, ops  # noqa: E402
+from sdb200 import ops, pipeline  # noqa: E402
 from sdb200.samplers import DDIMSampler  # noqa: E402
 from sdb200.util import instantiate_from_config, remap_config  # noqa: E402
 from measure import card, emit, event_ms, wall_s  # noqa: E402
@@ -53,10 +53,8 @@ def main():
     import sample_diffusion as S
     dev = torch.device("cuda")
     m = instantiate_from_config(remap_config(S.celebahq_config()))
+    m = pipeline.load_random_weights(m, dev, gen_device=dev).eval()
     u = m.model.diffusion_model
-    u.load_weights(arch.random_state_dict(u.shapes, 11, device=dev), dev)
-    m.first_stage_model.load_weights(arch.random_state_dict(m.first_stage_model.shapes, 12, device=dev), dev)
-    m = m.to(dev).eval()
     u.use_cuda_graph = True
     shape = [a.batch_size, 3, 64, 64]
     sampler = DDIMSampler(m)

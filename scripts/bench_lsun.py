@@ -12,7 +12,7 @@ import sys
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from sdb200 import arch  # noqa: E402
+from sdb200 import pipeline  # noqa: E402
 from sdb200.samplers import DDIMSampler  # noqa: E402
 from sdb200.util import instantiate_from_config, remap_config  # noqa: E402
 from measure import card, emit, event_ms, wall_s  # noqa: E402
@@ -30,10 +30,8 @@ def main():
     import sample_diffusion as S
     dev = torch.device("cuda")
     m = instantiate_from_config(remap_config(S.lsun_churches_config()))
+    m = pipeline.load_random_weights(m, dev, gen_device=dev).eval()
     u = m.model.diffusion_model
-    u.load_weights(arch.random_state_dict(u.shapes, 11, device=dev), dev)
-    m.first_stage_model.load_weights(arch.random_state_dict(m.first_stage_model.shapes, 12, device=dev), dev)
-    m = m.to(dev).eval()
     m.scale_factor.fill_(0.22)
     u.use_cuda_graph = True
     shape = [a.batch_size, 4, 32, 32]

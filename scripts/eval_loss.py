@@ -27,7 +27,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import sdb200  # noqa: E402
-from sdb200 import arch  # noqa: E402
+from sdb200 import pipeline  # noqa: E402
 from sdb200.util import instantiate_from_config, remap_config  # noqa: E402
 
 KEYS = ("loss_simple", "loss_vlb", "loss")
@@ -37,13 +37,7 @@ def load_model(opt, device):
     if opt.random_init:
         print("--random_init: seeded random-init weights")
         model = instantiate_from_config(remap_config(sdb200.checkpoint.load_config(opt.config)))
-        stages = [model.model.diffusion_model, model.first_stage_model]
-        if model.cond_stage_model is not model.first_stage_model:       # __is_first_stage__: one module, one set
-            stages.append(model.cond_stage_model)
-        for seed, stage in enumerate(stages, 11):
-            if getattr(stage, "shapes", None):                            # None / Identity hold no weights
-                stage.load_weights(arch.random_state_dict(stage.shapes, seed, device=device), device)
-        return model.to(device).eval()
+        return pipeline.load_random_weights(model, device, gen_device=device).eval()
     if not opt.ckpt or not os.path.exists(opt.ckpt):
         raise FileNotFoundError(f"checkpoint {opt.ckpt!r} does not exist (pass --ckpt, or --random_init)")
     return sdb200.checkpoint.load_model_from_config(opt.config, opt.ckpt, device=device)

@@ -22,7 +22,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import sdb200  # noqa: E402
-from sdb200 import arch, ops  # noqa: E402
+from sdb200 import arch, ops, pipeline  # noqa: E402
 from sdb200.samplers import DDIMSampler  # noqa: E402
 from sdb200.util import instantiate_from_config, remap_config  # noqa: E402
 
@@ -46,10 +46,7 @@ def load_model(ckpt=None, random_init=False, tiny=False, device="cuda"):
     node = inpaint_config(arch.TINY_INPAINT_UNET, arch.TINY_VQ_NOATTN) if tiny else inpaint_config()
     if not random_init:
         return sdb200.checkpoint.load_model_from_config({"model": node}, ckpt, device=dev)
-    model = instantiate_from_config(remap_config(node))
-    for stage, seed in ((model.model.diffusion_model, 11), (model.first_stage_model, 12)):
-        stage.load_weights(arch.random_state_dict(stage.shapes, seed, device=dev), dev)
-    return model.to(dev).eval()
+    return pipeline.load_random_weights(instantiate_from_config(remap_config(node)), dev, gen_device=dev).eval()
 
 
 def latent_size(model, h, w):

@@ -31,7 +31,7 @@ sys.path.insert(0, os.path.dirname(HERE))
 sys.path.insert(0, HERE)
 import sdb200  # noqa: E402
 from sample_imagenet import make_grid  # noqa: E402
-from sdb200 import arch  # noqa: E402
+from sdb200 import arch, pipeline  # noqa: E402
 from sdb200.retrieval import DATABASES, Searcher  # noqa: E402
 from sdb200.samplers import DDIMSampler, PLMSSampler  # noqa: E402
 from sdb200.util import instantiate_from_config, remap_config  # noqa: E402
@@ -57,10 +57,7 @@ def load_model(ckpt=None, random_init=False, tiny=False, device="cuda", unsafe_c
     node = rdm_config(arch.TINY_RDM_UNET, arch.TINY_KL_F16) if tiny else rdm_config()
     if not random_init:
         return sdb200.checkpoint.load_model_from_config({"model": node}, ckpt, device=dev, allow_pickle=unsafe_ckpt)
-    model = instantiate_from_config(remap_config(node))
-    for stage, seed in ((model.model.diffusion_model, 11), (model.first_stage_model, 12)):
-        stage.load_weights(arch.random_state_dict(stage.shapes, seed, device=dev), dev)
-    return model.to(dev).eval()
+    return pipeline.load_random_weights(instantiate_from_config(remap_config(node)), dev, gen_device=dev).eval()
 
 
 def load_clip(clip_ckpt=None, clip_vocab=None, random_init=False, tiny=False, device="cuda", unsafe_ckpt=False):

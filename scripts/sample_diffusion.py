@@ -10,8 +10,8 @@ or the VQ-f4 models (CelebA-HQ, FFHQ, LSUN-Bedrooms: configs/latent-diffusion/*-
 
 -r is a checkpoint (its directory holds config.yaml) or a logdir holding model.ckpt and config.yaml. DDIM with eta
 (default 1.0) or, with -v, the ancestral sampler over all training steps (progressive_denoising). Sampling runs inside
-ema_scope(), so checkpoints with EMA copies sample with them. With --random_init no checkpoint is read: the UNet and the
-first stage get seeded random weights (the config comes from -r, --config, or the built-in LSUN-Churches values).
+ema_scope(), so checkpoints with EMA copies sample with them. With --random_init no checkpoint is read: every stage with
+weights gets seeded random weights (the config comes from -r, --config, or the built-in LSUN-Churches values).
 Samples are written as sample_XXXXXX.png and one .npz of uint8 NHWC images, converted exactly as the reference does.
 """
 import argparse
@@ -26,7 +26,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import sdb200  # noqa: E402
-from sdb200 import arch  # noqa: E402
+from sdb200 import arch, pipeline  # noqa: E402
 from sdb200.samplers import DDIMSampler  # noqa: E402
 from sdb200.util import instantiate_from_config, remap_config  # noqa: E402
 
@@ -177,11 +177,7 @@ def main(argv=None):
     if opt.random_init:
         node = sdb200.checkpoint.load_config(config) if config else lsun_churches_config()
         print("--random_init: seeded random-init weights (images will be noise-like)")
-        model = instantiate_from_config(remap_config(node))
-        model.model.diffusion_model.load_weights(
-            arch.random_state_dict(model.model.diffusion_model.shapes, 11, device=dev), dev)
-        model.first_stage_model.load_weights(arch.random_state_dict(model.first_stage_model.shapes, 12, device=dev), dev)
-        model = model.to(dev).eval()
+        model = pipeline.load_random_weights(instantiate_from_config(remap_config(node)), dev, gen_device=dev).eval()
         global_step = None
     else:
         model = sdb200.checkpoint.load_model_from_config(config, ckpt, device=dev)

@@ -24,7 +24,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import sdb200  # noqa: E402
-from sdb200 import arch  # noqa: E402
+from sdb200 import arch, pipeline  # noqa: E402
 from sdb200.samplers import DDIMSampler  # noqa: E402
 from sdb200.util import instantiate_from_config, remap_config  # noqa: E402
 
@@ -67,10 +67,7 @@ def load_model(ckpt=None, random_init=False, tiny=False, device="cuda", model="c
     node = make(*tiny_cfgs) if tiny else make()
     if not random_init:
         return sdb200.checkpoint.load_model_from_config({"model": node}, ckpt, device=dev)
-    model = instantiate_from_config(remap_config(node))
-    for stage, seed in ((model.model.diffusion_model, 11), (model.first_stage_model, 12), (model.cond_stage_model, 13)):
-        stage.load_weights(arch.random_state_dict(stage.shapes, seed, device=dev), dev)
-    return model.to(dev).eval()
+    return pipeline.load_random_weights(instantiate_from_config(remap_config(node)), dev, gen_device=dev).eval()
 
 
 def make_grid(images, nrow, padding=2):

@@ -30,11 +30,9 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import sdb200  # noqa: E402
-from sdb200 import arch  # noqa: E402
+from sdb200 import arch, pipeline  # noqa: E402
 from sdb200.samplers import DDIMSampler  # noqa: E402
 from sdb200.util import instantiate_from_config, remap_config  # noqa: E402
-
-UNET_SEED, VQ_SEED, COND_SEED = 11, 12, 13
 
 
 def semantic_config(unet_cfg=None, vq_cfg=None, cond_cfg=None, image_size=None):
@@ -94,11 +92,7 @@ def load_model(ckpt=None, random_init=False, tiny=False, config=None, device="cu
             semantic_config(image_size=image_size))
     if not random_init:
         return sdb200.checkpoint.load_model_from_config({"model": node}, ckpt, device=dev)
-    model = instantiate_from_config(remap_config(node))
-    for stage, seed in ((model.model.diffusion_model, UNET_SEED), (model.first_stage_model, VQ_SEED),
-                        (model.cond_stage_model, COND_SEED)):
-        stage.load_weights(arch.random_state_dict(stage.shapes, seed, device=dev), dev)
-    return model.to(dev).eval()
+    return pipeline.load_random_weights(instantiate_from_config(remap_config(node)), dev, gen_device=dev).eval()
 
 
 @torch.no_grad()

@@ -62,14 +62,17 @@ def build_laion_model(unet_cfg=None, vae_cfg=None, bert_cfg=None):
 
 
 def load_random_weights(model, device, seeds=(11, 12, 13), gen_device=None):
-    """Seeded synthetic weights for all three stages (no checkpoint offline). gen_device='cuda' draws on the GPU."""
+    """Seeded synthetic weights for a LatentDiffusion (no checkpoint offline): the UNet, first stage and cond stage get
+    seeds[0], seeds[1] and seeds[2]. A cond stage that is the first stage (__is_first_stage__) is loaded once, with the
+    first stage's seed, and stages without `shapes` (Identity, no cond stage) hold no weights. gen_device='cuda' draws
+    on the GPU, which gives other numbers than the CPU default."""
     gd = gen_device or "cpu"
-    u = model.model.diffusion_model
-    u.load_weights(arch.random_state_dict(u.shapes, seeds[0], device=gd), device)
-    v = model.first_stage_model
-    v.load_weights(arch.random_state_dict(v.shapes, seeds[1], device=gd), device)
-    c = model.cond_stage_model
-    c.load_weights(arch.random_state_dict(c.shapes, seeds[2], device=gd), device)
+    stages = [model.model.diffusion_model, model.first_stage_model]
+    if model.cond_stage_model is not model.first_stage_model:
+        stages.append(model.cond_stage_model)
+    for stage, seed in zip(stages, seeds):
+        if getattr(stage, "shapes", None):
+            stage.load_weights(arch.random_state_dict(stage.shapes, seed, device=gd), device)
     return model.to(device)
 
 

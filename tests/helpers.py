@@ -1,4 +1,5 @@
 """Shared test helpers: golden loading, seeded weights, error metrics. The oracle is imported ONLY by tests."""
+import importlib.util
 import os
 import sys
 
@@ -24,6 +25,14 @@ _cache = {}
 
 def golden(name):
     return torch.load(os.path.join(GOLDEN, name), weights_only=True)
+
+
+def script(name):
+    """scripts/<name>.py as a module (the scripts are not a package)."""
+    spec = importlib.util.spec_from_file_location(name, os.path.join(ROOT, "scripts", name + ".py"))
+    mod = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(mod)
+    return mod
 
 
 def weights(kind, tag, seed):

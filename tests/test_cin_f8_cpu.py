@@ -1,8 +1,6 @@
 """The class-conditional ImageNet LDM-VQ-8 (models/ldm/cin256) on the host: the oracle (oracle/cin_f8_oracle.py) against
 the unmodified reference's outputs (tests/golden/cin_f8.pt), the architecture tables against the reference's key list of
 the whole model, both reference YAML nodes, checkpoint ingest with EMA weights, and argument checks."""
-import importlib.util
-import os
 
 import pytest
 import torch
@@ -12,7 +10,7 @@ import helpers  # noqa: F401  (sys.path for the oracle)
 import cin_f8_oracle as F8
 import cin_oracle as CO
 import uncond_oracle as U
-from helpers import golden, rel_l2
+from helpers import golden, rel_l2, script
 from sdb200 import arch
 
 UCFG = {"tiny": arch.TINY_CIN_F8_UNET, "cin256": arch.CIN256_F8_UNET}
@@ -28,13 +26,6 @@ def _sub(x, g):
     """The pixels the golden stores of a decoded image: every g["image_stride"]-th in both directions."""
     k = g["image_stride"]
     return x[..., ::k, ::k]
-
-
-def _script():
-    spec = importlib.util.spec_from_file_location("sample_imagenet", os.path.join(helpers.ROOT, "scripts", "sample_imagenet.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 @pytest.mark.parametrize("idx", range(5))
@@ -142,7 +133,7 @@ def test_reference_yaml_nodes_resolve(path):
     assert isinstance(m.first_stage_model, sdb200.VQModelInterface) and m.first_stage_model.shapes == arch.vq_param_shapes(arch.VQ_F8)
     assert isinstance(m.cond_stage_model, sdb200.ClassEmbedder) and m.cond_stage_model.n_classes == 1000
     assert m.use_ema and m.cond_stage_key == "class_label" and m.model.conditioning_key == "crossattn"
-    mine = _script().cin256_f8_config()
+    mine = script("sample_imagenet").cin256_f8_config()
     assert {k: v for k, v in mine["params"].items() if k not in ("unet_config", "first_stage_config", "cond_stage_config")} == \
         {k: v for k, v in p.items() if k not in ("unet_config", "first_stage_config", "cond_stage_config")}
     assert mine["params"]["unet_config"] == p["unet_config"]
@@ -153,7 +144,7 @@ def test_load_tiny_checkpoint_with_ema(tmp_path):
     the EMA copies become the UNet's "ema" weight set."""
     import sdb200
     from sdb200 import checkpoint
-    node = _script().cin256_f8_config(arch.TINY_CIN_F8_UNET, arch.TINY_VQ_F8, arch.TINY_CIN_F8_COND)
+    node = script("sample_imagenet").cin256_f8_config(arch.TINY_CIN_F8_UNET, arch.TINY_VQ_F8, arch.TINY_CIN_F8_COND)
     cfg = tmp_path / "config.yaml"
     cfg.write_text(yaml.safe_dump({"model": {"base_learning_rate": 1.0e-06, **node}}))
     ushapes = arch.unet_param_shapes(arch.TINY_CIN_F8_UNET)
@@ -217,7 +208,7 @@ def test_first_stage_arguments():
 
 def test_script_rejects_guidance_for_cin256():
     """cin256 has no unconditional label: any scale other than 1.0 is an error before anything is built."""
-    mod = _script()
+    mod = script("sample_imagenet")
     for scale in ("3", "0.5"):
         with pytest.raises(ValueError, match="unconditional"):
             mod.main(["--model", "cin256", "--scale", scale, "--random_init", "--tiny"])

@@ -4,14 +4,13 @@ Multi-head d = 32 attention at the UNet's head counts and token counts against f
 holds NaN), the UNet, the VQ-f8 first stage with its level attention and the quantizer against the unmodified reference
 (tests/golden/cin_f8.pt) or fp64, graph replay and the C handle against eager, unguided DDIM trajectories on EMA
 weights, every GEMM tile plan of the model's GEMM problems, and the sampling script."""
-import os
 
 import pytest
 import torch
 
 import helpers  # noqa: F401
-from helpers import golden, rel_l2
-from sdb200 import arch, ops
+from helpers import golden, rel_l2, script
+from sdb200 import arch, ops, pipeline
 from workloads import GEMM_MODEL_WORKLOADS
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(1800)]
@@ -50,14 +49,6 @@ def _vq(tag, dev):
         _models[key] = sdb200.VQModelInterface(**VCFG[tag]).load_weights(
             arch.random_state_dict(arch.vq_param_shapes(VCFG[tag]), g["vq_seed"]), dev)
     return _models[key]
-
-
-def _script():
-    import importlib.util
-    spec = importlib.util.spec_from_file_location("sample_imagenet", os.path.join(helpers.ROOT, "scripts", "sample_imagenet.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 # ------------------------------------------------------------------------------------------------ d = 32 attention
@@ -189,16 +180,12 @@ def test_quantizer_indices_vs_fp64(cuda_dev):
 def _tiny_model(dev):
     from sdb200.util import instantiate_from_config, remap_config
     g = golden("cin_f8.pt")
-    m = instantiate_from_config(remap_config(_script().cin256_f8_config(arch.TINY_CIN_F8_UNET, arch.TINY_VQ_F8,
-                                                                        arch.TINY_CIN_F8_COND)))
-    ushapes = arch.unet_param_shapes(arch.TINY_CIN_F8_UNET)
-    unet = m.model.diffusion_model
-    unet.load_weights(arch.random_state_dict(ushapes, g["unet_seed"]), dev)
-    unet.set_weight_set("ema", arch.random_state_dict(ushapes, g["ema_seed"]))
-    m.first_stage_model.load_weights(arch.random_state_dict(arch.vq_param_shapes(arch.TINY_VQ_F8), g["vq_seed"]), dev)
-    m.cond_stage_model.load_weights(arch.random_state_dict(arch.class_embedder_param_shapes(arch.TINY_CIN_F8_COND),
-                                                           g["cond_seed"]), dev)
-    return m.to(dev).eval()
+    node = script("sample_imagenet").cin256_f8_config(arch.TINY_CIN_F8_UNET, arch.TINY_VQ_F8, arch.TINY_CIN_F8_COND)
+    m = pipeline.load_random_weights(instantiate_from_config(remap_config(node)), dev,
+                                     seeds=(g["unet_seed"], g["vq_seed"], g["cond_seed"]))
+    m.model.diffusion_model.set_weight_set("ema", arch.random_state_dict(arch.unet_param_shapes(arch.TINY_CIN_F8_UNET),
+                                                                         g["ema_seed"]))
+    return m.eval()
 
 
 @pytest.mark.parametrize("eta", [0, 1])
@@ -231,7 +218,7 @@ def test_tiny_unguided_ddim10_matches_reference(cuda_dev, monkeypatch, eta, grap
 
 
 def test_sample_imagenet_script_cin256_tiny(cuda_dev, tmp_path):
-    mod = _script()
+    mod = script("sample_imagenet")
     path = mod.main(["--model", "cin256", "--random_init", "--tiny", "--outdir", str(tmp_path), "--classes", "25", "187",
                      "--n_samples_per_class", "2", "--ddim_steps", "4"])
     from PIL import Image

@@ -1,8 +1,6 @@
 """The class-conditional ImageNet LDM (cin256-v2) on the host: the oracle (oracle/cin_oracle.py, ldm_oracle.unet_forward
 with one head) against the unmodified reference's outputs (tests/golden/cin.pt), the architecture tables against the
 reference's key list of the whole model, config resolution, checkpoint ingest and argument checks."""
-import importlib.util
-import os
 
 import pytest
 import torch
@@ -12,18 +10,11 @@ import helpers  # noqa: F401  (sys.path for the oracle)
 import cin_oracle as CO
 import ldm_oracle as O
 import vq_oracle as V
-from helpers import golden, rel_l2
+from helpers import golden, rel_l2, script
 from sdb200 import arch
 
 UCFG = {"tiny_cin": arch.TINY_CIN_UNET, "cin256": arch.CIN256_V2_UNET}
 CCFG = {"tiny_cin": arch.TINY_CIN_COND, "cin256": arch.CIN256_V2_COND}
-
-
-def _script():
-    spec = importlib.util.spec_from_file_location("sample_imagenet", os.path.join(helpers.ROOT, "scripts", "sample_imagenet.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 @pytest.mark.parametrize("idx", range(5))
@@ -70,7 +61,7 @@ def test_arch_tables_match_reference_keys():
 
 def test_target_map_resolves_every_cin_target():
     from sdb200.util import TARGET_MAP, get_obj_from_str
-    node = _script().cin_config()
+    node = script("sample_imagenet").cin_config()
     targets = [node["target"]] + [node["params"][k]["target"] for k in ("unet_config", "first_stage_config",
                                                                            "cond_stage_config")]
     for t in targets:
@@ -106,7 +97,7 @@ def test_load_tiny_cin_checkpoint(tmp_path):
     load_model_from_config with no missing or unexpected keys."""
     import sdb200
     from sdb200 import checkpoint
-    node = _script().cin_config(arch.TINY_CIN_UNET, arch.TINY_VQ, arch.TINY_CIN_COND)
+    node = script("sample_imagenet").cin_config(arch.TINY_CIN_UNET, arch.TINY_VQ, arch.TINY_CIN_COND)
     cfg = tmp_path / "config.yaml"
     cfg.write_text(yaml.safe_dump({"model": {"base_learning_rate": 1.0e-04, **node}}))
     sd = {"model.diffusion_model." + k: t for k, t in

@@ -4,14 +4,13 @@ Single-head attention at d = 384 / 576 / 960 against fp64 (memory the kernel mus
 descriptor checks, the attn1 out-projection GEMM with FiLM and residual together (the one-token cross-attention fold)
 against fp64, the ClassEmbedder, and the UNet, a guided DDIM trajectory and its VQ decode against the unmodified
 reference (tests/golden/cin.pt)."""
-import os
 
 import pytest
 import torch
 
 import helpers  # noqa: F401
-from helpers import golden, rel_l2
-from sdb200 import arch
+from helpers import golden, rel_l2, script
+from sdb200 import arch, pipeline
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900)]
 UCFG = {"tiny_cin": arch.TINY_CIN_UNET, "cin256": arch.CIN256_V2_UNET}
@@ -174,24 +173,12 @@ def test_cin256_graph_autotune_c_handle_and_class_switch(cuda_dev):
     assert torch.equal(replay2, eager2) and not torch.equal(eager2, eager)
 
 
-def _sample_imagenet_module():
-    import importlib.util
-    spec = importlib.util.spec_from_file_location("sample_imagenet", os.path.join(helpers.ROOT, "scripts", "sample_imagenet.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
 def _tiny_model(dev):
     from sdb200.util import instantiate_from_config, remap_config
     g = golden("cin.pt")
-    mod = _sample_imagenet_module()
-    m = instantiate_from_config(remap_config(mod.cin_config(arch.TINY_CIN_UNET, arch.TINY_VQ, arch.TINY_CIN_COND)))
-    m.model.diffusion_model.load_weights(arch.random_state_dict(arch.unet_param_shapes(arch.TINY_CIN_UNET), g["unet_seed"]), dev)
-    m.first_stage_model.load_weights(arch.random_state_dict(arch.vq_param_shapes(arch.TINY_VQ), g["vq_seed"]), dev)
-    m.cond_stage_model.load_weights(arch.random_state_dict(arch.class_embedder_param_shapes(arch.TINY_CIN_COND),
-                                                           g["cond_seed"]), dev)
-    return m.to(dev).eval()
+    node = script("sample_imagenet").cin_config(arch.TINY_CIN_UNET, arch.TINY_VQ, arch.TINY_CIN_COND)
+    m = instantiate_from_config(remap_config(node))
+    return pipeline.load_random_weights(m, dev, seeds=(g["unet_seed"], g["vq_seed"], g["cond_seed"])).eval()
 
 
 def test_guided_ddim_trajectory_and_decode(cuda_dev):
@@ -214,7 +201,7 @@ def test_guided_ddim_trajectory_and_decode(cuda_dev):
 
 
 def test_sample_imagenet_script_random_init(cuda_dev, tmp_path):
-    mod = _sample_imagenet_module()
+    mod = script("sample_imagenet")
     path = mod.main(["--random_init", "--tiny", "--outdir", str(tmp_path), "--classes", "25", "187",
                      "--n_samples_per_class", "2", "--ddim_steps", "4"])
     from PIL import Image

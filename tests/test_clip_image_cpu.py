@@ -2,7 +2,6 @@
 transformers' CLIPVisionModelWithProjection (tests/golden/clip_image.pt), a numpy restatement of the bicubic resize the
 preprocessing kernel implements against F.interpolate, the database builder's manifest / shard / --resume logic, and the
 constructor's errors."""
-import importlib.util
 import os
 
 import numpy as np
@@ -10,19 +9,10 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-import helpers
-from helpers import golden
+from helpers import golden, script
 from sdb200 import arch
 
 A = -0.75
-
-
-def _script():
-    spec = importlib.util.spec_from_file_location("build_rdm_database",
-                                                  os.path.join(helpers.ROOT, "scripts", "build_rdm_database.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 # ------------------------------------------------------------------------------------------------ arch tables
@@ -111,7 +101,7 @@ def _tree(root, names):
 
 
 def test_manifest_lists_images_sorted_and_skips_other_files(tmp_path):
-    mod = _script()
+    mod = script("build_rdm_database")
     _tree(str(tmp_path), ["b/2.png", "a.jpg", "b/1.PNG", "c/d/e.webp"])
     (tmp_path / "notes.txt").write_text("x")
     assert mod.list_images(str(tmp_path)) == ["a.jpg", "b/1.PNG", "b/2.png", "c/d/e.webp"]
@@ -126,7 +116,7 @@ def test_manifest_lists_images_sorted_and_skips_other_files(tmp_path):
 
 
 def test_shard_naming_and_ranges_keep_manifest_order():
-    mod = _script()
+    mod = script("build_rdm_database")
     assert mod.shard_ranges(10, 4) == [(0, 0, 4), (1, 4, 8), (2, 8, 10)]
     assert mod.shard_ranges(8, 4) == [(0, 0, 4), (1, 4, 8)]
     names = [mod.shard_name(k) for k in (0, 9, 10, 123456)]
@@ -135,7 +125,7 @@ def test_shard_naming_and_ranges_keep_manifest_order():
 
 def test_written_shards_load_through_retrieval_and_resume_check(tmp_path):
     from sdb200.retrieval import load_database
-    mod = _script()
+    mod = script("build_rdm_database")
     d = str(tmp_path)
     rng = np.random.default_rng(0)
     emb = rng.standard_normal((10, 768)).astype(np.float32)
@@ -158,21 +148,14 @@ def test_written_shards_load_through_retrieval_and_resume_check(tmp_path):
     assert not mod.shard_complete(p1, 4, 8)
 
 
-def _knn2img_parser():
-    spec = importlib.util.spec_from_file_location("knn2img", os.path.join(helpers.ROOT, "scripts", "knn2img.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod.get_parser()
-
-
 def test_knn2img_database_dir_defaults_to_none():
-    opt = _knn2img_parser().parse_args([])
+    opt = script("knn2img").get_parser().parse_args([])
     assert opt.database_dir is None and opt.database == "artbench-surrealism"
-    assert _knn2img_parser().parse_args(["--database_dir", "x"]).database_dir == "x"
+    assert script("knn2img").get_parser().parse_args(["--database_dir", "x"]).database_dir == "x"
 
 
 def test_builder_flags():
-    mod = _script()
+    mod = script("build_rdm_database")
     opt = mod.get_parser().parse_args(["--images", "a", "--outdir", "b"])
     assert (opt.batch, opt.shard_size, opt.resume, opt.clip_ckpt, opt.random_init) == (256, 100000, False, None, False)
     with pytest.raises(ValueError):

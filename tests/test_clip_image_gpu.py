@@ -13,7 +13,7 @@ import torch
 import torch.nn.functional as F
 
 import helpers
-from helpers import golden, rel_l2
+from helpers import golden, rel_l2, script
 from sdb200 import arch, ops
 from sdb200.clip_image import _table
 from workloads import GEMM_MODEL_WORKLOADS
@@ -177,12 +177,7 @@ def test_build_database_search_and_knn2img(cuda_dev, tmp_path):
         w, h = Image.open(os.path.join(imgs, manifest[i])).size
         assert tuple(data["patch_coords"][i]) == (0, 0, w, h)
     # the builder's embeddings are the embedder's on the decoded images
-    import importlib.util
-    spec = importlib.util.spec_from_file_location("build_rdm_database",
-                                                  os.path.join(helpers.ROOT, "scripts", "build_rdm_database.py"))
-    builder = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(builder)
-    emb = builder.load_embedder(random_init=True, tiny=True, device=cuda_dev)
+    emb = script("build_rdm_database").load_embedder(random_init=True, tiny=True, device=cuda_dev)
     some = [torch.from_numpy(np.asarray(Image.open(os.path.join(imgs, manifest[i])).convert("RGB"))) for i in (0, 1, 2)]
     assert rel_l2(emb.encode_uint8(some), torch.from_numpy(data["embedding"][:3])) < 1e-5
     # each image's own embedding finds that image first

@@ -3,7 +3,6 @@ tests/golden/first_stage.pt by oracle/make_golden_first_stage.py) through the co
 the architecture tables against the reference's key lists, the oracle against the reference's outputs for the four
 geometries no LDM uses, VQModel.decode_code's argument checks, scripts/autoencode.py's argument and size checks, and the
 loud failure of the engine without CUDA."""
-import importlib.util
 import os
 
 import numpy as np
@@ -15,7 +14,7 @@ import helpers  # noqa: F401  (sys.path for the oracle)
 import cin_f8_oracle as F8
 import rdm_oracle as RO
 import vq_oracle as VO
-from helpers import golden, rel_l2
+from helpers import golden, rel_l2, script
 import sdb200
 from sdb200 import arch, checkpoint
 from sdb200.util import TARGET_MAP, instantiate_from_config, remap_config
@@ -30,13 +29,6 @@ def _g():
 
 def _shapes(cfg):
     return arch.vq_param_shapes(cfg) if "n_embed" in cfg else arch.vae_param_shapes(cfg)
-
-
-def _script():
-    spec = importlib.util.spec_from_file_location("autoencode", os.path.join(helpers.ROOT, "scripts", "autoencode.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 def _write_yaml(tmp_path, name):
@@ -176,7 +168,7 @@ def test_fails_loudly_without_cuda(cfg):
 
 
 def test_autoencode_arguments(tmp_path):
-    S = _script()
+    S = script("autoencode")
     p = S.get_parser()
     cfg = _write_yaml(tmp_path, "kl-f32")
     with pytest.raises(ValueError, match="--ckpt, or --random_init"):
@@ -201,7 +193,7 @@ def test_autoencode_arguments(tmp_path):
 
 def test_autoencode_image_inputs(tmp_path):
     from PIL import Image
-    S = _script()
+    S = script("autoencode")
     p = S.get_parser()
     cfg = _write_yaml(tmp_path, "vq-f8-n256")
     d = tmp_path / "imgs"

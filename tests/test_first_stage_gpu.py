@@ -2,7 +2,6 @@
 the unmodified reference (tests/golden/first_stage.pt) at full width, their small members against the oracle, the index
 decisions of the quantizer, VQModel against VQModelInterface, the 1x1 latent heads up to 128 channels against fp64, and
 scripts/autoencode.py end to end for all nine configs."""
-import os
 
 import numpy as np
 import pytest
@@ -12,7 +11,7 @@ import yaml
 import helpers  # noqa: F401
 import cin_f8_oracle as F8
 import rdm_oracle as RO
-from helpers import golden, rel_l2
+from helpers import golden, rel_l2, script
 import sdb200
 from sdb200 import arch, ops
 
@@ -196,12 +195,9 @@ def test_pointwise_small_rejects_past_128(cuda_dev):
 # ------------------------------------------------------------------------------------------------ the script
 @pytest.mark.parametrize("name", sorted(arch.FIRST_STAGES))
 def test_autoencode_script_random_init(cuda_dev, tmp_path, name):
-    import importlib.util
     from PIL import Image
     _models.clear()
-    spec = importlib.util.spec_from_file_location("autoencode", os.path.join(helpers.ROOT, "scripts", "autoencode.py"))
-    S = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(S)
+    S = script("autoencode")
     cfg_path = tmp_path / "config.yaml"
     cfg_path.write_text(yaml.safe_dump(golden("first_stage.pt")["yamls"][name]))
     out = tmp_path / "out"

@@ -1,8 +1,6 @@
 """The LDM inpainting model on the host: the oracle (oracle/inpaint_oracle.py) against the unmodified reference's
 make_batch / interpolate / composite outputs (tests/golden/inpaint.pt), the architecture tables against the reference's
 state-dict keys, and config / checkpoint ingest (DummyLoss, __is_first_stage__, both key prefixes)."""
-import importlib.util
-import os
 
 import numpy as np
 import pytest
@@ -10,15 +8,8 @@ import torch
 
 import helpers  # noqa: F401  (sys.path for the oracle)
 import inpaint_oracle as P
-from helpers import golden
+from helpers import golden, script
 from sdb200 import arch
-
-
-def _script():
-    spec = importlib.util.spec_from_file_location("inpaint_script", os.path.join(helpers.ROOT, "scripts", "inpaint.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 def _x_dec(case):
@@ -69,7 +60,7 @@ def test_arch_tables_match_reference_keys():
 def test_config_instantiates_with_first_stage_as_cond_stage():
     import sdb200
     from sdb200.util import instantiate_from_config, remap_config
-    node = _script().inpaint_config(arch.TINY_INPAINT_UNET, arch.TINY_VQ_NOATTN)
+    node = script("inpaint").inpaint_config(arch.TINY_INPAINT_UNET, arch.TINY_VQ_NOATTN)
     assert node["params"]["first_stage_config"]["params"]["lossconfig"]["target"].endswith("DummyLoss")
     model = instantiate_from_config(remap_config(node))
     assert isinstance(model, sdb200.LatentDiffusion)
@@ -80,7 +71,8 @@ def test_config_instantiates_with_first_stage_as_cond_stage():
 
 def test_checkpoint_with_both_prefixes_loads_without_missing_keys():
     from sdb200.util import instantiate_from_config, remap_config
-    model = instantiate_from_config(remap_config(_script().inpaint_config(arch.TINY_INPAINT_UNET, arch.TINY_VQ_NOATTN)))
+    node = script("inpaint").inpaint_config(arch.TINY_INPAINT_UNET, arch.TINY_VQ_NOATTN)
+    model = instantiate_from_config(remap_config(node))
     u = arch.random_state_dict(arch.unet_param_shapes(arch.TINY_INPAINT_UNET), 11)
     v = arch.random_state_dict(arch.vq_param_shapes(arch.TINY_VQ_NOATTN), 12)
     sd = {"model.diffusion_model." + k: t for k, t in u.items()}

@@ -1,7 +1,6 @@
 """The LDM inpainting model on the H100: the prepare / composite kernels bit-exact against the reference's make_batch,
 interpolate and composite (tests/golden/inpaint.pt), the two-source conv_in im2col and the UNet's concat route
 bit-identical to the 7-channel input, UNet / VQ / DDIM parity with the reference, and scripts/inpaint.py end to end."""
-import importlib.util
 import os
 
 import numpy as np
@@ -9,19 +8,12 @@ import pytest
 import torch
 
 import helpers  # noqa: F401
-from helpers import golden, rel_l2
-from sdb200 import arch, ops
+from helpers import golden, rel_l2, script
+from sdb200 import arch, ops, pipeline
 
 pytestmark = pytest.mark.gpu
 UCFG = {"tiny": arch.TINY_INPAINT_UNET, "big": arch.INPAINTING_BIG_UNET}
 VCFG = {"tiny": arch.TINY_VQ_NOATTN, "big": arch.VQ_F4_NOATTN}
-
-
-def _script():
-    spec = importlib.util.spec_from_file_location("inpaint_script", os.path.join(helpers.ROOT, "scripts", "inpaint.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 _UNETS = {}
@@ -120,18 +112,18 @@ def test_vq_noattn_encode_decode(cuda_dev, idx):
 
 
 def _tiny_model(dev):
-    S = _script()
+    S = script("inpaint")
     return S, S.load_model(random_init=True, tiny=True, device=dev)
 
 
 def test_tiny_end_to_end_ddim10(cuda_dev):
     from sdb200.samplers import DDIMSampler
-    e = golden("inpaint.pt")["e2e"]
+    g = golden("inpaint.pt")
+    e = g["e2e"]
     S, m = _tiny_model(cuda_dev)
     assert torch.equal(m.alphas_cumprod.cpu(), e["alphas_cumprod"])
     # load_model(random_init) draws on the device generator: load the CPU-drawn golden weights instead
-    m.model.diffusion_model.load_weights(arch.random_state_dict(arch.unet_param_shapes(arch.TINY_INPAINT_UNET), 11), cuda_dev)
-    m.first_stage_model.load_weights(arch.random_state_dict(arch.vq_param_shapes(arch.TINY_VQ_NOATTN), 12), cuda_dev)
+    pipeline.load_random_weights(m, cuda_dev, seeds=(g["unet_seed"], g["vq_seed"]))
     img, mk = e["image"][None].to(cuda_dev), e["mask"][None].to(cuda_dev)
     with m.ema_scope():
         out, c, s, x = S.inpaint(m, DDIMSampler(m), img, mk, steps=10, x_T=e["x_T"].to(cuda_dev), return_latents=True)
@@ -176,7 +168,8 @@ def test_script_tiny_writes_one_png_per_pair(cuda_dev, tmp_path):
     indir.mkdir()
     _write_pair(str(indir), "a", 32, 48, 0)
     _write_pair(str(indir), "b", 40, 32, 1)
-    written = _script().main(["--indir", str(indir), "--outdir", str(outdir), "--steps", "5", "--random_init", "--tiny"])
+    written = script("inpaint").main(["--indir", str(indir), "--outdir", str(outdir), "--steps", "5", "--random_init",
+                                      "--tiny"])
     assert sorted(os.path.basename(p) for p in written) == ["a.png", "b.png"]
     assert Image.open(outdir / "a.png").size == (48, 32) and Image.open(outdir / "b.png").size == (32, 40)
 
@@ -187,5 +180,5 @@ def test_script_full_size_512(cuda_dev, tmp_path):
     indir, outdir = tmp_path / "in", tmp_path / "out"
     indir.mkdir()
     _write_pair(str(indir), "x", 512, 512, 2)
-    written = _script().main(["--indir", str(indir), "--outdir", str(outdir), "--steps", "5", "--random_init"])
+    written = script("inpaint").main(["--indir", str(indir), "--outdir", str(outdir), "--steps", "5", "--random_init"])
     assert len(written) == 1 and Image.open(written[0]).size == (512, 512)

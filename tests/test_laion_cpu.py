@@ -3,8 +3,6 @@ transformers BERT fast tokenizer on a synthetic vocabulary, the BERT oracle (ora
 unmodified reference's outputs (tests/golden/laion.pt), the architecture tables against the reference's key list of the
 whole model, config plumbing, checkpoint ingest, host-side input checks and the script's host logic."""
 import collections
-import importlib.util
-import os
 
 import pytest
 import torch
@@ -13,7 +11,7 @@ import yaml
 import helpers  # noqa: F401  (sys.path for the oracle)
 import bert_oracle as BO
 import ldm_oracle as O
-from helpers import golden, rel_l2
+from helpers import golden, rel_l2, script
 from sdb200 import arch
 
 CORPUS = ("a photograph of an astronaut riding a horse on mars , highly detailed digital painting . the quick brown "
@@ -37,13 +35,6 @@ PROMPTS = [
     "a [CLS] horse [SEP][PAD] [MASK] [UNK] [cls] x[SEP]y",                                # literal special tokens
     "〈quoted〉 «guillemets» „low“ ¿qué? ¡sí! ‰ † ‡ • ‧ ·",                                # Unicode punctuation
 ]
-
-
-def _script():
-    spec = importlib.util.spec_from_file_location("txt2img_script", os.path.join(helpers.ROOT, "scripts", "txt2img.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 def _vocab():
@@ -236,7 +227,7 @@ def test_load_tiny_laion_checkpoint(tmp_path, fmt):
 def test_txt2img_laion400m_host_logic(tmp_path, monkeypatch):
     """--laion400m switches config / checkpoint / output directory as the reference does; the built-in LAION config is
     used when the YAML is absent; the stand-in and unconditional ids are bert-base-uncased's."""
-    mod = _script()
+    mod = script("txt2img")
     import argparse
     opt = argparse.Namespace(laion400m=True, config=mod.DEFAULT_CONFIG, ckpt="x.ckpt", outdir="outputs/txt2img-samples")
     mod.apply_laion400m(opt)

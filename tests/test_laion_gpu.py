@@ -76,12 +76,7 @@ def test_tiny_guided_plms_from_ids_to_image(cuda_dev):
     g = golden("laion.pt")
     d = g["plms"]
     model = pipeline.build_laion_model(arch.TINY_LAION_UNET, arch.TINY_VAE, arch.TINY_BERT)
-    model.model.diffusion_model.load_weights(
-        arch.random_state_dict(arch.unet_param_shapes(arch.TINY_LAION_UNET), g["unet_seed"]), cuda_dev)
-    model.first_stage_model.load_weights(arch.random_state_dict(arch.vae_param_shapes(arch.TINY_VAE), g["vae_seed"]), cuda_dev)
-    model.cond_stage_model.load_weights(arch.random_state_dict(arch.bert_param_shapes(arch.TINY_BERT), g["bert_seed"]),
-                                        cuda_dev)
-    model = model.to(cuda_dev).eval()
+    model = pipeline.load_random_weights(model, cuda_dev, seeds=(g["unet_seed"], g["vae_seed"], g["bert_seed"])).eval()
     assert isinstance(model.cond_stage_model, sdb200.BERTEmbedder)
     pipe = pipeline.Txt2Img(model, sampler="plms", steps=10, scale=7.5, height=32, width=32, f=2)
     ids, un, x_T = d["ids"].to(cuda_dev), d["uc_ids"].to(cuda_dev), d["x_T"].to(cuda_dev)

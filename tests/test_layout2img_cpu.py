@@ -3,8 +3,6 @@ layout2img_oracle's UNet whose spatial transformers run every block of the state
 vq_oracle's decode) against the unmodified reference's outputs (tests/golden/layout2img.pt), the architecture tables
 against the reference's key list of the whole model and the YAML, checkpoint ingest from the unchanged YAML with the EMA set, the transformer depths the
 engine accepts, and the host logic of scripts/layout2img.py."""
-import importlib.util
-import os
 
 import numpy as np
 import pytest
@@ -18,18 +16,10 @@ import layout2img_oracle as L
 import ldm_oracle as O
 import uncond_oracle as U
 import vq_oracle as VO
-from helpers import golden, rel_l2
+from helpers import golden, rel_l2, script
 from sdb200 import arch
 
 STAGES = ("model.", "first_stage_model.", "cond_stage_model.")
-
-
-def _script():
-    spec = importlib.util.spec_from_file_location("layout2img_script", os.path.join(helpers.ROOT, "scripts",
-                                                                                    "layout2img.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 def tiny_node(g):
@@ -175,7 +165,7 @@ def test_unchanged_yaml_and_built_in_node_build_the_engine_classes():
     import sdb200
     from sdb200.util import instantiate_from_config, remap_config
     g = golden("layout2img.pt")
-    assert _script().layout2img_config() == g["yaml_node"]
+    assert script("layout2img").layout2img_config() == g["yaml_node"]
     m = instantiate_from_config(remap_config(g["yaml_node"]))
     assert isinstance(m, sdb200.LatentDiffusion) and m.use_ema and m.scale_factor == 1.0
     assert m.cond_stage_key == "coordinates_bbox"
@@ -252,7 +242,7 @@ def _bert():
 
 def test_token_files(tmp_path):
     """.pt and .npy ids of shape [92] (repeated --n_samples times) or [B, 92]; anything else is rejected."""
-    mod = _script()
+    mod = script("layout2img")
     bert = _bert()
     row = torch.arange(92) * 89 % 8192
     torch.save(row, tmp_path / "one.pt")
@@ -278,7 +268,7 @@ def test_token_files(tmp_path):
     (torch.zeros(1, 2, 92, dtype=torch.long), TypeError, "2-D"),
 ])
 def test_token_files_out_of_range_or_wrong_length_are_rejected(tmp_path, bad, err, match):
-    mod = _script()
+    mod = script("layout2img")
     path = tmp_path / "bad.pt"
     torch.save(bad, path)
     with pytest.raises(err, match=match):
@@ -286,7 +276,7 @@ def test_token_files_out_of_range_or_wrong_length_are_rejected(tmp_path, bad, er
 
 
 def test_random_init_stand_in_ids_and_arguments():
-    mod = _script()
+    mod = script("layout2img")
     bert = _bert()
     ids = mod.stand_in_ids(bert, 3, 42)
     assert ids.shape == (3, 92) and torch.equal(ids, mod.stand_in_ids(bert, 3, 42))
@@ -305,7 +295,7 @@ def test_random_init_builds_the_model_the_config_names(tmp_path, monkeypatch):
     """--random_init instantiates --config, or the built-in node when the default path is absent; another missing path is
     an error."""
     import sdb200
-    mod = _script()
+    mod = script("layout2img")
     g = golden("layout2img.pt")
     monkeypatch.chdir(tmp_path)
     seen = []

@@ -18,9 +18,9 @@ import test_attention_sweep_gpu as AS
 import test_elementwise_sweep_gpu as ES
 import test_gemm_plans_gpu as GP
 import test_norm_sweep_gpu as NS
-from helpers import golden, rel_l2
+from helpers import golden, rel_l2, script
 from sweeps import record
-from test_layout2img_cpu import _script, tiny_node, tiny_state_dict
+from test_layout2img_cpu import tiny_node, tiny_state_dict
 from test_pdl_order_gpu import audit_workload
 from workloads import _bert, _run_unet, _vq
 from sdb200 import arch
@@ -120,7 +120,7 @@ def _tiny_model(tmp_path, dev, fmt):
         torch.save({"state_dict": sd}, ck)
     else:
         checkpoint.write_safetensors(str(ck), sd)
-    return _script().load_model(str(cfg), str(ck), dev), cfg, ck
+    return script("layout2img").load_model(str(cfg), str(ck), dev), cfg, ck
 
 
 def _codes(m, z):
@@ -144,7 +144,7 @@ def test_tiny_unguided_ddim_matches_reference(cuda_dev, tmp_path, monkeypatch, e
     g = golden("layout2img.pt")
     d = g["tiny"]
     r = d[f"ddim_eta{eta}"]
-    mod = _script()
+    mod = script("layout2img")
     m, _, _ = _tiny_model(tmp_path, cuda_dev, fmt)
     assert torch.equal(m.alphas_cumprod.cpu(), g["alphas_cumprod"]) and m.scale_factor == 1.0
     m.model.diffusion_model.use_cuda_graph = True

@@ -1,7 +1,6 @@
 """scripts/measure.py on the host: the UNet FLOP count every bench script reports, the JSON line they print, and that
 the measurement helpers live only there (no bench script defines its own or imports another bench script)."""
 import ast
-import importlib.util
 import json
 import os
 
@@ -11,9 +10,7 @@ import helpers
 from sdb200 import arch
 
 SCRIPTS = os.path.join(helpers.ROOT, "scripts")
-_spec = importlib.util.spec_from_file_location("measure", os.path.join(SCRIPTS, "measure.py"))
-measure = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(measure)
+measure = helpers.script("measure")
 
 # (config, batch, latent h, w, context tokens) -> FLOPs, as the bench scripts count them for their workloads
 UNET_FLOPS = [

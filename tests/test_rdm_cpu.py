@@ -2,7 +2,6 @@
 the host: the oracle (oracle/rdm_oracle.py) against the unmodified reference's outputs (tests/golden/rdm.pt), the
 architecture tables against the reference's key list of the whole model, the YAML node, the schedule, the retrieval
 database's loading and normalisation, the Searcher's host logic, CLIP tokenization and the script's arguments."""
-import importlib.util
 import json
 import os
 
@@ -12,7 +11,7 @@ import torch
 
 import helpers  # noqa: F401  (sys.path for the oracle)
 import rdm_oracle as RO
-from helpers import golden, rel_l2
+from helpers import golden, rel_l2, script
 from sdb200 import arch
 
 UCFG = {"tiny": arch.TINY_RDM_UNET, "rdm": arch.RDM_UNET}
@@ -31,13 +30,6 @@ def _unit_rows(shape, seed):
 def _sub(x, g):
     k = g["image_stride"]
     return x[..., ::k, ::k]
-
-
-def _script():
-    spec = importlib.util.spec_from_file_location("knn2img", os.path.join(helpers.ROOT, "scripts", "knn2img.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 @pytest.mark.parametrize("idx", range(4))
@@ -128,14 +120,14 @@ def test_reference_yaml_node_resolves():
     assert m.first_stage_model.shapes == arch.vae_param_shapes(arch.KL_F16)
     assert isinstance(m.cond_stage_model, torch.nn.Identity)
     assert m.use_ema and m.scale_factor == pytest.approx(0.22765929) and m.model.conditioning_key == "crossattn"
-    assert _script().rdm_config() == node
+    assert script("knn2img").rdm_config() == node
     assert "ldm.modules.encoders.modules.FrozenCLIPTextEmbedder" in TARGET_MAP
 
 
 def test_schedule_linear_end():
     """linear_start 0.0015, linear_end 0.015: the engine's schedule equals the reference's buffers."""
     from sdb200.util import instantiate_from_config, remap_config
-    m = instantiate_from_config(remap_config(_script().rdm_config(arch.TINY_RDM_UNET, arch.TINY_KL_F16)))
+    m = instantiate_from_config(remap_config(script("knn2img").rdm_config(arch.TINY_RDM_UNET, arch.TINY_KL_F16)))
     assert m.linear_end == 0.015 and torch.equal(m.alphas_cumprod, golden("rdm.pt")["alphas_cumprod"])
 
 
@@ -256,7 +248,7 @@ def test_kl_first_stage_level_attention_arguments():
 
 def test_script_arguments():
     """The reference's defaults, and the argument checks that run before anything is built."""
-    mod = _script()
+    mod = script("knn2img")
     opt = mod.get_parser().parse_args([])
     assert (opt.H, opt.W, opt.ddim_steps, opt.scale, opt.n_samples, opt.knn, opt.database, opt.ddim_eta) == \
         (768, 768, 50, 5.0, 3, 10, "artbench-surrealism", 0.0)

@@ -11,8 +11,8 @@ import torch
 
 import helpers  # noqa: F401
 import rdm_oracle as RO
-from helpers import golden, rel_l2
-from sdb200 import arch, ops
+from helpers import golden, rel_l2, script
+from sdb200 import arch, ops, pipeline
 from workloads import GEMM_MODEL_WORKLOADS
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(1800)]
@@ -58,14 +58,6 @@ def _kl(tag, dev):
         _models[key] = sdb200.AutoencoderKL(**VCFG[tag]).load_weights(
             arch.random_state_dict(arch.vae_param_shapes(VCFG[tag]), golden("rdm.pt")["vae_seed"]), dev)
     return _models[key]
-
-
-def _script():
-    import importlib.util
-    spec = importlib.util.spec_from_file_location("knn2img", os.path.join(helpers.ROOT, "scripts", "knn2img.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 # ------------------------------------------------------------------------------------------------ CLIP text embedding
@@ -297,13 +289,11 @@ def test_kl_f16_encode_vs_reference(cuda_dev):
 def _tiny_model(dev):
     from sdb200.util import instantiate_from_config, remap_config
     g = golden("rdm.pt")
-    m = instantiate_from_config(remap_config(_script().rdm_config(arch.TINY_RDM_UNET, arch.TINY_KL_F16)))
-    ushapes = arch.unet_param_shapes(arch.TINY_RDM_UNET)
-    unet = m.model.diffusion_model
-    unet.load_weights(arch.random_state_dict(ushapes, g["unet_seed"]), dev)
-    unet.set_weight_set("ema", arch.random_state_dict(ushapes, g["ema_seed"]))
-    m.first_stage_model.load_weights(arch.random_state_dict(arch.vae_param_shapes(arch.TINY_KL_F16), g["vae_seed"]), dev)
-    return m.to(dev).eval()
+    m = instantiate_from_config(remap_config(script("knn2img").rdm_config(arch.TINY_RDM_UNET, arch.TINY_KL_F16)))
+    m = pipeline.load_random_weights(m, dev, seeds=(g["unet_seed"], g["vae_seed"]))
+    m.model.diffusion_model.set_weight_set("ema", arch.random_state_dict(arch.unet_param_shapes(arch.TINY_RDM_UNET),
+                                                                         g["ema_seed"]))
+    return m.eval()
 
 
 @pytest.mark.parametrize("name", ["ddim_eta0", "ddim_eta1", "plms"])
@@ -359,7 +349,7 @@ def _tiny_vocab(path):
 
 @pytest.mark.parametrize("neighbors", [False, True])
 def test_knn2img_script_tiny(cuda_dev, tmp_path, monkeypatch, neighbors):
-    mod = _script()
+    mod = script("knn2img")
     monkeypatch.chdir(tmp_path)
     _write_db(str(tmp_path / "data" / "rdm" / "retrieval_databases" / "artbench-surrealism"), 3000, 64, 1)
     vocab = _tiny_vocab(str(tmp_path / "vocab"))

@@ -2,8 +2,6 @@
 against the unmodified reference (tests/golden/semantic.pt), both reference configs through TARGET_MAP, the
 architecture tables against the reference's state-dict keys, the schedule, checkpoint ingest, and the host-side checks
 of SpatialRescaler and scripts/semantic_synthesis.py (id validation, size rule, PNG modes, unsupported options)."""
-import importlib.util
-import os
 
 import numpy as np
 import pytest
@@ -12,7 +10,7 @@ import torch
 import helpers  # noqa: F401  (sys.path for the oracle)
 import semantic_oracle as SO
 import uncond_oracle as U
-from helpers import golden, rel_l2
+from helpers import golden, rel_l2, script
 from sdb200 import arch, checkpoint
 from sdb200.util import instantiate_from_config, remap_config
 
@@ -42,14 +40,6 @@ def _yaml_model(image_size, monitor):
 
 SS256 = _yaml_model(64, monitor=False)
 SS512 = _yaml_model(128, monitor=True)
-
-
-def _script():
-    spec = importlib.util.spec_from_file_location("semantic_script",
-                                                  os.path.join(helpers.ROOT, "scripts", "semantic_synthesis.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 def _cond_cfg(name):
@@ -234,7 +224,7 @@ def test_rescaler_label_ids_checked_on_host():
                                       (16, 16, True), (1024, 2048, True),
                                       (250, 256, False), (256, 8, False), (24, 32, False), (0, 16, False)])
 def test_size_rule(h, w, ok):
-    check = _script().check_size
+    check = script("semantic_synthesis").check_size
     if ok:
         check(h, w)
     else:
@@ -244,7 +234,7 @@ def test_size_rule(h, w, ok):
 
 def test_label_png_modes(tmp_path):
     from PIL import Image
-    S = _script()
+    S = script("semantic_synthesis")
     lab = SO.voronoi_labels(32, 48, 182, 5)
     Image.fromarray(lab, mode="L").save(tmp_path / "l.png")
     assert np.array_equal(S.read_label_map(str(tmp_path / "l.png")), lab)
@@ -266,7 +256,7 @@ def test_label_png_modes(tmp_path):
 
 
 def test_script_config_matches_reference_nodes():
-    S = _script()
+    S = script("semantic_synthesis")
     for node, size in ((SS256, None), (SS512, 128)):
         assert S.semantic_config(image_size=size) == {k: v for k, v in node.items() if k != "base_learning_rate"}
     with pytest.raises(ValueError):

@@ -3,7 +3,6 @@ bit) and fp64, the label kernel bit-identical to the float kernel on the one-hot
 DDIM-10 against the unmodified reference (tests/golden/semantic.pt), graph replay against eager with the conditioning
 refreshed, the full model at a larger-than-training size, scripts/semantic_synthesis.py end to end, and every GEMM
 plan at the full UNet's GEMM problems."""
-import importlib.util
 import os
 
 import numpy as np
@@ -13,20 +12,12 @@ import torch.nn.functional as F
 
 import helpers  # noqa: F401
 import semantic_oracle as SO
-from helpers import golden, rel_l2
-from sdb200 import arch, ops
+from helpers import golden, rel_l2, script
+from sdb200 import arch, ops, pipeline
 from workloads import GEMM_MODEL_WORKLOADS
 
 pytestmark = pytest.mark.gpu
 UCFG = {"tiny": arch.TINY_SEMANTIC_UNET, "big": arch.SEMANTIC_SYNTHESIS_UNET}
-
-
-def _script():
-    spec = importlib.util.spec_from_file_location("semantic_script",
-                                                  os.path.join(helpers.ROOT, "scripts", "semantic_synthesis.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 def _gen(shape, seed):
@@ -160,13 +151,11 @@ def test_unet_eps_matches_reference(cuda_dev, idx):
 
 
 def _tiny_model(dev):
-    Sc = _script()
+    Sc = script("semantic_synthesis")
+    g = golden("semantic.pt")
     m = Sc.load_model(random_init=True, tiny=True, device=dev)
     # load_model(random_init) draws on the device generator: load the CPU-drawn golden weights instead
-    m.model.diffusion_model.load_weights(arch.random_state_dict(arch.unet_param_shapes(arch.TINY_SEMANTIC_UNET), 11), dev)
-    m.first_stage_model.load_weights(arch.random_state_dict(arch.vq_param_shapes(arch.TINY_VQ_F4), 12), dev)
-    m.cond_stage_model.load_weights(arch.random_state_dict(
-        arch.spatial_rescaler_param_shapes(arch.TINY_SEMANTIC_COND), 13), dev)
+    pipeline.load_random_weights(m, dev, seeds=(g["unet_seed"], g["vq_seed"], g["cond_seed"]))
     return Sc, m
 
 
@@ -231,7 +220,7 @@ _FULL = {}
 
 def _full(dev):
     if "m" not in _FULL:
-        Sc = _script()
+        Sc = script("semantic_synthesis")
         _FULL["m"] = (Sc, Sc.load_model(random_init=True, device=dev, image_size=128))
     return _FULL["m"]
 
@@ -272,13 +261,14 @@ def test_script_writes_pngs(cuda_dev, tmp_path):
     p = Image.fromarray(SO.voronoi_labels(32, 48, 20, 2), mode="L").convert("P")
     p.putdata(SO.voronoi_labels(32, 48, 20, 2).reshape(-1).tolist())
     p.save(indir / "b.png")
-    written = _script().main(["--indir", str(indir), "--outdir", str(outdir), "--steps", "4", "--n_samples", "2",
-                              "--random_init", "--tiny"])
+    Sc = script("semantic_synthesis")
+    written = Sc.main(["--indir", str(indir), "--outdir", str(outdir), "--steps", "4", "--n_samples", "2",
+                       "--random_init", "--tiny"])
     assert sorted(os.path.basename(q) for q in written) == ["a_00.png", "a_01.png", "b_00.png", "b_01.png"]
     assert Image.open(outdir / "a_01.png").size == (64, 64) and Image.open(outdir / "b_00.png").size == (48, 32)
     # the full 256 model from random weights, one map
     Image.fromarray(SO.voronoi_labels(64, 128, 182, 3), mode="L").save(tmp_path / "map.png")
-    written = _script().main([str(tmp_path / "map.png"), "--outdir", str(outdir), "--steps", "2", "--random_init"])
+    written = Sc.main([str(tmp_path / "map.png"), "--outdir", str(outdir), "--steps", "2", "--random_init"])
     assert Image.open(written[0]).size == (128, 64)
 
 

@@ -1,6 +1,7 @@
 """Weight plumbing of every engine stage on the host: what `load_state_dict` adopts under a prefix, which checkpoint
 leftovers are dropped silently, how missing, unexpected and misshapen tensors are reported, that host moves pack
-nothing, and that `load_weights` rejects an incomplete state dict. No GPU."""
+nothing, that `load_weights` rejects an incomplete state dict, and which stages of a LatentDiffusion
+`pipeline.load_random_weights` seeds with which seed. No GPU."""
 import re
 
 import pytest
@@ -8,7 +9,9 @@ import torch
 import torch.nn as nn
 
 import sdb200
-from sdb200 import arch
+from helpers import script
+from sdb200 import arch, pipeline
+from sdb200.util import PackedStage, instantiate_from_config, remap_config
 
 # id -> (constructor, where the stage's keys sit below the stage, checkpoint keys the stage drops without reporting)
 STAGES = {
@@ -141,3 +144,37 @@ def test_unet_weight_sets_checked_and_reset_by_a_reload():
     assert unet._active == "ema" and set(unet._packed) == {"raw"}
     holder.load_state_dict(full)            # fresh weights: every packed set is stale
     assert unet._active == "raw" and unet._packed == {} and unet.has_weight_set("ema")
+
+
+# one LDM of each kind: (script, its config function, the tiny members)
+LDMS = {
+    "cin_three_stages": ("sample_imagenet", "cin_config", (arch.TINY_CIN_UNET, arch.TINY_VQ, arch.TINY_CIN_COND)),
+    "inpaint_first_stage_is_cond": ("inpaint", "inpaint_config", (arch.TINY_INPAINT_UNET, arch.TINY_VQ_NOATTN)),
+    "superres_identity_cond": ("superres", "superres_config", (arch.TINY_BSR_UNET, arch.TINY_VQ_F4)),
+    "lsun_unconditional": ("sample_diffusion", "lsun_churches_config", (arch.TINY_ATTN_UNET, arch.TINY_VAE)),
+}
+
+
+@pytest.mark.parametrize("name", list(LDMS))
+def test_load_random_weights_seeds_each_weighted_stage_once(name, monkeypatch):
+    """UNet, first stage and cond stage get seeds 11, 12 and 13; a cond stage that is the first stage is loaded once,
+    with 12, and an Identity or absent cond stage is skipped."""
+    mod, make, members = LDMS[name]
+    m = instantiate_from_config(remap_config(getattr(script(mod), make)(*members)))
+    loads = []
+    load = PackedStage.load_weights
+    monkeypatch.setattr(PackedStage, "load_weights", lambda self, sd, device: loads.append(self) or load(self, sd, device))
+    assert pipeline.load_random_weights(m, "cpu") is m
+    seeded = [m.model.diffusion_model, m.first_stage_model]
+    if name == "cin_three_stages":
+        seeded.append(m.cond_stage_model)
+    elif name == "inpaint_first_stage_is_cond":
+        assert m.cond_stage_model is m.first_stage_model
+    elif name == "superres_identity_cond":
+        assert isinstance(m.cond_stage_model, nn.Identity)
+    else:
+        assert m.cond_stage_model is None
+    assert len(loads) == len(seeded) and all(a is b for a, b in zip(loads, seeded))
+    for stage, seed in zip(seeded, (11, 12, 13)):
+        want = arch.random_state_dict(stage.shapes, seed)
+        assert list(stage._host_sd) == list(want) and all(torch.equal(stage._host_sd[k], t) for k, t in want.items())

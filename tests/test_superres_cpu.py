@@ -2,24 +2,15 @@
 (oracle/superres_oracle.py) against the unmodified reference (tests/golden/superres.pt), the LR conversion, the size
 rule of scripts/superres.py, and the bsr_sr architecture tables against the reference's state-dict keys."""
 import hashlib
-import importlib.util
-import os
 
 import pytest
 import torch
 
 import helpers  # noqa: F401  (sys.path for the oracle)
 import superres_oracle as S
-from helpers import golden
+from helpers import golden, script
 from sdb200 import arch
 from sdb200.diffusion import split_geometry, split_tables
-
-
-def _script():
-    spec = importlib.util.spec_from_file_location("superres_script", os.path.join(helpers.ROOT, "scripts", "superres.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 def _sha(t):
@@ -83,7 +74,7 @@ def test_lr_conversion_bit_exact(idx):
     (60, 60, ValueError),                             # plain path needs multiples of 8
 ])
 def test_size_rule(h, w, path):
-    choose = _script().choose_path
+    choose = script("superres").choose_path
     if path is ValueError:
         with pytest.raises(ValueError):
             choose(h, w)
@@ -120,7 +111,8 @@ def test_arch_tables_match_reference_keys():
 def test_config_instantiates_with_identity_cond_stage_and_loads():
     import sdb200
     from sdb200.util import instantiate_from_config, remap_config
-    model = instantiate_from_config(remap_config(_script().superres_config(arch.TINY_BSR_UNET, arch.TINY_VQ_F4)))
+    node = script("superres").superres_config(arch.TINY_BSR_UNET, arch.TINY_VQ_F4)
+    model = instantiate_from_config(remap_config(node))
     assert isinstance(model, sdb200.LatentDiffusion) and isinstance(model.cond_stage_model, torch.nn.Identity)
     assert model.model.conditioning_key == "concat" and model.cond_stage_key == "LR_image"
     u = arch.random_state_dict(arch.unet_param_shapes(arch.TINY_BSR_UNET), 11)

@@ -2,7 +2,6 @@
 the patch unfold bit-identical to nn.Unfold, the weighted stitch against fp64 fold(o·w)/fold(w), UNet / VQ-f4 / tiled
 DDIM parity with the reference, the full model at 256² -> 1024² against per-tile calls stitched by the oracle, the size
 rule, scripts/superres.py end to end, and every GEMM plan at the model's GEMM problems."""
-import importlib.util
 import os
 
 import pytest
@@ -10,20 +9,13 @@ import torch
 
 import helpers  # noqa: F401
 import superres_oracle as S
-from helpers import golden, rel_l2
-from sdb200 import arch, diffusion, ops
+from helpers import golden, rel_l2, script
+from sdb200 import arch, diffusion, ops, pipeline
 from sdb200.diffusion import split_geometry, split_tables
 from workloads import GEMM_MODEL_WORKLOADS
 
 pytestmark = pytest.mark.gpu
 UCFG = {"tiny": arch.TINY_BSR_UNET, "big": arch.BSR_SR_UNET}
-
-
-def _script():
-    spec = importlib.util.spec_from_file_location("superres_script", os.path.join(helpers.ROOT, "scripts", "superres.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 def _gen(shape, seed):
@@ -124,11 +116,11 @@ def test_vq_f4_decode(cuda_dev):
 
 
 def _tiny_model(dev):
-    Sc = _script()
+    Sc = script("superres")
+    g = golden("superres.pt")
     m = Sc.load_model(random_init=True, tiny=True, device=dev)
     # load_model(random_init) draws on the device generator: load the CPU-drawn golden weights instead
-    m.model.diffusion_model.load_weights(arch.random_state_dict(arch.unet_param_shapes(arch.TINY_BSR_UNET), 11), dev)
-    m.first_stage_model.load_weights(arch.random_state_dict(arch.vq_param_shapes(arch.TINY_VQ_F4), 12), dev)
+    pipeline.load_random_weights(m, dev, seeds=(g["unet_seed"], g["vq_seed"]))
     return Sc, m
 
 
@@ -195,7 +187,7 @@ _FULL = {}
 
 def _full(dev):
     if "m" not in _FULL:
-        Sc = _script()
+        Sc = script("superres")
         _FULL["m"] = (Sc, Sc.load_model(random_init=True, device=dev))
     return _FULL["m"]
 
@@ -252,7 +244,8 @@ def test_script_tiny_writes_4x_png(cuda_dev, tmp_path):
     r = np.random.default_rng(0)
     for name, (h, w) in (("a", (24, 32)), ("b", (128, 192))):
         Image.fromarray(r.integers(0, 256, (h, w, 3), dtype=np.uint8)).save(indir / f"{name}.png")
-    written = _script().main(["--indir", str(indir), "--outdir", str(outdir), "--steps", "4", "--random_init", "--tiny"])
+    written = script("superres").main(["--indir", str(indir), "--outdir", str(outdir), "--steps", "4", "--random_init",
+                                       "--tiny"])
     assert sorted(os.path.basename(p) for p in written) == ["a.png", "b.png"]
     assert Image.open(outdir / "a.png").size == (128, 96) and Image.open(outdir / "b.png").size == (768, 512)
 

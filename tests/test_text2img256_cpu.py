@@ -5,8 +5,6 @@ model, checkpoint ingest from the unchanged YAML with the EMA set, and the host 
 text-conditional config."""
 import contextlib
 import functools
-import importlib.util
-import os
 
 import pytest
 import torch
@@ -18,18 +16,11 @@ import cin_f8_oracle as F8
 import ldm_oracle as O
 import uncond_oracle as U
 import vq_oracle as VO
-from helpers import golden, rel_l2
+from helpers import golden, rel_l2, script
 from sdb200 import arch
 
 SCHEDULE = dict(linear_start=0.0015, linear_end=0.0195)      # text2img256/config.yaml
 STAGES = ("model.", "first_stage_model.", "cond_stage_model.")
-
-
-def _script():
-    spec = importlib.util.spec_from_file_location("txt2img_script", os.path.join(helpers.ROOT, "scripts", "txt2img.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 def tiny_node(g):
@@ -210,7 +201,7 @@ def _models():
 
 def test_txt2img_tokenizer_and_stand_in_ids_follow_the_cond_stage_class():
     import sdb200
-    mod = _script()
+    mod = script("txt2img")
     bert, clip = _models()
     assert mod.text_encoder_kind(bert) == "bert" and mod.text_encoder_kind(clip) == "clip"
     ids, un = mod.stand_in_ids("bert", bert.cond_stage_model, 3, 1234, "cpu")
@@ -232,7 +223,7 @@ def test_txt2img_tokenizer_and_stand_in_ids_follow_the_cond_stage_class():
 
 
 def test_txt2img_rejects_latent_shape_flags_that_do_not_match_the_model():
-    mod = _script()
+    mod = script("txt2img")
     bert, clip = _models()
     mod.check_latent_shape(bert, 3, 4)            # TINY_TEXT2IMG256_UNET in_channels 3, TINY_VQ_F4 three levels
     mod.check_latent_shape(clip, 4, 2)            # TINY_VAE: two levels
@@ -247,7 +238,7 @@ def test_txt2img_random_init_builds_the_model_the_config_names(tmp_path, monkeyp
     """--random_init instantiates --config; the built-in SD-v1 / LAION models stay the fallback for the reference's two
     default paths when those files are absent."""
     import sdb200
-    mod = _script()
+    mod = script("txt2img")
     g = golden("text2img256.pt")
     monkeypatch.chdir(tmp_path)
     seen = []
@@ -271,7 +262,7 @@ def test_txt2img_random_init_builds_the_model_the_config_names(tmp_path, monkeyp
 def test_txt2img_defaults_unchanged(monkeypatch):
     """The default command is SD-v1 (CLIP, 4 latent channels, f 8), --laion400m switches as before, and both pass the
     latent-shape check with the default --C 4 --f 8."""
-    mod = _script()
+    mod = script("txt2img")
     import argparse
     opt = argparse.Namespace(laion400m=False, config=mod.DEFAULT_CONFIG, ckpt="x.ckpt", outdir="o")
     assert vars(mod.apply_laion400m(opt)) == dict(laion400m=False, config=mod.DEFAULT_CONFIG, ckpt="x.ckpt", outdir="o")

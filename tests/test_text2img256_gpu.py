@@ -14,9 +14,9 @@ import yaml
 import helpers  # noqa: F401
 import test_attention_sweep_gpu as AS
 import test_gemm_plans_gpu as GP
-from helpers import golden, rel_l2
+from helpers import golden, rel_l2, script
 from sweeps import record
-from test_text2img256_cpu import _script, tiny_node, tiny_state_dict
+from test_text2img256_cpu import tiny_node, tiny_state_dict
 from workloads import _run_unet, text2img256
 from sdb200 import arch
 
@@ -78,7 +78,7 @@ def _tiny_model(tmp_path, dev, fmt):
         torch.save({"state_dict": sd}, ck)
     else:
         checkpoint.write_safetensors(str(ck), sd)
-    return _script().load_model_from_config(str(cfg), str(ck), dev), cfg, ck
+    return script("txt2img").load_model_from_config(str(cfg), str(ck), dev), cfg, ck
 
 
 def _codes(m, z):
@@ -160,7 +160,7 @@ def test_txt2img_script_tiny_checkpoint_with_bert_vocab(cuda_dev, tmp_path):
     (vocab / "vocab.txt").write_text("\n".join(["[PAD]", "[unused0]", "[UNK]", "[CLS]", "[SEP]", "[MASK]"] + letters +
                                                ["##" + c for c in letters] + ["virus", "monster"]) + "\n")
     out = tmp_path / "out"
-    mod = _script()
+    mod = script("txt2img")
     mod.main(["--config", str(cfg), "--ckpt", str(ck), "--H", "64", "--W", "64", "--C", "3", "--f", "4", "--scale", "5.0",
               "--dpm_solver", "--ddim_steps", "4", "--n_samples", "2", "--n_iter", "1", "--outdir", str(out),
               "--bert_vocab", str(vocab), "--prompt", "a virus monster", "--no_watermark"])

@@ -7,7 +7,7 @@ import yaml
 
 import helpers  # noqa: F401  (sys.path for the oracle)
 import uncond_oracle as U
-from helpers import golden, rel_l2
+from helpers import golden, rel_l2, script
 from sdb200 import arch
 
 CFG = {"tiny_attn": arch.TINY_ATTN_UNET, "tiny_attn_plain": arch.TINY_ATTN_PLAIN_UNET, "lsun": arch.LSUN_CHURCHES_UNET}
@@ -86,13 +86,7 @@ def test_unet_argument_checks():
 
 
 def _lsun_yaml(tmp_path, unet_cfg, vae_cfg):
-    import importlib.util
-    import os
-    spec = importlib.util.spec_from_file_location(
-        "sample_diffusion", os.path.join(helpers.ROOT, "scripts", "sample_diffusion.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    node = mod.lsun_churches_config(unet_cfg, vae_cfg)
+    node = script("sample_diffusion").lsun_churches_config(unet_cfg, vae_cfg)
     node["params"]["scheduler_config"] = {"target": "ldm.lr_scheduler.LambdaLinearScheduler",
                                           "params": {"warm_up_steps": [10000], "cycle_lengths": [10000000000000],
                                                      "f_start": [1.0e-6], "f_max": [1.0], "f_min": [1.0]}}

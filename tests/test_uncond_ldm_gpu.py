@@ -14,8 +14,8 @@ import yaml
 
 import helpers  # noqa: F401
 import uncond_oracle as U
-from helpers import golden, rel_l2
-from sdb200 import arch
+from helpers import golden, rel_l2, script
+from sdb200 import arch, pipeline
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900)]
 CFG = {"tiny_attn": arch.TINY_ATTN_UNET, "tiny_attn_plain": arch.TINY_ATTN_PLAIN_UNET, "lsun": arch.LSUN_CHURCHES_UNET}
@@ -166,18 +166,14 @@ def test_rejections(cuda_dev):
 
 
 def _model(dev, timesteps=1000, use_ema=False):
-    import importlib.util
     from sdb200.util import instantiate_from_config, remap_config
-    spec = importlib.util.spec_from_file_location("sample_diffusion", os.path.join(helpers.ROOT, "scripts", "sample_diffusion.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
+    g = golden("lsun.pt")
+    mod = script("sample_diffusion")
     node = mod.lsun_churches_config(arch.TINY_ATTN_UNET, arch.TINY_VAE)
     node["params"].update(timesteps=timesteps, use_ema=use_ema)
     m = instantiate_from_config(remap_config(node))
-    m.model.diffusion_model.load_weights(_sd("tiny_attn"), dev)
-    m.first_stage_model.load_weights(arch.random_state_dict(arch.vae_param_shapes(arch.TINY_VAE), 12), dev)
-    m = m.to(dev).eval()
-    m.scale_factor.fill_(golden("lsun.pt")["scale_factor"])
+    m = pipeline.load_random_weights(m, dev, seeds=(g["unet_seed"], g["vae_seed"])).eval()
+    m.scale_factor.fill_(g["scale_factor"])
     return m, mod
 
 

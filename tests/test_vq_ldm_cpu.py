@@ -1,8 +1,6 @@
 """The VQ-f4 latent diffusion models on the host: the oracle (oracle/vq_oracle.py) against the unmodified reference's
 outputs (tests/golden/vq.pt), the architecture tables against the reference's key lists, the GEMM weight packing of
 widths that are multiples of 32 only, argument checks, and config / checkpoint ingest of a CelebA-HQ-style model."""
-import importlib.util
-import os
 
 import pytest
 import torch
@@ -11,7 +9,7 @@ import yaml
 import helpers  # noqa: F401  (sys.path for the oracle)
 import uncond_oracle as U
 import vq_oracle as V
-from helpers import golden, rel_l2
+from helpers import golden, rel_l2, script
 from sdb200 import arch
 
 UCFG = {"tiny_vq": arch.TINY_VQ_UNET, "celebahq": arch.CELEBAHQ_UNET}
@@ -115,10 +113,7 @@ def test_vq_first_stage_arguments():
 
 
 def _celebahq_yaml(tmp_path):
-    spec = importlib.util.spec_from_file_location("sample_diffusion", os.path.join(helpers.ROOT, "scripts", "sample_diffusion.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    node = mod.celebahq_config(arch.TINY_VQ_UNET, arch.TINY_VQ)
+    node = script("sample_diffusion").celebahq_config(arch.TINY_VQ_UNET, arch.TINY_VQ)
     p = tmp_path / "config.yaml"
     p.write_text(yaml.safe_dump({"model": {"base_learning_rate": 2.0e-06, **node}}))
     return str(p)

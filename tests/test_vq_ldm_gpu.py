@@ -12,8 +12,8 @@ import torch.nn.functional as F
 import yaml
 
 import helpers  # noqa: F401
-from helpers import golden, rel_l2
-from sdb200 import arch
+from helpers import golden, rel_l2, script
+from sdb200 import arch, pipeline
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900)]
 UCFG = {"tiny_vq": arch.TINY_VQ_UNET, "celebahq": arch.CELEBAHQ_UNET}
@@ -332,27 +332,17 @@ def test_vq_encode_vs_reference(cuda_dev):
     assert h.shape == case["h"].shape and err < 2e-3
 
 
-def _sample_diffusion_module():
-    import importlib.util
-    spec = importlib.util.spec_from_file_location("sample_diffusion", os.path.join(helpers.ROOT, "scripts", "sample_diffusion.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
 def test_ddim_eta0_trajectory_with_ema(cuda_dev):
     """DDIM-10, eta 0, of the tiny VQ LDM (celebahq config values) inside ema_scope, then decode_first_stage."""
     from sdb200.samplers import DDIMSampler
     from sdb200.util import instantiate_from_config, remap_config
     g = golden("vq.pt")
     d = g["ddim"]
-    mod = _sample_diffusion_module()
-    m = instantiate_from_config(remap_config(mod.celebahq_config(arch.TINY_VQ_UNET, arch.TINY_VQ)))
-    unet = m.model.diffusion_model
-    unet.load_weights(arch.random_state_dict(arch.unet_param_shapes(arch.TINY_VQ_UNET), g["unet_seed"]), cuda_dev)
-    unet.set_weight_set("ema", arch.random_state_dict(arch.unet_param_shapes(arch.TINY_VQ_UNET), g["ema_seed"]))
-    m.first_stage_model.load_weights(arch.random_state_dict(arch.vq_param_shapes(arch.TINY_VQ), g["vq_seed"]), cuda_dev)
-    m = m.to(cuda_dev).eval()
+    node = script("sample_diffusion").celebahq_config(arch.TINY_VQ_UNET, arch.TINY_VQ)
+    m = pipeline.load_random_weights(instantiate_from_config(remap_config(node)), cuda_dev,
+                                     seeds=(g["unet_seed"], g["vq_seed"])).eval()
+    m.model.diffusion_model.set_weight_set("ema", arch.random_state_dict(arch.unet_param_shapes(arch.TINY_VQ_UNET),
+                                                                         g["ema_seed"]))
     assert m.use_ema and torch.equal(m.alphas_cumprod.cpu(), d["alphas_cumprod"])
     with m.ema_scope():
         s, _ = DDIMSampler(m).sample(10, batch_size=2, shape=[3, 16, 16], eta=0.0, verbose=False,
@@ -369,7 +359,7 @@ def test_sample_diffusion_script_random_init_celebahq_config(cuda_dev, tmp_path)
     """The script with a CelebA-HQ-style config (VQ first stage, 3x64x64 latents shrunk to the tiny members)."""
     import glob
     import numpy as np
-    mod = _sample_diffusion_module()
+    mod = script("sample_diffusion")
     cfg = tmp_path / "config.yaml"
     cfg.write_text(yaml.safe_dump({"model": mod.celebahq_config(arch.TINY_VQ_UNET, arch.TINY_VQ)}))
     logdir = mod.main(["--random_init", "--config", str(cfg), "-n", "2", "--batch_size", "2", "-c", "4", "-e", "0",
