@@ -40,10 +40,11 @@ enum {
   SDB_ACT_GELU = 4,       /* gelu_erf(x) = 0.5 x (1 + erf(x / sqrt 2)), exact nn.GELU: the BERTEmbedder feed-forward
                              (x_transformer.py:199-202) */
                           /* 5 is not an activation: sdb_gemm rejects it, as it rejects every value not listed here */
-  SDB_ACT_RELU = 6,       /* max(x, 0): the LPIPS VGG16 trunk's ReLUs (include/sdb200_ae_loss.h) */
-  SDB_ACT_LEAKY_RELU = 7  /* x > 0 ? x : 0.2 x: the PatchGAN discriminator's LeakyReLU(0.2). The two ReLU activations
-                             run in their own epilogue instantiation and never split K: a requested split-K factor
-                             resolves to 1 */
+  SDB_ACT_RELU = 6,       /* x < 0 ? 0 : x: the LPIPS VGG16 trunk's ReLUs (include/sdb200_ae_loss.h); a NaN stays NaN,
+                             as in torch.relu */
+  SDB_ACT_LEAKY_RELU = 7  /* x > 0 ? x : 0.2 x: the PatchGAN discriminator's LeakyReLU(0.2); a NaN stays NaN. The two
+                             ReLU activations run in their own epilogue instantiation and never split K: a requested
+                             split-K factor resolves to 1 */
 };
 
 /*

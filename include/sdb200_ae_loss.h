@@ -70,7 +70,8 @@ int sdb_im2col(const void* x, int32_t nb, int32_t h, int32_t w, int32_t c, int32
  *           out[0*nb + b] = sum l, out[1*nb + b] = sum relu(1 - l), out[2*nb + b] = sum relu(1 + l),
  *           out[3*nb + b] = sum softplus(-l), out[4*nb + b] = sum softplus(l)      (g_loss, hinge_d_loss,
  *           vanilla_d_loss of taming vqperceptual.py; softplus as F.softplus: x > 20 ? x : log1p(exp(x)))
- * out: fp64 [1 or 5, nb]. The batch means and the weighting are left to the host.
+ * out: fp64 [1 or 5, nb]. The batch means and the weighting are left to the host. A NaN element makes its sample's sum
+ * NaN, as in the reference: the clamp of kind 2 and the relu of kind 3 keep a NaN (torch.clamp, F.relu).
  */
 int sdb_ae_loss_terms(const float* a, const float* bb, int32_t kind, int32_t nb, int64_t n, int32_t cc, double* out,
                       sdb_stream_t stream);

@@ -183,6 +183,9 @@ __global__ void im2col_kernel(const __half* __restrict__ x, int nb, int h, int w
 }
 
 __device__ __forceinline__ float softplus_(float x) { return x > 20.f ? x : log1pf(expf(x)); }
+// torch.clamp and F.relu keep a NaN; fminf / fmaxf would replace it with the other operand
+__device__ __forceinline__ float clamp_nan(float x, float lo, float hi) { return x < lo ? lo : (x > hi ? hi : x); }
+__device__ __forceinline__ float relu_nan(float x) { return x < 0.f ? 0.f : x; }
 
 // ae_loss_terms: one CTA per sample (the terms are small next to the convs); thread j sums elements j, j + 256, ... in
 // fp64, then a fixed shuffle tree per warp and the eight warp sums in order, as sdb_diffusion_loss does
@@ -204,13 +207,13 @@ __global__ void __launch_bounds__(kAeThreads) ae_terms_kernel(const float* __res
       const size_t pix = static_cast<size_t>(b) * (n / cc) + i / cc;
       const int ch = static_cast<int>(i % cc);
       const float m = a[pix * 2 * cc + ch];
-      const float lv = fminf(fmaxf(a[pix * 2 * cc + cc + ch], -30.f), 20.f);
+      const float lv = clamp_nan(a[pix * 2 * cc + cc + ch], -30.f, 20.f);
       acc[0] += static_cast<double>(__fsub_rn(__fsub_rn(__fadd_rn(__fmul_rn(m, m), expf(lv)), 1.f), lv));
     } else {
       const float l = a[(static_cast<size_t>(b) * n + i) * cc];
       acc[0] += static_cast<double>(l);
-      acc[1] += static_cast<double>(fmaxf(__fsub_rn(1.f, l), 0.f));
-      acc[2] += static_cast<double>(fmaxf(__fadd_rn(1.f, l), 0.f));
+      acc[1] += static_cast<double>(relu_nan(__fsub_rn(1.f, l)));
+      acc[2] += static_cast<double>(relu_nan(__fadd_rn(1.f, l)));
       acc[3] += static_cast<double>(softplus_(-l));
       acc[4] += static_cast<double>(softplus_(l));
     }

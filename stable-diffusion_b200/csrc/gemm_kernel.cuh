@@ -121,10 +121,11 @@ __device__ __forceinline__ float apply_act(float x, int act) {
   return x;
 }
 // The activation of an epilogue of kind KIND: kind 4 carries only the ReLU family (SDB_ACT_RELU, SDB_ACT_LEAKY_RELU),
-// so the other kinds compile exactly the code they had before it existed.
+// so the other kinds compile exactly the code they had before it existed. Both keep a NaN (and -0), as torch.relu and
+// F.leaky_relu do: fmaxf(x, 0) would turn a NaN into 0.
 template <int KIND>
 __device__ __forceinline__ float epi_act(float x, int act) {
-  if (KIND == 4) return act == SDB_ACT_RELU ? fmaxf(x, 0.0f) : (x > 0.0f ? x : 0.2f * x);
+  if (KIND == 4) return act == SDB_ACT_RELU ? (x < 0.0f ? 0.0f : x) : (x > 0.0f ? x : 0.2f * x);
   return apply_act(x, act);
 }
 

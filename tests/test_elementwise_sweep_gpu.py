@@ -1178,6 +1178,14 @@ ENTRY_POINT_TESTS = {
     "sdb_watermark_dwtdct": ("test_safety_gpu.py",),
     "sdb_fill_f32": ("test_handle_gpu.py",),
     "sdb_sample_plms": ("test_handle_gpu.py",),
+    # evaluation (include/sdb200_eval.h, include/sdb200_ae_loss.h)
+    "sdb_q_sample_t": ("test_losses_gpu.py",),
+    "sdb_diffusion_loss": ("test_losses_gpu.py",),
+    "sdb_lpips_scale": ("test_ae_loss_sweep_gpu.py", "test_ae_loss_gpu.py"),
+    "sdb_maxpool2x2": ("test_ae_loss_sweep_gpu.py", "test_ae_loss_gpu.py"),
+    "sdb_lpips_head": ("test_ae_loss_sweep_gpu.py", "test_ae_loss_gpu.py"),
+    "sdb_im2col": ("test_ae_loss_sweep_gpu.py", "test_ae_loss_gpu.py"),
+    "sdb_ae_loss_terms": ("test_ae_loss_sweep_gpu.py", "test_ae_loss_gpu.py"),
 }
 # entry points whose Python caller is not ops.<name without sdb_>: the call a test file makes to reach them
 CALLED_AS = {
@@ -1194,7 +1202,8 @@ CALLED_AS = {
 }
 HOST_ONLY = ("sdb_last_error", "sdb_version", "sdb_sm_count", "sdb_launch_count", "sdb_debug_trace", "sdb_knn_workspace",
              "sdb_gemm_plan", "sdb_plan_begin", "sdb_plan_end", "sdb_plan_size", "sdb_plan_run", "sdb_plan_launch",
-             "sdb_plan_destroy", "sdb_unet_create", "sdb_unet_forward", "sdb_unet_destroy")
+             "sdb_plan_destroy", "sdb_unet_create", "sdb_unet_forward", "sdb_unet_destroy", "sdb_lpips_head_work")
+ALL_SIGNATURES = {**_l.SIGNATURES, **_l.EVAL_SIGNATURES, **_l.AE_LOSS_SIGNATURES}
 
 
 def _calls(src, sym):
@@ -1205,9 +1214,9 @@ def _calls(src, sym):
 
 def test_every_entry_point_maps_to_its_tests():
     assert set(ENTRY_POINT_TESTS).isdisjoint(HOST_ONLY)
-    assert set(ENTRY_POINT_TESTS) | set(HOST_ONLY) == set(_l.SIGNATURES), (
-        "unmapped: " + str(sorted(set(_l.SIGNATURES) - set(ENTRY_POINT_TESTS) - set(HOST_ONLY)))
-        + ", not in SIGNATURES: " + str(sorted((set(ENTRY_POINT_TESTS) | set(HOST_ONLY)) - set(_l.SIGNATURES))))
+    assert set(ENTRY_POINT_TESTS) | set(HOST_ONLY) == set(ALL_SIGNATURES), (
+        "unmapped: " + str(sorted(set(ALL_SIGNATURES) - set(ENTRY_POINT_TESTS) - set(HOST_ONLY)))
+        + ", in no signature table: " + str(sorted((set(ENTRY_POINT_TESTS) | set(HOST_ONLY)) - set(ALL_SIGNATURES))))
     here = os.path.dirname(os.path.abspath(__file__))
     missing, silent = [], []
     for sym, files in ENTRY_POINT_TESTS.items():

@@ -21,6 +21,8 @@ Bounds (calibrated on the default plans; the largest observed ratio is printed p
                    concats (K = 9 x 2560 = 23040) reach 1.5e-5, default plans included
   fp16 output      |out - ref| <= ulp16(ref) + TAU * absref
   SILU/QUICK_GELU/GELU  |out - ref| <= 1.2 TAU * absref + ACT_REL * |v| (+ one fp16 ulp for fp16 outputs)
+  RELU / LEAKY_RELU     |out - ref| <= TAU * absref (+ LRELU_ULPS u |v| for the fp32 slope 0.2f x): both are
+                        1-Lipschitz; they run in epilogue kind 4, which never splits K
   GEGLU            |out - ref| <= ulp16 + TAU (|gelu(g)| absref_x + 1.2 |x| absref_g) + ACT_REL |x| (|g| + 1)
   hi/lo            hi == fp16(f32); |hi + lo - f32| <= 2e-6 |f32| + 6e-8
   statistics       every slot finite, T as sdb_gemm_plan reports it, and the slots summed over T within 1e-5 of the
@@ -38,13 +40,15 @@ import helpers  # noqa: F401  (puts the repository on sys.path)
 from helpers import rel_l2
 from sdb200 import arch, ops
 from sdb200 import lib as _l
-from sdb200.lib import ACT_GEGLU, ACT_GELU, ACT_NONE, ACT_QUICK_GELU, ACT_SILU
+from sdb200.lib import ACT_GEGLU, ACT_GELU, ACT_LEAKY_RELU, ACT_NONE, ACT_QUICK_GELU, ACT_RELU, ACT_SILU
 from sweeps import NAN, Tally, check_coverage, eoff, record, ulp16
 from workloads import GEMM_WORKLOADS, _unet
 
 TAU = 1e-5        # elementwise bound of the fp32 accumulation, relative to the abs-value reference
 REL_L2 = 1e-5     # rel-L2 of fp32 outputs for K <= 4608, growing as sqrt(K) beyond (one 64-deep wgmma K step after another)
 ACT_REL = 4e-6    # __expf / rcp.approx / erf polynomial inside the epilogue activations, relative to |v|
+LRELU_ULPS = 4 * 2.0 ** -24   # LeakyReLU's 0.2f * x: 0.2f is 0.2 (1 + 1.5e-8), and the product rounds once
+RELU_FAMILY = (ACT_RELU, ACT_LEAKY_RELU)
 BNS = (32, 64, 128, 160, 256)
 MODES = [(1, 0), (2, 2), (4, 2)] + [(s, 1) for s in (2, 3, 4, 6, 8, 12, 16, 24, 32)]
 
@@ -119,6 +123,12 @@ def act_ref(v, av, act, bn):
         return v * torch.sigmoid(s * v), 1.2 * TAU * av + ACT_REL * v.abs()
     if act == ACT_GELU:     # exact GELU; its slope is within [-0.17, 1.13], bound as SILU's
         return _gelu64(v), 1.2 * TAU * av + ACT_REL * v.abs()
+    if act == ACT_RELU:
+        return torch.where(v < 0, torch.zeros_like(v), v), TAU * av
+    if act == ACT_LEAKY_RELU:
+        return torch.where(v > 0, v, 0.2 * v), TAU * av + LRELU_ULPS * v.abs()
+    if act != ACT_GEGLU:
+        raise ValueError(f"act_ref: no reference for activation {act}")
     M, n = v.shape      # GEGLU: each accumulator tile of bn columns is [bn/2 values | bn/2 gates]
     vv, aa = v.view(M, n // bn, 2, bn // 2), av.view(M, n // bn, 2, bn // 2)
     x, g, ax, ag = vv[:, :, 0], vv[:, :, 1], aa[:, :, 0], aa[:, :, 1]
@@ -174,7 +184,7 @@ def label(p):
     if p["rps"]:
         bits.append(f"rps={p['rps']}")
     if p["act"]:
-        bits.append({1: "geglu", 2: "qgelu", 3: "silu", 4: "gelu"}[p["act"]])
+        bits.append({1: "geglu", 2: "qgelu", 3: "silu", 4: "gelu", 6: "relu", 7: "lrelu"}[p["act"]])
     if p["alpha"] != 1.0:
         bits.append(f"alpha={p['alpha']:g}")
     bits.append("out=" + "".join(k for k in ("f16", "f32", "lo") if p[k]))
@@ -295,6 +305,23 @@ def explicit_plans(d, geglu_bn):
     return out
 
 
+def split_requests_not_unsplit(d):
+    """The split-K requests (splits -1, 2, 8; workspace or cluster mode) of a ReLU-family problem that sdb_gemm_plan
+    does not resolve to one split, with the plan it chose: kind 4 has no split-K second pass and no cluster split-K."""
+    bad = []
+    dd = _copy(d)
+    dd.workspace = ops.splitk_workspace(torch.device("cuda", torch.cuda.current_device())).data_ptr()
+    dd.workspace_floats = ops.WS_FLOATS
+    dd.block_n, dd.pair = 0, 0
+    for sp in (-1, 2, 8):
+        for mode in (0, 2):
+            dd.splits, dd.splitk_mode = sp, mode
+            pl = _plan(dd)
+            if pl is None or pl[2:4] != (1, 0):
+                bad.append(((sp, mode), pl))
+    return bad
+
+
 def tuner_view(d, p, stats_ok):
     """The descriptor gemm() hands to the autotuner for this request: nothing explicit, statistics placeholder."""
     dd = _copy(d)
@@ -336,7 +363,7 @@ def classify(d, plan, sms):
     film_table = 0
     if d.film:
         film_table = int(rps % 64 == 0) if d.taps == 1 else int(tw * th >= 64 and rps == d.h * d.w)
-    kind = 2
+    kind = 4 if d.act in RELU_FAMILY else 2      # the ReLU family never splits K (no cluster split-K: kind 3)
     if fast and geglu and not d.out_f32 and not d.out_f16_lo and not ws:
         kind = 1
     elif fast and d.act == ACT_NONE and (not d.film or film_table) and not (d.out_f32 and d.out_f16 and d.out_f16_lo):
@@ -366,7 +393,7 @@ def classify(d, plan, sms):
     return cls
 
 
-REQUIRED = ({f"kind{k}" for k in range(4)} | {"fast", "scalar", "film_table0", "film_table1", "splitk<10>", "splitk<40>",
+REQUIRED = ({f"kind{k}" for k in range(5)} | {"fast", "scalar", "film_table0", "film_table1", "splitk<10>", "splitk<40>",
             "splitk<32>", "splitk_scalar", "cg1", "cg2", "cluster2", "cluster4", "stride2_shift0", "stride2_shift1",
             "nsrc1", "nsrc2", "nsrc3", "nsrc4", "tail32", "TN>1"})
 COVER = defaultdict(int)
@@ -469,6 +496,12 @@ def sweep_problem(X, failures, calib, sms, ws, arena):
     stats_ok = (p["stats"] and p["f32"] and not geglu and (p["taps"] == 9 or p["rps"]) and M % rps == 0
                 and p["n"] % p["sg"] == 0)
     plans = [None] + [pl for pl in explicit_plans(d, geglu_bn) if pl != default]
+    if p["act"] in RELU_FAMILY:
+        for req, pl in split_requests_not_unsplit(d):
+            failures.append((lab, f"request splits/mode {req}", "ReLU family split", str(pl)))
+        for pl in [default] + plans[1:]:
+            if pl[2] > 1:
+                failures.append((lab, str(pl), "ReLU family split", "explicit plan accepted"))
     tunable = p["block_n"] == 0 and p["pair"] == 0 and p["splitk_mode"] == 0 and p["splits"] in (0, -1) and not geglu
     cands = []
     if tunable:
@@ -579,6 +612,20 @@ SYNTHETIC = {
     "silu_conv_split": _synthetic(geo=(2, 8, 8), taps=9, chans=(640,), n=640, act=ACT_SILU, f16=True),
     "hilo_film_rows": _synthetic(geo=(2 * 80,), chans=(320, 320, 320), hilo=True, n=320, film=(960, 320, 2), rps=80,
                                  res=True, f16=True, lo=True),
+    # epilogue kind 4 (ReLU / LeakyReLU): TMA-store and scalar stores, each output set, FiLM per row and as a column
+    # table, residual, statistics and a stride-2 conv; every split-K request resolves to one split
+    "relu_conv_f16": _synthetic(geo=(2, 16, 16), taps=9, chans=(128,), n=128, act=ACT_RELU, f16=True, f32=False),
+    "lrelu_scalar_n36": _synthetic(n=36, act=ACT_LEAKY_RELU, res=True),
+    "relu_f16_f32_lo": _synthetic(geo=(512,), chans=(256,), n=256, act=ACT_RELU, f16=True, lo=True),
+    "lrelu_film_rows": _synthetic(geo=(2 * 80,), chans=(320,), n=320, act=ACT_LEAKY_RELU, film=(640, 320, 2), rps=80,
+                                  res=True),
+    "relu_film_table": _synthetic(geo=(2 * 128,), chans=(512,), n=256, act=ACT_RELU, film=(256, 0, 2), rps=128,
+                                  res=True, f16=True),
+    "lrelu_conv_stats": _synthetic(geo=(2, 16, 16), taps=9, chans=(64,), n=128, act=ACT_LEAKY_RELU, res=True, stats=True,
+                                   sg=4),
+    "relu_conv_s2": _synthetic(geo=(2, 32, 32), taps=9, chans=(64,), conv_stride=2, n=128, act=ACT_RELU, f16=True),
+    "lrelu_conv_s2_shift": _synthetic(geo=(2, 16, 24), taps=9, chans=(128,), conv_stride=2, conv_shift=1, n=64,
+                                      act=ACT_LEAKY_RELU, f16=True, f32=False),
 }
 
 
@@ -801,6 +848,22 @@ def test_reference_epilogue_cpu():
     assert torch.allclose(out[:, 64:], v[:, 128:192] * _gelu64(v[:, 192:]), rtol=1e-12)
     assert float(ulp16(torch.tensor([1.0, 1.5, 2.0, 1e-6]))[0]) == 2.0 ** -10
     assert float(ulp16(torch.tensor([1e-6]))[0]) == 2.0 ** -24
+
+
+def test_relu_family_reference_cpu():
+    """ReLU and LeakyReLU(0.2) in fp64 with the accumulation bound alone (plus the slope's ulps for LeakyReLU); an
+    activation without a reference raises instead of being checked against another one."""
+    v = torch.tensor([[-2.0, -0.5, 0.0, 3.0]], dtype=torch.float64)
+    av = v.abs() + 1.0
+    out, bound = act_ref(v, av, ACT_RELU, 128)
+    assert out.tolist() == [[0.0, 0.0, 0.0, 3.0]] and torch.equal(bound, TAU * av)
+    out, bound = act_ref(v, av, ACT_LEAKY_RELU, 128)
+    assert torch.allclose(out, torch.tensor([[-0.4, -0.1, 0.0, 3.0]], dtype=torch.float64), rtol=1e-15)
+    assert torch.equal(bound, TAU * av + LRELU_ULPS * v.abs())
+    for bad in (5, 8):
+        with pytest.raises(ValueError):
+            act_ref(v, av, bad, 128)
+    assert " relu " in label(_synthetic(act=ACT_RELU)) and " lrelu " in label(_synthetic(act=ACT_LEAKY_RELU))
 
 
 def test_signature_dedups_and_keeps_layouts_cpu():

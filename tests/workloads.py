@@ -303,3 +303,51 @@ def _wl_first_stage(cfg, dev):
 
 FIRST_STAGE_WORKLOADS = {name: (lambda cfg: lambda dev: _wl_first_stage(cfg, dev))(cfg)
                          for name, cfg in arch.FIRST_STAGES.items()}
+
+
+# test_ae_loss_sweep_gpu.py: the KL autoencoders' validation loss (seeded LPIPSWithDiscriminator weights), kept out of
+# the tables above for the same reason
+AE_DISC_START = 50
+
+
+def _wl_ae_loss(dev, nb, h, w):
+    """Both LPIPSWithDiscriminator calls (optimizer_idx 0: rec / LPIPS / KL / g_loss; 1: the hinge discriminator loss)
+    on each side of disc_start, for an nb x h x w image pair and a KL-f8 posterior with logvar drawn across both clamps."""
+    import sdb200
+    from sdb200 import ae_loss
+    from sdb200.vae import DiagonalGaussianDistribution
+    m = sdb200.LPIPSWithDiscriminator(disc_start=AE_DISC_START, kl_weight=1e-6, disc_weight=0.5)
+    m.load_state_dict(ae_loss.random_loss_state_dict(ae_loss.loss_param_shapes(), 21))
+    m = m.to(dev).eval()
+    g = torch.Generator(device=dev).manual_seed(10)
+    x = torch.rand(nb, 3, h, w, generator=g, device=dev) * 2 - 1
+    xr = (x + 0.2 * torch.randn(nb, 3, h, w, generator=g, device=dev)).clamp(-1, 1)
+    zh, zw = h // 8, w // 8
+    mom = torch.randn(nb * zh * zw, 8, generator=g, device=dev)
+    mom[:, 4:] *= 25
+    post = DiagonalGaussianDistribution(mom, nb, zh, zw, 4)
+    outs = []
+    for idx in (0, 1):
+        for gs in (AE_DISC_START - 1, AE_DISC_START):
+            loss, log = m(x, xr, post, idx, gs, split="val")
+            outs += [loss] + [log[k] for k in sorted(log)]
+    return outs
+
+
+def _wl_lpips_min_side(dev):
+    """LPIPS at the smallest side it takes (four 2x2 pools leave one pixel): 16² at batch 3 and 16x24 at batch 1."""
+    import sdb200
+    from sdb200 import ae_loss
+    lp = sdb200.LPIPS().load_weights(ae_loss.random_loss_state_dict(ae_loss.lpips_param_shapes(), 22), dev)
+    g = torch.Generator(device=dev).manual_seed(11)
+    s = ae_loss.LPIPS_MIN_SIDE
+    return [lp(torch.rand(nb, 3, s, w, generator=g, device=dev) * 2 - 1, torch.rand(nb, 3, s, w, generator=g,
+                                                                                    device=dev) * 2 - 1)
+            for nb, w in ((3, s), (1, s + 8))]
+
+
+AE_LOSS_WORKLOADS = {
+    "ae_loss_256": lambda dev: _wl_ae_loss(dev, 4, 256, 256),        # scripts/eval_autoencoder.py's default batch
+    "ae_loss_72x104": lambda dev: _wl_ae_loss(dev, 2, 72, 104),      # pools 9 x 13 -> 4 x 6: odd row and column dropped
+    "lpips_min_side": _wl_lpips_min_side,
+}
